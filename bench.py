@@ -12,9 +12,16 @@ Printed JSON (rank 0, one line):
   value  images/s with the batch already resident in HBM (CUDA events, max over ranks);
   e2e    same step through the public API from pinned HOST buffers: per step an H2D copy of images+labels and a D2H read
          of the loss inside the timed region;
-  roofline  the dominant kernel (tcgen05 implicit-GEMM conv, fwd+dgrad launches): algorithmic FLOP / CUDA-event time of
-            every launch of it inside the timed region, against the measured tensor peak;
+  roofline  the dominant kernel (wgmma implicit-GEMM conv, fwd+dgrad launches): algorithmic FLOP / CUDA-event time of
+            every launch of it inside the timed region, against the tensor peak;
   cpu_baseline  oracle/port.py (CPU restatement pinned to the reference) on a bounded sample, N=1 rank 0 only.
+
+--dump-outputs DIR writes, after the timed steps, what the last timed step computed (rank 0) as DIR/<name>.npy: the step's losses
+(float64), the student's and the teacher's main logits, and a fixed seeded sample of the updated student and discriminator
+parameters (float32).  Inputs and initial weights are seeded, so two builds run with the same arguments can be compared output for
+output.  Every reduction on the timed path adds in a fixed order, so a build reproduces its own dump bit for bit; between two builds
+that sum in different orders, the random-init training amplifies last-bit differences from step to step, so compare those with
+few steps (--steps 1).
 """
 import argparse
 import json
@@ -52,7 +59,7 @@ def _peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return dict(hbm=d["hbm_gbs"], bf16=d["bf16_tflops"], bf16_sus=d.get("bf16_tflops_sustained", d["bf16_tflops"]), src="measured")
-    return dict(hbm=6650.0, bf16=1590.0, bf16_sus=1400.0, src="fallback")
+    return dict(hbm=3350.0, bf16=989.0, bf16_sus=989.0, src="H100 SXM data sheet")
 
 
 class ClockSampler:
@@ -100,8 +107,8 @@ def synthetic(batch, seed):
 
 # ------------------------------------------------------------------------------------------------------------------
 def run_reference(args, rank, world):
-    """The reference's own algorithm (oracle/port.py: CPU restatement pinned against /root/reference by golden fixtures;
-    /root/reference itself does not exist on the GPU box) on all host threads.  Bounded sample: batch 1 per step."""
+    """The reference's own algorithm (oracle/port.py: CPU restatement pinned against the unmodified reference by golden fixtures,
+    so the reference tree itself is not needed here) on all host threads.  Bounded sample: batch 1 per step."""
     if rank != 0:
         return
     import torch
@@ -200,7 +207,7 @@ def cpu_baseline_leg(timed=3):
 
 def torch_cuda_eager_context(batch=4, steps=5):
     """Context only (not the contract's reference arm): the same restatement with its torch ops on cuda:0 -- cuDNN / cuBLAS eager, TF32
-    allowed (torch's default), i.e. what the reference's stock code path costs on this B200.  Batch 4 bounds its memory."""
+    allowed (torch's default), i.e. what the reference's stock code path costs on this GPU.  Batch 4 bounds its memory."""
     import torch
     from oracle import cases, port
     try:
@@ -230,6 +237,32 @@ def torch_cuda_eager_context(batch=4, steps=5):
         return out
     except Exception as ex:                                                # noqa: BLE001
         return {"error": repr(ex)[:200]}
+
+
+DUMP_PARAM_SAMPLE = 1 << 20          # parameters per model kept by --dump-outputs (a fixed, seeded sample; 64 MB cap on the whole dump)
+
+
+def dump_outputs(model, out_dir):
+    """The arrays a caller of NetModel.optimize_parameters() receives from one step: losses, logits, updated parameters."""
+    import numpy as np
+    import torch
+    torch.cuda.synchronize()
+    os.makedirs(out_dir, exist_ok=True)
+    names = ["mc_G_loss", "pi_G_loss", "pa_G_loss", "G_loss", "D_loss"]
+    arrays = {"losses": np.array([float(getattr(model, n)) for n in names], dtype=np.float64),
+              "student_logits": model.preds_S[0].detach().float().cpu().numpy(),
+              "teacher_logits": model.preds_T[0].detach().float().cpu().numpy()}
+    for key, solver in (("student_params", model.G_solver), ("discriminator_params", model.D_solver)):
+        flat = solver.flat_p.detach()
+        if flat.numel() > DUMP_PARAM_SAMPLE:
+            g = torch.Generator().manual_seed(0)
+            idx = torch.randperm(flat.numel(), generator=g)[:DUMP_PARAM_SAMPLE].sort().values
+            flat = flat[idx.to(flat.device)]
+        arrays[key + "_sample" if flat.numel() < solver.flat_p.numel() else key] = flat.float().cpu().numpy()
+    total = sum(a.nbytes for a in arrays.values())
+    assert total <= 64 << 20, total
+    for k, a in arrays.items():
+        np.save(os.path.join(out_dir, k + ".npy"), a)
 
 
 # ------------------------------------------------------------------------------------------------------------------
@@ -312,15 +345,17 @@ def run_ours(args, rank, local_rank, world):
         clocks.start()
     ms = timed(args.steps, step_resident)
     clk = clocks.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(model, args.dump_outputs)
     ms_e2e = timed(args.steps, step_e2e)
     launches = launches_per_step * args.steps
 
-    # roofline pass: the same steps executed eagerly with a CUDA-event pair around every tcgen05 conv launch
+    # roofline pass: the same steps executed eagerly with a CUDA-event pair around every wgmma conv launch
     # (events recorded inside a captured graph cannot be timed)
     conv_log = []
     model._graphs = None
     model.overlap_streams = False                                  # one stream: an event pair must bracket ONE kernel, not its neighbours on other streams
-    ops.CONV_EVENT_LOG = conv_log                                  # ops.conv2d_fwd records (start, end, flops) per tcgen05 launch
+    ops.CONV_EVENT_LOG = conv_log                                  # ops.conv2d_fwd records (start, end, flops) per wgmma launch
     ms_eager = timed(args.steps, step_resident)
     ops.CONV_EVENT_LOG = None
 
@@ -333,10 +368,10 @@ def run_ours(args, rank, local_rank, world):
             dist.destroy_process_group()
         return
     peaks = _peaks()
-    tf32_peak = peaks["bf16_sus"] / 2.0                            # kind::tf32 issues at half the bf16 rate
+    tf32_peak = peaks["bf16_sus"] / 2.0                            # wgmma tf32 issues at half the bf16 rate
     wg_log = [r for r in conv_log if r[3][0] == "wgrad"]
     all_log = conv_log
-    conv_log = [r for r in conv_log if r[3][0] in ("fwd", "dgrad", "fwd3x")]         # the dominant kernel: conv_fwd_sm100_kernel (fwd + dgrad)
+    conv_log = [r for r in conv_log if r[3][0] in ("fwd", "dgrad", "fwd3x")]         # the dominant kernel: conv_fwd_sm90_kernel (fwd + dgrad)
     conv_ms = sum(r[0].elapsed_time(r[1]) for r in conv_log)
     conv_flop = sum(r[2] for r in conv_log)
     wg_ms = sum(r[0].elapsed_time(r[1]) for r in wg_log)
@@ -349,12 +384,6 @@ def run_ours(args, rank, local_rank, world):
         for k, v in sorted(agg.items(), key=lambda kv: -kv[1][1])[:40]:
             print("CONV %-48s n=%3d  %7.3f ms/step  %6.0f TF" % (k, v[0] // args.steps, v[1] / args.steps, v[2] / max(v[1], 1e-9) / 1e9), file=sys.stderr)
     achieved = conv_flop / (conv_ms * 1e-3) / 1e12 if conv_ms > 0 else 0.0
-    # DRAM traffic cannot be measured outside a profiler: `traffic` stays null here; the ncu capture of one representative launch
-    # (committed under profiles/) is quoted separately with its own algorithmic bytes
-    traffic_ncu = None
-    tp = os.path.join(ROOT, "profiles", "conv_fwd_traffic.json")
-    if os.path.exists(tp):
-        traffic_ncu = json.load(open(tp))
     # whole step: algorithmic conv FLOP of one image (SURVEY.md §8d, hooks on the reference model) x batch, over the TIMED (graph) step
     step_flop = (FLOP_T + FLOP_S + 2 * FLOP_S - FLOP_STEM1) * BATCH_PER_GPU
     out = {
@@ -363,18 +392,17 @@ def run_ours(args, rank, local_rank, world):
         "data": "synthetic",
         "config": {"workload": WORKLOAD,
                    "global_batch": BATCH_PER_GPU * world, "parallelism": "dp%d" % world, "gradient_exchange": (args.allreduce if world > 1 else "none"),
-                   "precision": "fp32 storage; TF32 tensor-core operands (round-to-nearest by TMA), fp32 accumulate; student stem+layer1 forward in split-precision 3xTF32",
+                   "precision": "fp32 storage; TF32 tensor-core operands (round-to-nearest by TMA), fp32 accumulate; student stem, layer1 and layer2 forward in split-precision 3xTF32",
                    "cuda_graph": bool(use_graph), "launch_count_note": "gpu_launches = our kernels counted on an eager step x steps (graph replays re-issue the same launches)",
-                   "l2": "per-step working set (activations ~10 GB) is far larger than the 126 MB L2: no flush needed"},
+                   "l2": "per-step working set (activations ~10 GB) is far larger than the 50 MB L2: no flush needed"},
         "e2e": {"value": e2e, "unit": "images/s", "h2d_bytes_per_step": pin_i.numel() * 4 + pin_l.numel() * 8, "d2h_bytes_per_step": 4,
                 "ms_per_step": ms_e2e / args.steps},
         "gpu_launches": int(launches),
         "clocks": clk,
-        "roofline": {"bound": "tensor", "kernel": "conv_fwd_sm100_kernel (tcgen05 implicit GEMM: teacher fwd, student fwd, student dgrad)",
+        "roofline": {"bound": "tensor", "kernel": "conv_fwd_sm90_kernel (wgmma implicit GEMM: teacher fwd, student fwd, student dgrad)",
                      "achieved": achieved, "peak": tf32_peak, "unit": "TFLOP/s", "frac": achieved / tf32_peak if tf32_peak else None,
                      "flop_counting": "algorithmic 2*N*OH*OW*Cout*Cin*KH*KW per launch; split-precision (3xTF32) launches are counted ONCE",
-                     "peak_source": "%s bf16 sustained cuBLAS peak / 2 (TF32 operands)" % peaks["src"], "traffic": None,
-                     "traffic_ncu": traffic_ncu,
+                     "peak_source": "%s bf16 peak / 2 (TF32 operands)" % peaks["src"], "traffic": None,
                      "launches_timed": len(conv_log), "share_of_eager_step": conv_ms / ms_eager if ms_eager else None,
                      "wgrad_kernel": {"achieved": wg_flop / (wg_ms * 1e-3) / 1e12 if wg_ms > 0 else None,
                                       "frac": (wg_flop / (wg_ms * 1e-3) / 1e12) / tf32_peak if wg_ms > 0 and tf32_peak else None,
@@ -413,6 +441,8 @@ def main():
     ap.add_argument("--allreduce", default="nccl", choices=["nccl", "nvls"],
                     help="N > 1: nccl = bucketed ncclAllReduce inside the backward pass; nvls = reduction fused into the SGD kernel over NVSwitch multicast")
     ap.add_argument("--allreduce-buckets", type=int, default=4, help="N > 1: ranges of the flat student gradient all-reduced from inside the backward pass (0: one all-reduce after it)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last step's losses, logits and a parameter sample to DIR/<name>.npy")
     ap.add_argument("--config", type=int, default=3, choices=[3, 4], help="3: BASELINE.json configs[2] (the metric's configuration); 4: the 360x480 batch-16 shape of configs[3]")
     args = ap.parse_args()
     select_config(args.config)

@@ -1,4 +1,4 @@
-/* libskd_b200.so -- C ABI of the Blackwell-native structured-distillation step.
+/* libskd_b200.so -- C ABI of the Hopper-native (sm_90a) structured-distillation step.
  *
  * Drop-in boundary for the hot path of irfanICMLL/structure_knowledge_distillation (NetModel.optimize_parameters,
  * networks/kd_model.py:167-173).  Conventions are the reference's own native-ABI conventions
@@ -46,7 +46,7 @@ int skd_elu_cuda(int N, float* x, cudaStream_t);
 int skd_elu_backward_cuda(int N, const float* x, float* dx, cudaStream_t);
 int skd_elu_inv_cuda(int N, float* x, cudaStream_t);
 
-/* ---- B. fused NHWC ABN used between the tcgen05 convolutions (same math: libs/functions.py:81-109,113-162) ---- */
+/* ---- B. fused NHWC ABN used between the wgmma convolutions (same math: libs/functions.py:81-109,113-162) ---- */
 int skd_abn_num_splits(long long P, int C);   /* workspace = splits*C*2 floats */
 /* batch stats of x[P][C] -> mean,var (biased); running EMA with n/(n-1) (functions.py:90-91); scale=(|w|+eps)*rsqrt(var+eps),
    shift=b-mean*scale for the apply pass */
@@ -57,7 +57,7 @@ int skd_abn_stats_nhwc(long long P, int C, const float* x, const float* weight, 
 int skd_abn_fold(int C, const float* mean, const float* var, const float* weight, const float* bias, float eps, float* scale,
                  float* shift, cudaStream_t);
 /* out = act(x*scale+shift (+residual)) (*chan_mul[n][c] : Dropout2d mask, S = rows per image); out_pitch in floats;
-   round_tf32: store RNA-rounded TF32 values (the tensor feeds a tensor-core convolution) */
+   round_tf32: store TF32 values rounded to nearest even (the tensor feeds a tensor-core convolution) */
 int skd_abn_apply_nhwc(long long P, int C, int S, const float* x, float* out, int out_pitch, const float* scale,
                        const float* shift, int act, float slope, const float* residual, const float* chan_mul,
                        int round_tf32, cudaStream_t);
@@ -116,7 +116,7 @@ int skd_pairwise_bwd(int N, int nodes, int CS, const float* E, const float* pool
 /* dF[argmax] = dpooled on a pre-zeroed feature gradient (second half of skd_pairwise_bwd) */
 int skd_pairwise_scatter(int N, int nodes, int CS, const float* dpooled, const int* argmax, float* dF, long long sn, long long sc,
                          long long sp, cudaStream_t);
-/* tcgen05 path for large node counts (pool_scale -> 1/65: 8 385 nodes): E = [fT^|fS^] [fT^|-fS^]^T as one K-major TF32 GEMM per image with
+/* wgmma path for large node counts (pool_scale -> 1/65: 8 385 nodes): E = [fT^|fS^] [fT^|-fS^]^T as one K-major TF32 GEMM per image with
    the L2 reduction fused into the epilogue; E ([N][nodes][ldE], ldE % 4 == 0) may be NULL when no backward follows.  acc: 1 double. */
 long long skd_pairwise_affinity_sm100_workspace_floats(int N, int nodes, int CS, int CT);
 int skd_pairwise_affinity_sm100(int N, int nodes, int CS, int CT, const float* pooled_S, const float* pooled_T, const float* rnorm_S,
@@ -124,21 +124,21 @@ int skd_pairwise_affinity_sm100(int N, int nodes, int CS, int CT, const float* p
 long long skd_pairwise_affinity_bwd_sm100_workspace_floats(int N, int nodes, int CS, int ldE);
 int skd_pairwise_affinity_bwd_sm100(int N, int nodes, int CS, const float* E, int ldE, const float* pooled_S, const float* rnorm_S,
                                     const float* grad_out, float* dpooled, float* workspace, cudaStream_t);
-/* the tcgen05 conv kernel as a plain NT GEMM: D[M][Ncols] = A[M][K] B[Ncols][K]^T (D may be NULL), sumsq += sum D^2 (may be NULL) */
+/* the wgmma conv kernel as a plain NT GEMM: D[M][Ncols] = A[M][K] B[Ncols][K]^T (D may be NULL), sumsq += sum D^2 (may be NULL) */
 int skd_gemm_nt_sm100(int M, int Ncols, int K, const float* A, int lda, const float* B, float* D, int ldd, double* sumsq, cudaStream_t);
 
 /* ---- D. convolutions (every nn.Conv2d of networks/pspnet_combine.py; cuDNN in the reference) ---- */
-/* tcgen05 implicit GEMM: y = act((conv(x,w))*scale + shift + residual); w is [Cout][KH][KW][Cin]; Cin % 4 == 0 */
+/* wgmma implicit GEMM: y = act((conv(x,w))*scale + shift + residual); w is [Cout][KH][KW][Cin]; Cin % 4 == 0 */
 int skd_conv2d_fwd_sm100(int N, int H, int W, int Cin, int Cout, int KH, int KW, int stride, int pad, int dil, const float* x,
                          int ldx, const float* w, float* y, int ldy, const float* scale, const float* shift,
                          const float* residual, int ldr, int act, float slope, int round_tf32, cudaStream_t);
 /* split-precision forward (x = x_hi + x_lo, w = w_hi + w_lo, all four TF32-exact): three accumulation passes in one launch, fp32-grade
-   result; skd_split_tf32 produces the parts (hi = rna_tf32(v), lo = rna_tf32(v - hi)) */
+   result; skd_split_tf32 produces the parts (hi = rn_tf32(v), lo = rn_tf32(v - hi), round-to-nearest-even like the TMA conversion) */
 int skd_conv2d_fwd_sm100_3xtf32(int N, int H, int W, int Cin, int Cout, int KH, int KW, int stride, int pad, int dil, const float* x_hi,
                                 const float* x_lo, int ldx, const float* w_hi, const float* w_lo, float* y, int ldy, const float* scale,
                                 const float* shift, int act, float slope, cudaStream_t);
 int skd_split_tf32(long long n, const float* src, float* hi, float* lo, cudaStream_t);
-/* general form of the tcgen05 forward (discriminator path): optional split-precision operands (x_lo / w_lo both NULL -> plain TF32),
+/* general form of the wgmma forward (discriminator path): optional split-precision operands (x_lo / w_lo both NULL -> plain TF32),
    optional output extent (out_h / out_w > 0: positions past the natural size read zero-filled input), fused scale / shift / residual / act */
 int skd_conv2d_fwd_sm100_ex(int N, int H, int W, int Cin, int Cout, int KH, int KW, int stride, int pad, int dil, const float* x,
                             const float* x_lo, int ldx, const float* w, const float* w_lo, float* y, int ldy, int out_h, int out_w,
@@ -154,20 +154,12 @@ int skd_conv2d_fwd_sm100_splitk(int N, int H, int W, int Cin, int Cout, int KH, 
                                 const float* scale, const float* shift, const float* residual, int ldr, int act, float slope,
                                 float* workspace, long long workspace_floats, cudaStream_t);
 
-/* 3x3 / stride 1 / pad 1 convolution for Cin, Cout <= 128 (Cin a multiple of 32): the input halo tile of a 16 x 8 pixel output tile is
-   loaded once per 32-channel chunk and the nine taps read it through shifted shared-memory descriptors -- the general kernel moves
-   every activation line L2 -> shared memory nine times and is L2-bound at these widths.  skd_conv2d_fwd_sm100 / _3xtf32 / _ex route
-   eligible shapes here by themselves (skd_set_conv_halo(0) turns that off); this entry calls it directly.  x_lo / w_lo as in _ex. */
-void skd_set_conv_halo(int on);   /* bit 0: route eligible shapes to the halo kernel (default 1); bit 2: clusters of 4 with TMA-multicast weights (default off: slower) */
-int skd_conv3x3_halo_sm100(int N, int H, int W, int Cin, int Cout, const float* x, const float* x_lo, int ldx, const float* w,
-                           const float* w_lo, float* y, int ldy, const float* scale, const float* shift, int act, float slope, cudaStream_t);
-
 /* same kernel, output written through explicit element strides y[n*y_img + oy*y_row + ox*y_pix + c] (every-other-pixel sub-grids:
    the data gradient of a stride-2 convolution is 4 stride-1 convolutions of dy, one per input-pixel parity class) */
 int skd_conv2d_fwd_sm100_strided(int N, int H, int W, int Cin, int Cout, int KH, int KW, int stride, int pad, int dil, const float* x,
                                  int ldx, const float* w, float* y, long long y_pix, long long y_row, long long y_img, int out_h, int out_w,
                                  int round_tf32, cudaStream_t);   /* out_h/out_w > 0 override the output extent (far-end zero padding) */
-/* tcgen05 weight gradient: dw[Cout][KH][KW][Cin] = sum_pixels dy[p][co] * x[p+tap][ci]; workspace from the size query */
+/* wgmma weight gradient: dw[Cout][KH][KW][Cin] = sum_pixels dy[p][co] * x[p+tap][ci]; workspace from the size query */
 long long skd_conv2d_wgrad_sm100_workspace_floats(int N, int H, int W, int Cin, int Cout, int KH, int KW, int stride, int pad, int dil);
 int skd_conv2d_wgrad_sm100(int N, int H, int W, int Cin, int Cout, int KH, int KW, int stride, int pad, int dil, const float* x,
                            int ldx, const float* dy, int ldy, float* dw, float* workspace, cudaStream_t);
@@ -188,13 +180,9 @@ int skd_im2col_small(int N, int H, int W, int Cin, int KH, int KW, int stride, i
 int skd_weight_flip_transpose(int Cout, int Cin, int KH, int KW, const float* w, float* wt, int round_tf32, cudaStream_t);
 int skd_round_tf32(long long n, const float* src, float* dst, cudaStream_t);
 void skd_set_tf32_tma_type(int use_tfloat32_type);
-void skd_set_wgrad_linear(int on);     /* 1 (default): wgrad K-blocks are 32 consecutive pixels (im2col TMA); 0: 4x8 rectangles */
-void skd_set_wgrad_cta_pairs(int on);   /* 1 (default): cta_group::2 pairs (256 x 256 tiles) where Cout % 256 == 0 and Cin > 128 */
-void skd_set_conv_res_prefetch(int on); /* 1 (default): residual tiles arrive through a TMA ring in spare pipeline-stage buffers */
+void skd_set_wgrad_linear(int on);     /* 1 (default): wgrad K-blocks are 32 consecutive pixels (im2col TMA); 0: 4x8 pixel rectangles */
 void skd_set_conv_tile_order(int mode); /* 0 (default) front-to-back, 1 back-to-front, 2 alternate per launch (a consumer starts on
                                           the tail its producer left in L2) */
-void skd_set_conv_cta_pairs(int mode); /* 0: single-CTA tiles only; 1 (default): 256 x N tiles on CTA pairs (tcgen05 cta_group::2, half the
-                                          weight tile per CTA) where measured faster; 3: pairs wherever possible (tests) */
 void skd_set_conv_k_order(int mode);   /* K loop of k>1 convolutions: 0 (default) by working set, 1 taps outermost, 2 channel chunks outermost */
 void skd_set_conv_im2col(int on);      /* 1 (default): TMA im2col-mode M tiles for k>1 / strided convs; 0: rectangular tiled-mode tiles */
 
@@ -235,8 +223,7 @@ int skd_sgd_step_nvls(long long lo, long long hi, float* param_mc, const float* 
 int skd_sn_power_iter(int Cout, int taps, int Cin, const float* w_bar, float* u, float* v, float* u_save, float* v_save, float* sigma,
                       float* inv_sigma_vec, int vec_len, cudaStream_t);
 /* The same iteration for several layers in one call (the discriminator's four spectral-norm layers per forward), each phase a
-   grid over all layers and the whole GPU (the single-layer entry keeps a layer on one 8-CTA cluster: 197 us for l4's 512 x 4096
-   matrix; this one ~10 us for all four).  Deterministic (fixed-order partial sums, no atomics).  `layers` is a HOST array. */
+   grid over all layers and the whole GPU (the single-layer entry keeps a layer on one 8-CTA cluster).  Deterministic (fixed-order partial sums, no atomics).  `layers` is a HOST array. */
 typedef struct skd_sn_layer {
   int Cout, taps, Cin, vec_len;
   const float* w_bar; float* u; float* v; float* u_save; float* v_save; float* sigma; float* inv_sigma_vec;
@@ -313,7 +300,7 @@ int skd_eval_argmax_confusion(int H, int W, int C, const float* full, const long
                               int ignore_index, long long* confusion, unsigned char* pred, cudaStream_t);
 
 /* ---- Cityscapes training augmentation on the device (csrc/augment.cu) --------------------------------------------------------------
-   Replaces the per-sample CPU work of `CSDataSet.__getitem__` after cv2.imread (/root/reference/dataset/datasets.py:175-206):
+   Replaces the per-sample CPU work of `CSDataSet.__getitem__` after cv2.imread (reference dataset/datasets.py:175-206):
    id -> trainId table (:161-169), `generate_scale_label` = cv2.resize INTER_LINEAR / INTER_NEAREST by f_scale (:155-159), float32 mean
    subtraction (:180-181), padding with 0 / ignore_label (:183-193), crop (:196-200), HWC -> CHW (:202), mirror (:203-206) -- bit-exact
    with opencv's uint8 fixed-point resize.  The host draws the random numbers in the reference's order

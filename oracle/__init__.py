@@ -11,7 +11,7 @@ timed CPU baseline -- never as part of the product path.
 
 Parity pinning: the reference ships no tests / golden vectors (SURVEY.md §4).
 `oracle/port.py` is therefore pinned by differential execution against the
-reference's own Python modules imported from /root/reference
+reference's own Python modules imported from a checkout of it
 (`oracle/refshim.py`, `oracle/make_golden.py`) -- the resulting fixtures are
 committed under `tests/golden/` and re-checked by `tests/test_oracle_golden.py`.
 """

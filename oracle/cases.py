@@ -59,7 +59,7 @@ STEP_CASES = {
 }
 
 # BASELINE.json configs[2] at full size (batch 8 @ 512x1024, Pi+Pa+Ho, wgan-gp): generated once by
-# `python -m oracle.make_golden --full` (several minutes of CPU), checked on the B200 by tests/test_step_gpu.py.
+# `python -m oracle.make_golden --full` (several minutes of CPU), checked on the H100 by tests/test_step_gpu.py.
 FULL_CASES = {
     "baseline_cfg3_b8_512x1024": dict(batch=8, h=512, w=1024, cfg=dict(pi=True, pa=True, ho=True, adv_type="wgan-gp")),
 }
@@ -71,6 +71,30 @@ FULL_CASES = {
 CFG4_CASES = {
     "cfg4_pi_pa_360x480_b2": dict(batch=2, h=360, w=480, cfg=dict(pi=True, pa=True, ho=False, pool_scale=0.5)),
 }
+
+
+def sample_large(t, k=8192, limit=20000):
+    """A stored reference tensor above `limit` elements is kept as a fixed sample of flat positions, {"idx", "val"}, so that
+    every fixture stays below 1 MB; the positions depend only on the element count."""
+    if t.numel() <= limit:
+        return t
+    g = torch.Generator().manual_seed(t.numel())
+    idx = torch.randperm(t.numel(), generator=g)[:k].sort().values
+    return {"idx": idx.to(torch.int32), "val": t.flatten()[idx].clone()}
+
+
+def at_stored(t, stored):
+    """(values of `t`, reference values) at the positions a stored reference tensor keeps (all of them when it is not sampled)."""
+    if isinstance(stored, dict):
+        return t.flatten()[stored["idx"].long().to(t.device)], stored["val"]
+    return t, stored
+
+
+def stored_sum(a, b):
+    """Sum of two stored reference tensors of the same shape (sampled at the same positions)."""
+    if isinstance(a, dict):
+        return {"idx": a["idx"], "val": a["val"] + b["val"]}
+    return a + b
 
 
 def grad_digest(named_params, k=16):

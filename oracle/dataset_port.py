@@ -4,9 +4,9 @@ Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline leg may import 
 (structure_knowledge_distillation_b200/dataset + csrc/augment.cu) never does.
 
 What it restates, and where the arithmetic lives:
-  * `CSDataSet.__getitem__`                 /root/reference/dataset/datasets.py:170-210  (order of operations and of the RNG draws)
-  * `CSDataSet.generate_scale_label`        /root/reference/dataset/datasets.py:155-159  (cv2.resize INTER_LINEAR / INTER_NEAREST)
-  * `CSDataSet.id2trainId`                  /root/reference/dataset/datasets.py:161-169  (a 256-entry look-up table)
+  * `CSDataSet.__getitem__`                 dataset/datasets.py:170-210  (order of operations and of the RNG draws)
+  * `CSDataSet.generate_scale_label`        dataset/datasets.py:155-159  (cv2.resize INTER_LINEAR / INTER_NEAREST)
+  * `CSDataSet.id2trainId`                  dataset/datasets.py:161-169  (a 256-entry look-up table)
   * cv2.resize itself is a THIRD-PARTY dependency (opencv-python, 4.13.0 in this image; the reference pins no version).  Restated
     from OpenCV's published algorithm (modules/imgproc/src/resize.cpp): uint8 INTER_LINEAR = fixed-point separable interpolation,
     coefficients round(w * 2048) as int16, horizontal pass in int32, vertical pass

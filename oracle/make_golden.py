@@ -1,7 +1,7 @@
-"""Generate tests/golden/*.pt by running the UNMODIFIED reference Python (from /root/reference, CPU) on the
+"""Generate tests/golden/*.pt by running the UNMODIFIED reference Python (the checkout named by SKD_REFERENCE_ROOT, CPU) on the
 seeded cases of oracle/cases.py, and pin oracle/port.py against it on the spot.
 
-Run here (build container) only:   python -m oracle.make_golden
+SKD_REFERENCE_ROOT=<reference checkout> python -m oracle.make_golden
 TEST INFRASTRUCTURE ONLY.
 """
 import contextlib
@@ -198,7 +198,8 @@ def main():
     if "--full" in sys.argv:
         torch.save(step_goldens(ref, cases.FULL_CASES, check_port=False), os.path.join(GOLDEN_DIR, "steps_full.pt"))
         return
-    torch.save(dict(criterion=criterion_goldens(ref), adv=adv_goldens(ref)), os.path.join(GOLDEN_DIR, "criteria.pt"))
+    crit = {name: {k: cases.sample_large(v) if torch.is_tensor(v) else v for k, v in g.items()} for name, g in criterion_goldens(ref).items()}
+    torch.save(dict(criterion=crit, adv=adv_goldens(ref)), os.path.join(GOLDEN_DIR, "criteria.pt"))
     torch.save(discriminator_golden(ref), os.path.join(GOLDEN_DIR, "discriminator.pt"))
     torch.save(step_goldens(ref), os.path.join(GOLDEN_DIR, "steps.pt"))
     print("golden fixtures written to", GOLDEN_DIR, "torch", torch.__version__)

@@ -1,6 +1,6 @@
-"""TEST INFRASTRUCTURE -- generates tests/golden/dataset.pt by running the UNMODIFIED reference loader.
+"""TEST INFRASTRUCTURE -- generates tests/golden/dataset.pt.gz by running the UNMODIFIED reference loader.
 
-    python -m oracle.make_golden_dataset        (build container only: needs /root/reference and cv2)
+    SKD_REFERENCE_ROOT=<reference checkout> python -m oracle.make_golden_dataset        (needs cv2)
 
 Writes synthetic Cityscapes-like PNG pairs (uint8 BGR image, uint8 label ids 0..33 plus some 255) to a temporary directory, points the
 reference's `dataset/datasets.py::CSDataSet` (imported as shipped; only `torchvision`, which it imports and never uses, is stubbed when
@@ -8,7 +8,9 @@ absent) at them, seeds `random` / `np.random`, and records for every case: the r
 the (image, label) the reference returned.  oracle/dataset_port.py is then held to these bit for bit (tests/test_dataset_cpu.py), and
 the CUDA kernel to both (tests/test_dataset_gpu.py).
 """
+import gzip
 import importlib.util
+import io
 import os
 import random
 import sys
@@ -20,7 +22,7 @@ import torch
 
 from .refshim import REFERENCE_ROOT
 
-OUT = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests", "golden", "dataset.pt")
+OUT = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests", "golden", "dataset.pt.gz")
 IMG_MEAN = np.array((104.00698793, 116.66876762, 122.67891434), dtype=np.float32)        # train_and_eval.py:10
 
 # (name, raw H, raw W, crop (h, w), scale, mirror, number of draws)
@@ -75,7 +77,9 @@ def main():
             out["cases"].append({"name": name, "raw_image": torch.from_numpy(img), "raw_label": torch.from_numpy(lab), "crop": crop,
                                  "scale": scale, "mirror": mirror, "seed": seed, "items": items, "size": tuple(int(v) for v in size)})
             print(name, "draws", draws, "image", tuple(items[0][0].shape), "label", tuple(items[0][1].shape))
-    torch.save(out, OUT)
+    buf = io.BytesIO(); torch.save(out, buf)
+    with open(OUT, "wb") as f:                                  # gzip: the u8-derived values compress ~3x (fixtures stay < 1 MB)
+        f.write(gzip.compress(buf.getvalue(), 9, mtime=0))
     print("wrote", OUT, os.path.getsize(OUT) // 1024, "KB")
 
 

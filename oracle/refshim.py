@@ -1,8 +1,7 @@
-"""Import the UNMODIFIED reference Python from /root/reference on CPU.
+"""Import the UNMODIFIED reference Python on CPU from the checkout named by SKD_REFERENCE_ROOT.
 
-TEST INFRASTRUCTURE ONLY (see oracle/__init__.py).  This module only works in
-the build container: /root/reference does not exist on the GPU box, so nothing
-that runs there (gpu tests, smoke, bench) may call it.
+TEST INFRASTRUCTURE ONLY (see oracle/__init__.py): used to (re)generate the golden fixtures.  Nothing
+the tests, smoke() or bench.py run may call it -- they compare against the stored fixtures.
 
 Two import shims are needed (SURVEY.md §8c):
   * `tensorboardX`  -- utils/utils.py:10 imports SummaryWriter, never calls it
@@ -17,7 +16,7 @@ import os
 import sys
 import types
 
-REFERENCE_ROOT = os.environ.get("SKD_REFERENCE_ROOT", "/root/reference")
+REFERENCE_ROOT = os.environ.get("SKD_REFERENCE_ROOT", "")
 
 
 def reference_available():

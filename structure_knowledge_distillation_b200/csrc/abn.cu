@@ -1,19 +1,19 @@
-// Fused BatchNorm(+|w|+eps affine)+activation kernels for sm_100a.
+// Fused BatchNorm(+|w|+eps affine)+activation kernels for sm_90a.
 //
 // Part A: drop-in replacements for the reference's only native component, libs/src/bn.cu, behind the very same
 //         raw-pointer C ABI (libs/src/bn.h:7-19): tensors are NCHW viewed as (N, C, S), fp32.
-//         The reference launches ONE block per channel (bn.cu:237-300) -> at C=64 only 64 of 148 SMs work and the
+//         The reference launches ONE block per channel (bn.cu:237-300) -> at C=64 only 64 of 132 SMs work and the
 //         variance costs a second full pass.  Here every channel is reduced by a thread-block CLUSTER whose CTAs
 //         combine their partials through distributed shared memory: no workspace, no atomics, deterministic,
-//         single pass (shifted sums), float4 streaming loads, grid = C x cluster >= 2 waves of 148 SMs.
-// Part B: the NHWC (channels-last) kernels the B200 path itself uses between tcgen05 convolutions:
+//         single pass (shifted sums), float4 streaming loads, grid = C x cluster >= 2 waves of 132 SMs.
+// Part B: the NHWC (channels-last) kernels the H100 path itself uses between wgmma convolutions:
 //         split-row partial statistics -> finalize (+running stats, +folded scale/shift) -> one fused
 //         apply(+activation, +residual add, +Dropout2d channel mask) pass; and the matching backward.
 #include <cooperative_groups.h>
 
 #include "common.cuh"
 #include "skd.h"
-#include "sm100_ptx.cuh"
+#include "sm90_ptx.cuh"
 
 namespace cg = cooperative_groups;
 using namespace skd;
@@ -329,7 +329,7 @@ __global__ void nhwc_stats_finalize_kernel(const float* __restrict__ x, const fl
                                            float* __restrict__ var, float* __restrict__ scale,
                                            float* __restrict__ shift) {
   // one WARP per channel (8 channels per block): the R (~600) split partials of a channel are read by 32 lanes -- ~19 dependent loads
-  // per thread instead of 37 -- and folded with shuffles (ncu, round 2: the 2-block version took 10-12 us per layer, 58 times a step)
+  // per thread instead of 37 -- and folded with shuffles (the 2-block version was latency-bound, 58 times a step)
   const int lane = threadIdx.x & 31;
   const int c = blockIdx.x * 8 + (threadIdx.x >> 5);
   if (c >= C) return;
@@ -477,8 +477,8 @@ __global__ void nhwc_bwd_finalize_kernel(const float2* __restrict__ partial, int
 
 // dx = (dz - edz - y*eydz) * gamma*invstd ; dres = dz
 // The launch makes gridDim.x * blockDim.x a multiple of C4 whenever it can, so a thread meets ONE channel quad in every iteration of its
-// grid-stride loop: the per-channel terms fold once into dx = k1*(dz - edz) - k2*(x - mean) (ncu, round 2: the version that re-derived them per
-// element -- a 64-bit division, five parameter loads, four rsqrt -- was issue-bound at 4.1 TB/s while its sibling passes ran at 5.5).
+// grid-stride loop: the per-channel terms fold once into dx = k1*(dz - edz) - k2*(x - mean) (a version that re-derives them per
+// element -- a 64-bit division, five parameter loads, four rsqrt -- is issue-bound).
 __global__ void __launch_bounds__(256)
 nhwc_bwd_dx_kernel(const float* __restrict__ x, const float* __restrict__ out, const float* __restrict__ dout,
                    float* __restrict__ dx, float* __restrict__ dres, long long total4, int C4, int S,

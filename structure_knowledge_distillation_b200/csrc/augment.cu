@@ -1,5 +1,5 @@
 // Cityscapes training augmentation on the GPU: ONE kernel per batch does what `CSDataSet.__getitem__` does on the CPU after the two
-// cv2.imread calls (/root/reference/dataset/datasets.py:175-206): id -> trainId table, cv2.resize (uint8 INTER_LINEAR for the image,
+// cv2.imread calls (reference dataset/datasets.py:175-206): id -> trainId table, cv2.resize (uint8 INTER_LINEAR for the image,
 // INTER_NEAREST for the label) by the drawn scale factor, float32 mean subtraction, zero / ignore-label padding to the crop size,
 // crop, mirror, HWC -> CHW.  Only the crop's pixels are ever computed: the reference resizes the whole 1024 x 2048 image (up to
 // 2150 x 4301) and then throws away all but 512 x 1024 of it.

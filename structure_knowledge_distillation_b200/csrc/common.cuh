@@ -1,4 +1,4 @@
-// Shared device/host helpers for libskd_b200.so (sm_100a only).
+// Shared device/host helpers for libskd_b200.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cstdint>
@@ -6,18 +6,13 @@
 
 namespace skd {
 
-constexpr int kNumSMs = 148;           // B200: 2 dies x 74 SMs; grids are sized in multiples of this
+constexpr int kNumSMs = 132;           // H100 SXM; grids are sized in multiples of this
 
 // thread-local last-error text, exposed through skd_last_error()
 void set_error(const char* where, cudaError_t err);
 void set_error_msg(const char* where, const char* msg);
-// 1: TMA tensor maps use CU_TENSOR_MAP_DATA_TYPE_TFLOAT32, 0: FLOAT32 (tcgen05 then ignores the low 13 mantissa bits)
+// 1: TMA tensor maps use CU_TENSOR_MAP_DATA_TYPE_TFLOAT32, 0: FLOAT32 (wgmma then ignores the low 13 mantissa bits)
 extern int g_tf32_tma_type;
-
-// conv_halo_sm100.cu: 3x3 / stride 1 / pad 1 convolutions with Cin, Cout <= 128 through one halo tile per channel chunk
-bool conv3x3_halo_supported(int Cin, int Cout, int passes);
-int conv3x3_halo_launch(int N, int H, int W, int Cin, int Cout, const float* x, const float* x_lo, int ldx, const float* w, const float* w_lo,
-                        float* y, int ldy, const float* scale, const float* shift, int act, float slope, int round_tf32, cudaStream_t st);
 
 // Reference convention (libs/src/bn.cu:244-249): every launcher returns 1 on success, 0 on a CUDA error.
 extern unsigned long long g_kernel_launches;     // kernels this library launched (skd_kernel_launches())

@@ -1,6 +1,6 @@
-// SIMT direct convolutions (NHWC, fp32 FMA) for the shapes the tcgen05 path does not take:
+// SIMT direct convolutions (NHWC, fp32 FMA) for the shapes the wgmma path does not take:
 //   * the 3-channel stem convolution (Cin=3: K=27, nothing for a tensor core to chew on; HBM-bound on its output)
-//   * strided data-gradients (two student convs) until they move to the sub-grid tcgen05 formulation
+//   * strided data-gradients (two student convs) until they move to the sub-grid wgmma formulation
 // They are also the on-device cross-check for the tensor-core kernels in tests (exact fp32 accumulation order aside).
 #include "common.cuh"
 #include "skd.h"
@@ -65,43 +65,74 @@ direct_dgrad_kernel(Geo g, const float* __restrict__ dy, int ldy, const float* _
   }
 }
 
-// dw[co,kh,kw,ci] += sum_pixels dy[p,co] * x[p shifted, ci]; grid.y splits the pixels, atomics merge (dw pre-zeroed)
-__global__ void __launch_bounds__(256)
+// The two reductions below give each output column group ONE CTA that walks all pixels and adds its warps' partials in fixed order:
+// deterministic (a training run is bit-reproducible), and -- unlike a cluster-wide reduction -- they need no co-scheduled SMs, so they
+// still slip in beside the persistent convolution kernels of the overlapping streams.
+constexpr int kWgWarps = 16;
+
+// dw[co,kh,kw,ci] = sum_pixels dy[p,co] * x[p shifted, ci]: one CTA per (tap, 32 input channels, 32 output channels).  Lane = input
+// channel (coalesced x reads), warp = pixel phase; each lane keeps the 32 output channels' sums, the dy row arrives by one coalesced load
+// and warp shuffles.
+__global__ void __launch_bounds__(kWgWarps * 32)
 direct_wgrad_kernel(Geo g, const float* __restrict__ x, int ldx, const float* __restrict__ dy, int ldy, float* __restrict__ dw) {
-  const int K = g.KH * g.KW * g.Cin;
-  const long long outs = (long long)g.Cout * K;
-  const long long o = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (o >= outs) return;
-  const int co = (int)(o % g.Cout); const int k = (int)(o / g.Cout);
-  const int ci = k % g.Cin, tap = k / g.Cin, kh = tap / g.KW, kw = tap - kh * g.KW;
+  __shared__ float red[kWgWarps / 2][32][33];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int ci_tiles = (g.Cin + 31) / 32, co_tiles = (g.Cout + 31) / 32;
+  const int cot = blockIdx.x % co_tiles, r0 = blockIdx.x / co_tiles;
+  const int cit = r0 % ci_tiles, tap = r0 / ci_tiles;
+  const int kh = tap / g.KW, kw = tap - kh * g.KW;
+  const int ci = cit * 32 + lane, co_lane = cot * 32 + lane;
   const long long P = (long long)g.N * g.OH * g.OW;
-  const long long per = (P + gridDim.y - 1) / gridDim.y;
-  const long long p0 = (long long)blockIdx.y * per, p1 = (p0 + per < P) ? p0 + per : P;
-  float acc = 0.f;
-  for (long long p = p0; p < p1; ++p) {
-    const int ox = (int)(p % g.OW); const long long r = p / g.OW; const int oy = (int)(r % g.OH), n = (int)(r / g.OH);
+  float acc[32];
+#pragma unroll
+  for (int c = 0; c < 32; ++c) acc[c] = 0.f;
+  long long p = warp;
+  int ox = (int)(p % g.OW); long long r = p / g.OW; int oy = (int)(r % g.OH), n = (int)(r / g.OH);
+  for (; p < P; p += kWgWarps) {
     const int iy = oy * g.stride - g.pad + kh * g.dil, ix = ox * g.stride - g.pad + kw * g.dil;
-    if (iy < 0 || iy >= g.H || ix < 0 || ix >= g.W) continue;
-    acc = fmaf(__ldg(dy + p * ldy + co), __ldg(x + (((size_t)n * g.H + iy) * g.W + ix) * ldx + ci), acc);
+    if (iy >= 0 && iy < g.H && ix >= 0 && ix < g.W) {                     // warp-uniform
+      const float xv = ci < g.Cin ? __ldg(x + (((size_t)n * g.H + iy) * g.W + ix) * ldx + ci) : 0.f;
+      const float dv = co_lane < g.Cout ? __ldg(dy + p * ldy + co_lane) : 0.f;
+#pragma unroll
+      for (int c = 0; c < 32; ++c) acc[c] = fmaf(__shfl_sync(0xffffffffu, dv, c), xv, acc[c]);
+    }
+    ox += kWgWarps;
+    while (ox >= g.OW) { ox -= g.OW; if (++oy == g.OH) { oy = 0; ++n; } }
   }
-  atomicAdd(dw + ((size_t)co * g.KH * g.KW + tap) * g.Cin + ci, acc);
+  // warps w and w + 8 first, then the eight sums in order
+  constexpr int H = kWgWarps / 2;
+  if (warp >= H) {
+#pragma unroll
+    for (int c = 0; c < 32; ++c) red[warp - H][c][lane] = acc[c];
+  }
+  __syncthreads();
+  if (warp < H) {
+#pragma unroll
+    for (int c = 0; c < 32; ++c) red[warp][c][lane] = acc[c] + red[warp][c][lane];
+  }
+  __syncthreads();
+  for (int i = threadIdx.x; i < 32 * 32; i += kWgWarps * 32) {
+    const int c = i >> 5, l = i & 31, co = cot * 32 + c, cc = cit * 32 + l;
+    if (co >= g.Cout || cc >= g.Cin) continue;
+    float t = red[0][c][l];
+    for (int w = 1; w < H; ++w) t += red[w][c][l];
+    dw[((size_t)co * g.KH * g.KW + tap) * g.Cin + cc] = t;
+  }
 }
 
-// db[c] = sum_rows dy[row][c]  (conv bias gradient; also used for the 19-class heads)
-__global__ void __launch_bounds__(256)
-colsum_kernel(const float* __restrict__ dy, int ldy, long long P, int C, float* __restrict__ db) {
+// db[c] (+)= sum_rows dy[row][c]  (conv bias gradient; also used for the 19-class heads): 32 columns x 32 row lanes per CTA
+__global__ void __launch_bounds__(1024)
+colsum_kernel(const float* __restrict__ dy, int ldy, long long P, int C, float* __restrict__ db, int accumulate) {
+  __shared__ float sh[32][33];
   const int c = blockIdx.x * 32 + (threadIdx.x & 31);
   const int lane_r = threadIdx.x >> 5;
-  __shared__ float sh[8][33];
   float a = 0.f;
-  const long long per = (P + gridDim.y - 1) / gridDim.y;
-  const long long p0 = (long long)blockIdx.y * per, p1 = (p0 + per < P) ? p0 + per : P;
-  if (c < C) for (long long p = p0 + lane_r; p < p1; p += 8) a += __ldg(dy + p * ldy + c);
+  if (c < C) for (long long p = lane_r; p < P; p += 32) a += __ldg(dy + p * ldy + c);
   sh[lane_r][threadIdx.x & 31] = a;
   __syncthreads();
   if (lane_r == 0 && c < C) {
-    for (int k = 1; k < 8; ++k) a += sh[k][threadIdx.x & 31];
-    atomicAdd(db + c, a);
+    for (int k = 1; k < 32; ++k) a += sh[k][threadIdx.x & 31];
+    db[c] = accumulate ? db[c] + a : a;
   }
 }
 
@@ -169,24 +200,12 @@ extern "C" int skd_conv2d_dgrad_direct(int N, int H, int W, int Cin, int Cout, i
 extern "C" int skd_conv2d_wgrad_direct(int N, int H, int W, int Cin, int Cout, int KH, int KW, int stride, int pad, int dil,
                                        const float* x, int ldx, const float* dy, int ldy, float* dw, cudaStream_t st) {
   const Geo g = make_geo(N, H, W, Cin, Cout, KH, KW, stride, pad, dil);
-  const long long outs = (long long)Cout * KH * KW * Cin;
-  if (cudaMemsetAsync(dw, 0, outs * sizeof(float), st) != cudaSuccess) return finish("skd_conv2d_wgrad_direct(memset)");
-  const long long P = (long long)N * g.OH * g.OW;
-  int bx = (int)((outs + 255) / 256);
-  long long split = (8LL * kNumSMs + bx - 1) / bx;
-  if (split > (P + 63) / 64) split = (P + 63) / 64;
-  if (split < 1) split = 1;
-  direct_wgrad_kernel<<<dim3(bx, (unsigned)split), 256, 0, st>>>(g, x, ldx, dy, ldy, dw);
+  direct_wgrad_kernel<<<KH * KW * ((Cin + 31) / 32) * ((Cout + 31) / 32), kWgWarps * 32, 0, st>>>(g, x, ldx, dy, ldy, dw);
   return finish("skd_conv2d_wgrad_direct");
 }
 
 static int colsum_launch(long long P, int C, const float* dy, int ldy, float* db, bool accumulate, cudaStream_t st) {
-  if (!accumulate && cudaMemsetAsync(db, 0, (size_t)C * sizeof(float), st) != cudaSuccess) return finish("skd_colsum(memset)");
-  const int bx = (C + 31) / 32;
-  long long split = (4LL * kNumSMs + bx - 1) / bx;
-  if (split > (P + 63) / 64) split = (P + 63) / 64;
-  if (split < 1) split = 1;
-  colsum_kernel<<<dim3(bx, (unsigned)split), 256, 0, st>>>(dy, ldy, P, C, db);
+  colsum_kernel<<<(C + 31) / 32, 1024, 0, st>>>(dy, ldy, P, C, db, accumulate ? 1 : 0);
   return finish("skd_colsum");
 }
 extern "C" int skd_colsum(long long P, int C, const float* dy, int ldy, float* db, cudaStream_t st) { return colsum_launch(P, C, dy, ldy, db, false, st); }

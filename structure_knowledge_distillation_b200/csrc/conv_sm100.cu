@@ -1,34 +1,27 @@
-// tcgen05 implicit-GEMM 2-D convolution for sm_100a (replaces every cuDNN nn.Conv2d call of
+// wgmma implicit-GEMM 2-D convolution for sm_90a (replaces every cuDNN nn.Conv2d call of
 // networks/pspnet_combine.py on the hot path: forward here; dgrad reuses this kernel on the output gradient with
 // flipped/transposed weights; wgrad is conv_wgrad_sm100.cu).
 //
 //   D[M = N*OH*OW pixels][Cout] = sum_{tap, ci}  X[pixel shifted by tap][ci] * W[Cout][tap][ci]
 //
 // Layout: activations NHWC fp32 (row pitch ld*, so channel slices of a concat buffer are addressable in place),
-// weights [Cout][KH][KW][Cin] (K-major), fp32 storage, TF32 tensor-core math with fp32 accumulation in TMEM.
+// weights [Cout][KH][KW][Cin] (K-major), fp32 storage, TF32 tensor-core math with fp32 accumulation in registers.
 //
-// One persistent CTA per SM (or one CTA PAIR per TPC, template parameter PAIR = 2), 10 warps:
-//   warp 0   TMA producer  : per (tap, 32-channel chunk) one A box of X -- 128 consecutive output pixels in TMA im2col mode
-//                            (tap shift / padding / stride / dilation in the tensor map, out-of-bounds = hardware zero fill),
-//                            a flat [pixels][C] box for 1x1 convs, or a BH x BW rectangle in tiled mode -- plus one 3-D box
-//                            {32ch, 1 tap, BLOCK_N} of W, both 128B-swizzled, landing on a full[] mbarrier of a 2..8-stage
-//                            ring.  Split precision (3xTF32): the stage also holds the low parts of both operands.
-//   warp 1   MMA issuer    : 4 x tcgen05.mma.kind::tf32 (M=128, N=BLOCK_N, K=8) per stage (x3 for split precision),
-//                            accumulator in TMEM (2 accumulator stages x BLOCK_N columns), tcgen05.commit releases smem
-//                            stages / signals the epilogue.
-//   warps 2-9 epilogue     : two groups of four warps (one per TMEM lane quarter) take alternate 32-column chunks:
-//                            tcgen05.ld 32x32b -> registers -> fused per-channel scale/shift (folded BN or bias, staged
-//                            in smem), residual add (residual boxes arrive through a per-group TMA ring), ReLU /
-//                            leaky-ReLU -> 128B-swizzled smem staging -> TMA store of the 128px x 32ch box (coalesced,
-//                            async, hardware-clipped at the ragged edges).  Overlaps the next tile's MMAs through the
-//                            second TMEM accumulator stage.
-//   PAIR = 2               : cluster of two CTAs, tcgen05 cta_group::2: M = 256 per tile, each CTA stages its own 128 pixels
-//                            and half of the weight tile; the leader CTA issues the MMAs and multicasts the commits.
+// One persistent CTA per SM, three warpgroups:
+//   warpgroup 0     TMA producer (one thread): per (tap, 32-channel chunk) one A box of X -- 128 consecutive output pixels in TMA
+//                   im2col mode (tap shift / padding / stride / dilation in the tensor map, out-of-bounds = hardware zero fill),
+//                   a flat [pixels][C] box for 1x1 convs, or a BH x BW rectangle in tiled mode -- plus one 3-D box
+//                   {32ch, 1 tap, BLOCK_N} of W, both 128B-swizzled K-major, landing on a full[] mbarrier of a multi-stage ring.
+//                   Split precision (3xTF32): the stage also holds the low parts of both operands.
+//   warpgroups 1-2  consumers: warpgroup g owns GEMM rows 64g .. 64g+63 of the 128-pixel tile; 4 x wgmma.m64nNk8.tf32 per stage
+//                   (x3 for split precision), accumulator in registers, the stage released one stage later (one wgmma batch in
+//                   flight); epilogue straight from the registers: per-channel scale/shift (folded BN or bias), residual add,
+//                   ReLU / leaky-ReLU / ELU, optional TF32 rounding and fused sum of squares, global stores.
 #include <cuda.h>
 
 #include "common.cuh"
 #include "skd.h"
-#include "sm100_ptx.cuh"
+#include "sm90_ptx.cuh"
 
 using namespace skd;
 
@@ -36,27 +29,22 @@ namespace {
 
 constexpr int kBlockM = 128;
 constexpr int kBlockK = 32;                 // fp32 elements = 128 B = one swizzle row
-constexpr int kUmmaK = 8;                   // tf32
-constexpr int kThreads = 320;              // TMA warp + MMA warp + 8 epilogue warps
+constexpr int kWgmmaK = 8;                  // tf32
+constexpr int kThreads = 384;               // producer warpgroup + 2 consumer warpgroups
 constexpr int kABytes = kBlockM * kBlockK * 4;
-constexpr int kResSlots = 3;                // residual ring depth per epilogue group: two loads in flight while one is consumed
 
 struct ConvArgs {
   int N, OH, OW, Cout, Cin;
   int KH, KW, stride, pad, dil;
   int BH, BW, tiles_x, tiles_y;
   int m_tiles, n_tiles, k_chunks;
-  float* y; int ldy;
+  float* y; int ldy; long long y_row, y_img;   // output element (img, oy, ox, c) at y[img * y_img + oy * y_row + ox * ldy + c]
   const float* scale; const float* shift;
   const float* residual; int ldr;
   int act; float slope; int round_out;
-  int vec_ok;
-  int tma_store;
   double* sumsq;                   // optional: += sum of squares of every valid output element (fused L2 reduction)
   int no_store;                    // 1: the output tensor is not written at all (reduction-only epilogue)
-  int passes;                      // 1: TF32;  3: split-precision 3xTF32 (x_hi*w_hi + x_lo*w_hi + x_hi*w_lo, fp32-grade result)
-  int nstages;                     // A/B pipeline stages in use (the residual ring takes over the buffers of the others)
-  int res_prefetch;                // residual tiles arrive through a TMA ring (kResSlots 16 KB slots per epilogue group)
+  int nstages;                     // A/B pipeline stages in use
   int kc_outer;                    // K loop order: 1 = channel chunk outermost / taps innermost, 0 = taps outermost
   int reverse;                     // walk the tile list back to front (alternated per layer so a layer starts on the
                                    // activations its producer wrote last, which are still in L2)
@@ -65,92 +53,59 @@ struct ConvArgs {
   long long split_stride;          //   raw fp32 partials go to y + split * split_stride; splitk_epilogue_kernel adds them and applies the epilogue
 };
 
-// PAIR = 1: one CTA per 128 x BLOCK_N tile (cta_group::1).
-// PAIR = 2: a cluster of two CTAs (one TPC) computes a 256 x BLOCK_N tile with cta_group::2 MMAs: each CTA stages its own 128
-//           pixels of A and only HALF of the weight tile, so the L2 -> shared-memory traffic per FLOP drops by a third (with fp32
-//           operands a 128 x 256 cta_group::1 tile needs ~62 B/clk/SM of fill bandwidth at full tensor rate -- the limiter).
-template <int BLOCK_N, int PAIR>
+template <int BLOCK_N, bool SPLIT>
 struct Cfg {
-  static constexpr int kBBytes = (BLOCK_N / PAIR) * kBlockK * 4;
-  static constexpr int kStageBytes = kABytes + kBBytes;
-  static constexpr int kOutStageBytes = kBlockM * 32 * 4;                      // one 128-pixel x 32-channel chunk
-  static constexpr int kFixedBytes = 2 * kOutStageBytes + 768 /*align slack*/ + 256 /*barriers*/ + 2 * BLOCK_N * 4;
+  static constexpr int kBBytes = BLOCK_N * kBlockK * 4;
+  static constexpr int kStageBytes = (kABytes + kBBytes) * (SPLIT ? 2 : 1);   // split precision: {x_hi, w_hi, x_lo, w_lo}
+  static constexpr int kFixedBytes = 1024 /*align slack*/ + 256 /*barriers*/;
   static constexpr int kFit = (232448 - kFixedBytes) / kStageBytes;
-  static constexpr int kStages = kFit > 8 ? 8 : kFit;                           // 4 / 6 / 8 / 8 (PAIR 1), 6 / 8 (PAIR 2)
-  // split precision: the K steps of a tile go round-robin to kSub sub-accumulators that the epilogue adds with round-to-nearest fp32
-  // adds (the tensor core truncates on every accumulate: with hundreds of MMAs per tile that, not the operand split, limited the
-  // "fp32-grade" layers to ~1e-5).  2 stages x kSub x BLOCK_N columns.
-  static constexpr int kSub = BLOCK_N >= 256 ? 1 : (BLOCK_N == 128 ? 2 : 4);
-  static constexpr int kTmemCols = (2 * kSub * BLOCK_N < 32) ? 32 : 2 * kSub * BLOCK_N;       // power of two: 256..512
+  static constexpr int kStages = kFit > 8 ? 8 : kFit;
   static constexpr int kSmemBytes = kStages * kStageBytes + kFixedBytes;
+  static_assert(kStages >= 2, "at least two pipeline stages");
   static_assert(kSmemBytes <= 232448, "exceeds the 227 KB of shared memory a CTA may use");
 };
 
-template <int BLOCK_N, int PAIR>
+__device__ __forceinline__ float epi_act(float v, int act, float slope) {
+  if (act == ACT_RELU) return fmaxf(v, 0.f);
+  if (act == ACT_LEAKY) return v < 0.f ? v * slope : v;
+  if (act == ACT_ELU) return v < 0.f ? expm1f(v) : v;
+  return v;
+}
+
+template <int BLOCK_N, bool SPLIT>
 __global__ void __launch_bounds__(kThreads, 1)
-conv_fwd_sm100_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_w,
-                      const __grid_constant__ CUtensorMap tmap_y, const __grid_constant__ CUtensorMap tmap_x2,
-                      const __grid_constant__ CUtensorMap tmap_w2, const __grid_constant__ CUtensorMap tmap_r, const ConvArgs a) {
-  using C = Cfg<BLOCK_N, PAIR>;
+conv_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_w,
+                     const __grid_constant__ CUtensorMap tmap_x2, const __grid_constant__ CUtensorMap tmap_w2, const ConvArgs a) {
+  using C = Cfg<BLOCK_N, SPLIT>;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   // keep the pointer in the shared address space (integer round trips make nvcc emit generic LD/ST instead of LDS/STS)
   const uint32_t raw_addr = ptx::smem_u32(smem_raw);
   uint8_t* smem = smem_raw + (((raw_addr + 1023u) & ~1023u) - raw_addr);
-  uint8_t* out_stage = smem + C::kStages * C::kStageBytes;                   // 2 x 16 KB, 1024-aligned
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(out_stage + 2 * C::kOutStageBytes);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + C::kStages * C::kStageBytes);
   uint64_t* empty_bar = full_bar + C::kStages;
-  uint64_t* tmem_full = empty_bar + C::kStages;
-  uint64_t* tmem_empty = tmem_full + 2;
-  uint32_t* tmem_base_slot = reinterpret_cast<uint32_t*>(tmem_empty + 2);
-  uint64_t* res_full = reinterpret_cast<uint64_t*>(tmem_base_slot + 2);                  // [2 groups][kResSlots]
-  float* s_scale = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(full_bar) + 256);   // [BLOCK_N], 16B aligned
-  float* s_shift = s_scale + BLOCK_N;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  // pair mode: rank 0 is the leader (issues the MMAs; owns the full / tmem_empty barriers both CTAs signal)
-  const uint32_t cta_rank = (PAIR == 2) ? ptx::cluster_ctarank() : 0u;
-  const int tile0 = (PAIR == 2) ? (int)(blockIdx.x >> 1) : (int)blockIdx.x;      // first tile of this CTA / CTA pair
-  const int tile_step = (PAIR == 2) ? (int)(gridDim.x >> 1) : (int)gridDim.x;
-
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     ptx::prefetch_tmap(&tmap_x);
     ptx::prefetch_tmap(&tmap_w);
-    if (a.tma_store) ptx::prefetch_tmap(&tmap_y);
-    for (int s = 0; s < C::kStages; ++s) { ptx::mbar_init(&full_bar[s], 1); ptx::mbar_init(&empty_bar[s], 1); }
-    for (int s = 0; s < 2; ++s) { ptx::mbar_init(&tmem_full[s], 1); ptx::mbar_init(&tmem_empty[s], 8 * PAIR); }
-    for (int s = 0; s < 2 * (kResSlots + 1); ++s) ptx::mbar_init(&res_full[s], 1);
-    if (a.res_prefetch) ptx::prefetch_tmap(&tmap_r);
+    for (int s = 0; s < C::kStages; ++s) { ptx::mbar_init(&full_bar[s], 1); ptx::mbar_init(&empty_bar[s], 8); }   // one arrival per consumer warp
     ptx::fence_barrier_init();
   }
-  if (warp == 1) {
-    if constexpr (PAIR == 2) ptx::tmem_alloc_2cta<C::kTmemCols>(tmem_base_slot);
-    else ptx::tmem_alloc<C::kTmemCols>(tmem_base_slot);
-  }
-  ptx::tc_fence_before();
-  if constexpr (PAIR == 2) ptx::cluster_sync(); else __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem_base = *tmem_base_slot;
+  __syncthreads();
 
-  // pair mode: a tile is two consecutive M tiles (this CTA's is 2*pm + rank; a ragged last one is a phantom that loads zeros)
-  const int m_units = (PAIR == 2) ? (a.m_tiles + 1) / 2 : a.m_tiles;
-  const int total_tiles = m_units * a.n_tiles * a.splits;       // work units: (tile, K range); the K ranges of a tile are consecutive units
+  const int total_tiles = a.m_tiles * a.n_tiles * a.splits;     // work units: (tile, K range); the K ranges of a tile are consecutive units
   const int taps = a.KH * a.KW;
   const int k_iters = taps * a.k_chunks;
-  // split-precision (passes == 3): a stage holds {x_hi, w_hi, x_lo, w_lo} tiles and every K step issues hi*hi + lo*hi + hi*lo
-  const bool split3 = (a.passes == 3);
-  const int stage_stride = split3 ? 2 * C::kStageBytes : C::kStageBytes;
   const int tiles_per_img = a.tiles_x * a.tiles_y;
 
-  if (warp == 0) {
+  if (warp < 4) {
     // ===================== TMA producer =====================
-    if (lane == 0) {
+    if (threadIdx.x == 0) {
       int stage = 0; uint32_t phase = 0;
-      const uint32_t full_bar0 = (PAIR == 2) ? ptx::mapa_shared(&full_bar[0], 0) : 0u;   // the leader's full barriers
-      for (int tile = tile0; tile < total_tiles; tile += tile_step) {
+      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
         const int tu = a.reverse ? total_tiles - 1 - tile : tile;
         const int tl = tu / a.splits, sp = tu - tl * a.splits;
-        const int mu = tl / a.n_tiles, nt = tl - mu * a.n_tiles;
-        const int mt = (PAIR == 2) ? 2 * mu + (int)cta_rank : mu;
+        const int mt = tl / a.n_tiles, nt = tl - mt * a.n_tiles;
         const int img = mt / tiles_per_img, rem = mt - img * tiles_per_img;
         const int ty = rem / a.tiles_x, tx = rem - ty * a.tiles_x;
         const int iy0 = ty * a.BH * a.stride - a.pad, ix0 = tx * a.BW * a.stride - a.pad;
@@ -164,358 +119,138 @@ conv_fwd_sm100_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_c
           iq0 = (r2 % a.rOW) * a.stride - a.pad;
         }
         // kc_outer: channel chunk outermost, filter taps innermost -- the taps of one chunk re-read (shifted) the same input lines,
-        // L2 hits whatever Cin is.  Taps outermost streams Cin * 128 pixels * 148 CTAs between reuses (310 MB at Cin = 4096, far
-        // beyond L2: 679 -> 748 TFLOP/s on the PSP bottleneck) but measured ~5% faster while that working set still fits.
+        // L2 hits whatever Cin is; taps outermost streams Cin * 128 pixels per CTA between reuses.
         const int n_inner = a.kc_outer ? taps : a.k_chunks;
         const int k0 = sp * a.k_per_split, k1 = min(k_iters, k0 + a.k_per_split);
-        {
-          for (int k = k0; k < k1; ++k) {
-            const int io = k / n_inner, ii = k - io * n_inner;
-            const int kc = a.kc_outer ? io : ii, tap = a.kc_outer ? ii : io;
-            const int kh = tap / a.KW, kw = tap - kh * a.KW;
-            ptx::mbar_wait(&empty_bar[stage], phase ^ 1);
-            uint8_t* sa = smem + stage * stage_stride;
-            uint8_t* sb = sa + kABytes;
-            const uint32_t bytes = (uint32_t)stage_stride;
-            if constexpr (PAIR == 2) {
-              // both CTAs' loads complete on the LEADER's barrier, which expects the bytes of both
-              if (cta_rank == 0) ptx::mbar_expect_tx(&full_bar[stage], 2 * bytes);
-              const uint32_t fb = full_bar0 + (uint32_t)stage * 8u;
-              const int wrow = nt * BLOCK_N + (int)cta_rank * (BLOCK_N / 2);
-              for (int part = 0; part < (split3 ? 2 : 1); ++part) {
-                const CUtensorMap* mx = part ? &tmap_x2 : &tmap_x;
-                const CUtensorMap* mw = part ? &tmap_w2 : &tmap_w;
-                uint8_t* pa = sa + part * C::kStageBytes; uint8_t* pb = sb + part * C::kStageBytes;
-                if (a.im2col)
-                  ptx::tma_load_im2col_4d_2cta(pa, mx, fb, kc * kBlockK, iq0, ip0, in0, (uint16_t)(kw * a.dil), (uint16_t)(kh * a.dil));
-                else
-                  ptx::tma_load_4d_2cta(pa, mx, fb, kc * kBlockK, ix0 + kw * a.dil, iy0 + kh * a.dil, img);
-                ptx::tma_load_3d_2cta(pb, mw, fb, kc * kBlockK, tap, wrow);
-              }
-            } else {
-              ptx::mbar_expect_tx(&full_bar[stage], bytes);
-              for (int part = 0; part < (split3 ? 2 : 1); ++part) {
-                const CUtensorMap* mx = part ? &tmap_x2 : &tmap_x;
-                const CUtensorMap* mw = part ? &tmap_w2 : &tmap_w;
-                uint8_t* pa = sa + part * C::kStageBytes; uint8_t* pb = sb + part * C::kStageBytes;
-                if (a.im2col)
-                  ptx::tma_load_im2col_4d(pa, mx, &full_bar[stage], kc * kBlockK, iq0, ip0, in0, (uint16_t)(kw * a.dil), (uint16_t)(kh * a.dil));
-                else
-                  ptx::tma_load_4d(pa, mx, &full_bar[stage], kc * kBlockK, ix0 + kw * a.dil, iy0 + kh * a.dil, img);
-                ptx::tma_load_3d(pb, mw, &full_bar[stage], kc * kBlockK, tap, nt * BLOCK_N);
-              }
-            }
-            if (++stage == a.nstages) { stage = 0; phase ^= 1; }
-          }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer (pair mode: the leader CTA only) =====================
-    constexpr uint32_t idesc = ptx::make_idesc_tf32(kBlockM * PAIR, BLOCK_N, 0, 0);
-    int stage = 0; uint32_t phase = 0;
-    int acc = 0; uint32_t acc_phase = 0;
-    for (int tile = tile0; tile < total_tiles && cta_rank == 0; tile += tile_step) {
-      if (lane == 0) ptx::mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-      __syncwarp();
-      ptx::tc_fence_after();
-      const uint32_t tmem_acc = tmem_base + (uint32_t)(acc * C::kSub * BLOCK_N);
-      const int nsub = split3 ? C::kSub : 1;
-      uint32_t used = 0;
-      const int tu = a.reverse ? total_tiles - 1 - tile : tile;
-      const int sp = tu % a.splits;
-      const int nk = min(k_iters, (sp + 1) * a.k_per_split) - sp * a.k_per_split;      // K steps of this unit (all of them without split-K)
-      for (int k = 0; k < nk; ++k) {
-        if (lane == 0) {
-          ptx::mbar_wait(&full_bar[stage], phase);
-          ptx::tc_fence_after();
-          const uint32_t sa = ptx::smem_u32(smem + stage * stage_stride);
-          const uint32_t sb = sa + kABytes;
-          const int sub = k % nsub;
-          const uint32_t tmem_d = tmem_acc + (uint32_t)(sub * BLOCK_N);
-          auto mma = [&](uint64_t da, uint64_t db, uint32_t accumulate) {
-            if constexpr (PAIR == 2) ptx::mma_tf32_2cta(tmem_d, da, db, idesc, accumulate);
-            else ptx::mma_tf32(tmem_d, da, db, idesc, accumulate);
-          };
+        for (int k = k0; k < k1; ++k) {
+          const int io = k / n_inner, ii = k - io * n_inner;
+          const int kc = a.kc_outer ? io : ii, tap = a.kc_outer ? ii : io;
+          const int kh = tap / a.KW, kw = tap - kh * a.KW;
+          ptx::mbar_wait(&empty_bar[stage], phase ^ 1);
+          uint8_t* sa = smem + stage * C::kStageBytes;
+          ptx::mbar_expect_tx(&full_bar[stage], (uint32_t)C::kStageBytes);
 #pragma unroll
-          for (int kk = 0; kk < kBlockK / kUmmaK; ++kk) {
-            const uint64_t da = ptx::make_smem_desc_sw128(sa + kk * kUmmaK * 4, 16, 1024);
-            const uint64_t db = ptx::make_smem_desc_sw128(sb + kk * kUmmaK * 4, 16, 1024);
-            mma(da, db, ((used >> sub) & 1u) | (kk != 0 ? 1u : 0u));
-            if (split3) {                                       // + x_lo * w_hi + x_hi * w_lo (the lo tiles sit kStageBytes further)
-              mma(ptx::make_smem_desc_sw128(sa + C::kStageBytes + kk * kUmmaK * 4, 16, 1024), db, 1u);
-              mma(da, ptx::make_smem_desc_sw128(sb + C::kStageBytes + kk * kUmmaK * 4, 16, 1024), 1u);
-            }
+          for (int part = 0; part < (SPLIT ? 2 : 1); ++part) {
+            const CUtensorMap* mx = part ? &tmap_x2 : &tmap_x;
+            const CUtensorMap* mw = part ? &tmap_w2 : &tmap_w;
+            uint8_t* pa = sa + part * (kABytes + C::kBBytes);
+            uint8_t* pb = pa + kABytes;
+            if (a.im2col)
+              ptx::tma_load_im2col_4d(pa, mx, &full_bar[stage], kc * kBlockK, iq0, ip0, in0, (uint16_t)(kw * a.dil), (uint16_t)(kh * a.dil));
+            else
+              ptx::tma_load_4d(pa, mx, &full_bar[stage], kc * kBlockK, ix0 + kw * a.dil, iy0 + kh * a.dil, img);
+            ptx::tma_load_3d(pb, mw, &full_bar[stage], kc * kBlockK, tap, nt * BLOCK_N);
           }
-          used |= 1u << sub;
-          if constexpr (PAIR == 2) {                          // multicast: the stage / accumulator barriers of both CTAs
-            ptx::mma_commit_2cta(&empty_bar[stage]);
-            if (k == nk - 1) ptx::mma_commit_2cta(&tmem_full[acc]);
-          } else {
-            ptx::mma_commit(&empty_bar[stage]);               // smem stage reusable once these MMAs retire
-            if (k == nk - 1) ptx::mma_commit(&tmem_full[acc]);
-          }
+          if (++stage == a.nstages) { stage = 0; phase ^= 1; }
         }
-        __syncwarp();
-        if (++stage == a.nstages) { stage = 0; phase ^= 1; }
       }
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
     }
   } else {
-    // ===================== epilogue (warps 2..9: two groups of four, one warp per TMEM lane quarter) =====================
-    const int ew = warp - 2;
-    const int quarter = warp & 3;                              // TMEM lane quarter this warp may access
-    const int group = ew >> 2;                                 // group g takes the 32-column chunks ch = g, g+2, ...
-    const int row = quarter * 32 + lane;                       // accumulator row == pixel inside the tile
-    const int etid = ew * 32 + lane;                           // 0..255 over both groups
-    const bool is_store_leader = ((ew & 3) == 0 && lane == 0);
-    const int dy = row / a.BW, dx = row - dy * a.BW;
-    uint8_t* stg = out_stage + group * C::kOutStageBytes;
-    int acc = 0; uint32_t acc_phase = 0;
+    // ===================== consumers: warpgroup g = rows 64g .. 64g+63 of the tile =====================
+    const int g = (warp >> 2) - 1;
+    const int wq = warp & 3;
+    const int r_lo = g * 64 + wq * 16 + (lane >> 2);          // tile rows of this thread's fragment: r_lo and r_lo + 8
+    const int cq = 2 * (lane & 3);                             // first of the thread's two columns in every 8-column group
+    constexpr int R = BLOCK_N / 2;
+    float acc[R];
+    float tot[SPLIT ? R : 1];
     double sq_acc = 0.0;
-    const int gt = (ew & 3) * 32 + lane, ck = gt & 7;            // coalesced mapping: 8 threads per 128-byte pixel row
-    // residual ring (res_prefetch): the group's store leader TMA-loads the BH x BW x 32ch residual box of the chunks this group
-    // will process, kResSlots - 1 chunks ahead, into the buffers of the unused pipeline stages (same 128B-swizzled layout as the
-    // output staging tile).  Deep, asynchronous and issued by one thread: the epilogue warps never wait on global memory.
-    uint8_t* ring = smem + a.nstages * C::kStageBytes + group * (kResSlots * C::kOutStageBytes);
-    uint64_t* rfull = res_full + group * (kResSlots + 1);
-    // in-place mode (res_prefetch == 2): kResSlots + 1 slots per group -- the ring plus the group's staging buffer.  A slot receives the
-    // residual box (TMA load), the epilogue adds the scaled accumulator INTO it (each thread owns its pixel row: same swizzled
-    // addresses the staging write would use, no cross-thread exchange), and the TMA store reads it: one named barrier per chunk
-    // instead of three, and the next chunk never waits for the previous store to drain.
-    const int n_slots = a.res_prefetch == 2 ? kResSlots + 1 : kResSlots;
-    auto slot_ptr = [&](int slot) -> uint8_t* { return slot < kResSlots ? ring + slot * C::kOutStageBytes : stg; };
-    auto chunk_valid = [&](int t, int c) -> bool {
-      const int tl_ = (a.reverse ? total_tiles - 1 - t : t) / a.splits;
-      const int nt_ = tl_ % a.n_tiles;
-      return c < BLOCK_N / 32 && nt_ * BLOCK_N + c * 32 < a.Cout;
-    };
-    auto seek = [&](int& t, int& c) {                               // first (tile, chunk) of this group at or after (t, c)
-      while (t < total_tiles && !chunk_valid(t, c)) { t += tile_step; c = group; }
-    };
-    auto issue_residual = [&](int t, int c, int slot) {
-      const int tl_ = (a.reverse ? total_tiles - 1 - t : t) / a.splits;
-      const int mu_ = tl_ / a.n_tiles, nt_ = tl_ - mu_ * a.n_tiles;
-      const int mt_ = (PAIR == 2) ? 2 * mu_ + (int)cta_rank : mu_;
-      const int img_ = mt_ / tiles_per_img, rem_ = mt_ - img_ * tiles_per_img;
-      const int ty_ = rem_ / a.tiles_x, tx_ = rem_ - ty_ * a.tiles_x;
-      ptx::mbar_expect_tx(&rfull[slot], C::kOutStageBytes);
-      ptx::tma_load_4d(slot_ptr(slot), &tmap_r, &rfull[slot], nt_ * BLOCK_N + c * 32, tx_ * a.BW, ty_ * a.BH, img_);
-    };
-    int p_tile = total_tiles, p_ch = group;                          // next chunk to request (store leader only)
-    if (a.res_prefetch && is_store_leader) {
-      p_tile = tile0; seek(p_tile, p_ch);
-      for (int i = 0; i < n_slots && p_tile < total_tiles; ++i) { issue_residual(p_tile, p_ch, i); p_ch += 2; seek(p_tile, p_ch); }
-    }
-    int r_slot = 0; uint32_t r_phase = 0;                            // ring slot / parity of the chunk being consumed
-    int prev_slot = -1;                                              // in-place mode: slot whose store was committed one chunk ago
-    const uint32_t tmem_empty0 = (PAIR == 2) ? ptx::mapa_shared(&tmem_empty[0], 0) : 0u;   // the leader's tmem_empty barriers
-    for (int tile = tile0; tile < total_tiles; tile += tile_step) {
+    int stage = 0; uint32_t phase = 0;
+    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
       const int tu = a.reverse ? total_tiles - 1 - tile : tile;
       const int tl = tu / a.splits, sp = tu - tl * a.splits;
-      const int mu = tl / a.n_tiles, nt = tl - mu * a.n_tiles;
-      const int mt = (PAIR == 2) ? 2 * mu + (int)cta_rank : mu;
-      const int img = mt / tiles_per_img, rem = mt - img * tiles_per_img;
-      const int ty = rem / a.tiles_x, tx = rem - ty * a.tiles_x;
-      const int oy = ty * a.BH + dy, ox = tx * a.BW + dx;
-      const bool valid = (oy < a.OH) && (ox < a.OW) && (mt < a.m_tiles);
-      const size_t pix = ((size_t)img * a.OH + oy) * a.OW + ox;
-      float* yrow = a.y + (size_t)sp * a.split_stride + pix * a.ldy;
-      const float* rrow = (a.residual && valid) ? a.residual + pix * a.ldr : nullptr;
+      const int mt = tl / a.n_tiles, nt = tl - mt * a.n_tiles;
+      const int nk = min(k_iters, (sp + 1) * a.k_per_split) - sp * a.k_per_split;      // K steps of this unit
+      if constexpr (SPLIT) {
+#pragma unroll
+        for (int i = 0; i < R; ++i) tot[i] = 0.f;
+      }
+      int prev_stage = -1;
+      for (int k = 0; k < nk; ++k) {
+        ptx::mbar_wait(&full_bar[stage], phase);
+        const uint32_t sa = ptx::smem_u32(smem + stage * C::kStageBytes) + (uint32_t)(g * 64 * 128);
+        const uint32_t sb = ptx::smem_u32(smem + stage * C::kStageBytes) + (uint32_t)kABytes;
+        ptx::wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < kBlockK / kWgmmaK; ++kk) {
+          const uint64_t da = ptx::make_wgmma_desc_sw128(sa + kk * kWgmmaK * 4);
+          const uint64_t db = ptx::make_wgmma_desc_sw128(sb + kk * kWgmmaK * 4);
+          if constexpr (SPLIT) {
+            // split precision: this stage's x_hi*w_hi + x_lo*w_hi + x_hi*w_lo in a fresh accumulator, added to the running total with
+            // round-to-nearest fp32 adds below (the tensor core truncates on every accumulate: over hundreds of K steps that, not the
+            // operand split, would limit the "fp32-grade" layers)
+            constexpr uint32_t kLo = kABytes + C::kBBytes;
+            ptx::wgmma_tf32<BLOCK_N>(acc, da, db, kk != 0 ? 1u : 0u);
+            ptx::wgmma_tf32<BLOCK_N>(acc, ptx::make_wgmma_desc_sw128(sa + kLo + kk * kWgmmaK * 4), db, 1u);
+            ptx::wgmma_tf32<BLOCK_N>(acc, da, ptx::make_wgmma_desc_sw128(sb + kLo + kk * kWgmmaK * 4), 1u);
+          } else {
+            ptx::wgmma_tf32<BLOCK_N>(acc, da, db, (k | kk) != 0 ? 1u : 0u);
+          }
+        }
+        ptx::wgmma_commit();
+        if constexpr (SPLIT) {
+          ptx::wgmma_wait<0>();
+          ptx::fence_regs(acc);
+#pragma unroll
+          for (int i = 0; i < R; ++i) tot[i] += acc[i];
+          if (lane == 0) ptx::mbar_arrive(&empty_bar[stage]);
+        } else {
+          ptx::wgmma_wait<1>();                                  // the previous stage's wgmmas are done: release its buffers
+          if (prev_stage >= 0 && lane == 0) ptx::mbar_arrive(&empty_bar[prev_stage]);
+          prev_stage = stage;
+        }
+        if (++stage == a.nstages) { stage = 0; phase ^= 1; }
+      }
+      if constexpr (!SPLIT) {
+        ptx::wgmma_wait<0>();
+        ptx::fence_regs(acc);
+        if (prev_stage >= 0 && lane == 0) ptx::mbar_arrive(&empty_bar[prev_stage]);
+      }
+      if constexpr (SPLIT) {
+#pragma unroll
+        for (int i = 0; i < R; ++i) acc[i] = tot[i];
+      }
+      const float* v = acc;
 
-      // per-channel affine of this N tile -> shared memory (ones / zeros when absent, zeros past Cout)
-      ptx::named_bar_sync(3, 256);
-      if (etid < BLOCK_N) {
-        const int c = nt * BLOCK_N + etid;
-        s_scale[etid] = (c < a.Cout) ? (a.scale ? __ldg(a.scale + c) : 1.f) : 0.f;
-        s_shift[etid] = (c < a.Cout && a.shift) ? __ldg(a.shift + c) : 0.f;
+      // ---- epilogue straight from the fragment ----
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int row = r_lo + 8 * h;
+        const int img = mt / tiles_per_img, rem = mt - img * tiles_per_img;
+        const int ty = rem / a.tiles_x, tx = rem - ty * a.tiles_x;
+        const int dy = row / a.BW, dx = row - dy * a.BW;
+        const int oy = ty * a.BH + dy, ox = tx * a.BW + dx;
+        if (oy >= a.OH || ox >= a.OW) continue;
+        float* yrow = a.y + (size_t)sp * a.split_stride + (size_t)img * a.y_img + (size_t)oy * a.y_row + (size_t)ox * a.ldy;
+        const float* rrow = a.residual ? a.residual + (((size_t)img * a.OH + oy) * a.OW + ox) * a.ldr : nullptr;
+        float part = 0.f;
+#pragma unroll
+        for (int j = 0; j < BLOCK_N / 8; ++j) {
+          const int c = nt * BLOCK_N + 8 * j + cq;
+          if (c >= a.Cout) continue;
+          const bool two = c + 1 < a.Cout;
+          float v0 = v[4 * j + 2 * h], v1 = v[4 * j + 2 * h + 1];
+          if (a.scale) { v0 *= __ldg(a.scale + c); if (two) v1 *= __ldg(a.scale + c + 1); }
+          if (a.shift) { v0 += __ldg(a.shift + c); if (two) v1 += __ldg(a.shift + c + 1); }
+          if (rrow) { v0 += __ldg(rrow + c); if (two) v1 += __ldg(rrow + c + 1); }
+          v0 = epi_act(v0, a.act, a.slope); v1 = epi_act(v1, a.act, a.slope);
+          if (a.round_out) { v0 = ptx::round_tf32(v0); v1 = ptx::round_tf32(v1); }
+          if (a.sumsq) part = fmaf(v0, v0, two ? fmaf(v1, v1, part) : part);
+          if (a.no_store) continue;
+          if (two && !((reinterpret_cast<uintptr_t>(yrow + c)) & 7)) {
+            *reinterpret_cast<float2*>(yrow + c) = make_float2(v0, v1);
+          } else {
+            yrow[c] = v0;
+            if (two) yrow[c + 1] = v1;
+          }
+        }
+        sq_acc += (double)part;                                 // fp32 within a row of the tile, fp64 across rows and tiles
       }
-      ptx::named_bar_sync(3, 256);
-
-      ptx::mbar_wait(&tmem_full[acc], acc_phase);
-      ptx::tc_fence_after();
-      const uint32_t taddr = tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(acc * C::kSub * BLOCK_N);
-      const int nk_e = min(k_iters, (sp + 1) * a.k_per_split) - sp * a.k_per_split;     // K steps of this unit: sub-accumulators in use
-      const int nsub_e = split3 ? min(C::kSub, nk_e) : 1;
-#pragma unroll 1
-      for (int ch = group; ch < BLOCK_N / 32; ch += 2) {
-        const int c0 = nt * BLOCK_N + ch * 32;
-        if (c0 >= a.Cout) break;                                               // CTA-uniform
-        // residual tile read COALESCED (8 threads cover the 128 B of one pixel row, a warp covers 4 rows; the per-row
-        // mapping of the TMEM load would touch 32 lines per instruction).  Either prefetched one chunk ahead with cp.async
-        // into the spare pipeline-stage buffer (res_prefetch) or loaded into registers here, before the TMEM load.
-        const bool coalesced_res = (a.residual != nullptr) && a.tma_store && a.vec_ok;      // CTA-uniform
-        float4 q[8];
-        if (coalesced_res && !a.res_prefetch) {
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const int rr = i * 16 + (gt >> 3);
-            const int roy = ty * a.BH + rr / a.BW, rox = tx * a.BW + rr % a.BW;
-            q[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (roy < a.OH && rox < a.OW && c0 + ck * 4 + 3 < a.Cout && mt < a.m_tiles)
-              q[i] = __ldg(reinterpret_cast<const float4*>(a.residual + (((size_t)img * a.OH + roy) * a.OW + rox) * a.ldr + c0 + ck * 4));
-          }
-        }
-        uint32_t r[32];
-        ptx::tmem_ld_32x32(taddr + ch * 32, r);
-        ptx::tmem_ld_wait();
-        for (int sb2 = 1; sb2 < nsub_e; ++sb2) {                                  // split precision: the other sub-accumulators (RN fp32 adds)
-          uint32_t r2[32];
-          ptx::tmem_ld_32x32(taddr + sb2 * BLOCK_N + ch * 32, r2);
-          ptx::tmem_ld_wait();
-#pragma unroll
-          for (int j = 0; j < 32; ++j) r[j] = __float_as_uint(__uint_as_float(r[j]) + __uint_as_float(r2[j]));
-        }
-        float v[32];
-        const float4* sc4 = reinterpret_cast<const float4*>(s_scale + ch * 32);
-        const float4* sh4 = reinterpret_cast<const float4*>(s_shift + ch * 32);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const float4 sc = sc4[j], sh = sh4[j];
-          v[4 * j + 0] = fmaf(__uint_as_float(r[4 * j + 0]), sc.x, sh.x);
-          v[4 * j + 1] = fmaf(__uint_as_float(r[4 * j + 1]), sc.y, sh.y);
-          v[4 * j + 2] = fmaf(__uint_as_float(r[4 * j + 2]), sc.z, sh.z);
-          v[4 * j + 3] = fmaf(__uint_as_float(r[4 * j + 3]), sc.w, sh.w);
-        }
-        if (!coalesced_res) {
-          if (rrow) {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) if (c0 + j < a.Cout) v[j] += __ldg(rrow + c0 + j);
-          }
-          if (a.act == ACT_RELU) {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) v[j] = fmaxf(v[j], 0.f);
-          } else if (a.act == ACT_LEAKY) {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) v[j] = v[j] < 0.f ? v[j] * a.slope : v[j];
-          } else if (a.act == ACT_ELU) {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) v[j] = v[j] < 0.f ? expm1f(v[j]) : v[j];
-          }
-          if (a.round_out) {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) v[j] = ptx::round_tf32(v[j]);
-          }
-        }
-        if (a.sumsq && valid) {
-          float part = 0.f;                                                    // fp32 within a 32-element chunk, fp64 across chunks
-#pragma unroll
-          for (int j = 0; j < 32; ++j) if (c0 + j < a.Cout) part = fmaf(v[j], v[j], part);
-          sq_acc += (double)part;
-        }
-        if (a.no_store) continue;
-        if (a.res_prefetch == 2) {                                             // CTA-uniform: accumulate into the residual slot, store from it
-          uint8_t* rs = slot_ptr(r_slot);
-          ptx::mbar_wait(&rfull[r_slot], r_phase);                             // this chunk's residual box has landed
-          uint8_t* srow = rs + row * 128;
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            float4* sp4 = reinterpret_cast<float4*>(srow + ((j ^ (row & 7)) << 4));
-            float4 o = *sp4;
-            o.x += v[4 * j]; o.y += v[4 * j + 1]; o.z += v[4 * j + 2]; o.w += v[4 * j + 3];
-            if (a.act == ACT_RELU) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); o.z = fmaxf(o.z, 0.f); o.w = fmaxf(o.w, 0.f); }
-            else if (a.act == ACT_LEAKY) {
-              o.x = o.x < 0.f ? o.x * a.slope : o.x; o.y = o.y < 0.f ? o.y * a.slope : o.y;
-              o.z = o.z < 0.f ? o.z * a.slope : o.z; o.w = o.w < 0.f ? o.w * a.slope : o.w;
-            }
-            if (a.round_out) { o.x = ptx::round_tf32(o.x); o.y = ptx::round_tf32(o.y); o.z = ptx::round_tf32(o.z); o.w = ptx::round_tf32(o.w); }
-            *sp4 = o;
-          }
-          ptx::fence_proxy_async();
-          ptx::named_bar_sync(1 + group, 128);
-          if (is_store_leader) {
-            ptx::tma_store_4d(&tmap_y, rs, c0, tx * a.BW, ty * a.BH, img);
-            ptx::bulk_commit();
-            if (prev_slot >= 0 && p_tile < total_tiles) {
-              ptx::bulk_wait_read<1>();                                        // the store committed one chunk ago has read its slot: refill it
-              issue_residual(p_tile, p_ch, prev_slot); p_ch += 2; seek(p_tile, p_ch);
-            }
-          }
-          prev_slot = r_slot;
-          if (++r_slot == kResSlots + 1) { r_slot = 0; r_phase ^= 1; }
-          continue;
-        }
-        if (a.tma_store) {
-          // stage the chunk in shared memory (128B-swizzled rows) and let the TMA engine write the BH x BW x 32 box:
-          // fully coalesced, asynchronous, and pixels / channels outside the tensor are clipped by the hardware.
-          if (is_store_leader) ptx::bulk_wait_read<0>();                       // this group's previous store has read the buffer
-          ptx::named_bar_sync(1 + group, 128);
-          uint8_t* srow = stg + row * 128;
-#pragma unroll
-          for (int j = 0; j < 8; ++j)
-            *reinterpret_cast<float4*>(srow + ((j ^ (row & 7)) << 4)) = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-          if (coalesced_res) {
-            // residual add + activation on the staged tile (residual registers were loaded coalesced above)
-            ptx::named_bar_sync(1 + group, 128);
-            if (a.res_prefetch) {
-              ptx::mbar_wait(&rfull[r_slot], r_phase);                          // this chunk's residual box has landed
-              const uint8_t* rs = ring + r_slot * C::kOutStageBytes;
-#pragma unroll
-              for (int i = 0; i < 8; ++i) {
-                const int rr = i * 16 + (gt >> 3);
-                q[i] = *reinterpret_cast<const float4*>(rs + rr * 128 + ((ck ^ (rr & 7)) << 4));
-              }
-            }
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              const int rr = i * 16 + (gt >> 3);
-              float4* sp = reinterpret_cast<float4*>(stg + rr * 128 + ((ck ^ (rr & 7)) << 4));
-              float4 o = *sp;
-              o.x += q[i].x; o.y += q[i].y; o.z += q[i].z; o.w += q[i].w;
-              if (a.act == ACT_RELU) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); o.z = fmaxf(o.z, 0.f); o.w = fmaxf(o.w, 0.f); }
-              else if (a.act == ACT_LEAKY) {
-                o.x = o.x < 0.f ? o.x * a.slope : o.x; o.y = o.y < 0.f ? o.y * a.slope : o.y;
-                o.z = o.z < 0.f ? o.z * a.slope : o.z; o.w = o.w < 0.f ? o.w * a.slope : o.w;
-              }
-              if (a.round_out) { o.x = ptx::round_tf32(o.x); o.y = ptx::round_tf32(o.y); o.z = ptx::round_tf32(o.z); o.w = ptx::round_tf32(o.w); }
-              *sp = o;
-            }
-          }
-          ptx::fence_proxy_async();
-          ptx::named_bar_sync(1 + group, 128);
-          if (is_store_leader) {
-            ptx::tma_store_4d(&tmap_y, stg, c0, tx * a.BW, ty * a.BH, img);
-            ptx::bulk_commit();
-          }
-          if (a.res_prefetch) {
-            // every thread of the group has read the slot (barrier above, after its proxy fence): refill it
-            if (is_store_leader && p_tile < total_tiles) { issue_residual(p_tile, p_ch, r_slot); p_ch += 2; seek(p_tile, p_ch); }
-            if (++r_slot == kResSlots) { r_slot = 0; r_phase ^= 1; }
-          }
-        } else if (valid) {
-#pragma unroll
-          for (int j = 0; j < 32; j += 4) {
-            const int c = c0 + j;
-            if (a.vec_ok && c + 3 < a.Cout) {
-              *reinterpret_cast<float4*>(yrow + c) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
-            } else {
-#pragma unroll
-              for (int t = 0; t < 4; ++t) if (c + t < a.Cout) yrow[c + t] = v[j + t];
-            }
-          }
-        }
-      }
-      ptx::tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        if constexpr (PAIR == 2) ptx::mbar_arrive_cluster(tmem_empty0 + (uint32_t)acc * 8u);
-        else ptx::mbar_arrive(&tmem_empty[acc]);
-      }
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
     }
-    if (is_store_leader) ptx::bulk_wait<0>();
     if (a.sumsq) {
       for (int o = 16; o > 0; o >>= 1) sq_acc += __shfl_xor_sync(0xffffffffu, sq_acc, o);
       if (lane == 0) atomicAdd(a.sumsq, sq_acc);
     }
-  }
-
-  ptx::tc_fence_before();
-  if constexpr (PAIR == 2) ptx::cluster_sync(); else __syncthreads();   // pair: the peer may still read this CTA's smem / signal its barriers
-  if (warp == 1) {
-    ptx::tc_fence_after();
-    if constexpr (PAIR == 2) ptx::tmem_dealloc_2cta<C::kTmemCols>(tmem_base);
-    else ptx::tmem_dealloc<C::kTmemCols>(tmem_base);
   }
 }
 
@@ -542,11 +277,9 @@ EncodeIm2colFn get_encode_im2col() {
   return fn;
 }
 int g_conv_im2col = 1;
-int g_res_prefetch = 2;             // 0: residual read by the epilogue warps; 1: TMA ring + staged add; 2: TMA ring, add in place, store from the slot
 int g_tile_order = 0;             // 0 front-to-back, 1 back-to-front, 2 alternate per launch
 int g_tile_flip = 0;
 int g_k_order = 0;                // 0: by working set (channel chunks outermost when Cin >= 2048); 1: taps outermost; 2: chunks outermost
-int g_cta_pairs = 1;              // 0: never; 1: cta_group::2 pairs where they measured faster; 2|3: wherever they are possible
 
 EncodeTiledFn get_encode_tiled() {
   static EncodeTiledFn fn = nullptr;
@@ -564,10 +297,10 @@ EncodeTiledFn get_encode_tiled() {
 
 
 bool encode(CUtensorMap* m, int rank, const void* base, const cuuint64_t* dims, const cuuint64_t* strides_bytes,
-            const cuuint32_t* box, const cuuint32_t* estr, const char* who, bool is_output = false) {
+            const cuuint32_t* box, const cuuint32_t* estr, const char* who) {
   EncodeTiledFn fn = get_encode_tiled();
   if (!fn) { set_error_msg(who, "cuTensorMapEncodeTiled unavailable (no CUDA driver)"); return false; }
-  CUresult r = fn(m, (g_tf32_tma_type && !is_output) ? CU_TENSOR_MAP_DATA_TYPE_TFLOAT32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, (cuuint32_t)rank,
+  CUresult r = fn(m, g_tf32_tma_type ? CU_TENSOR_MAP_DATA_TYPE_TFLOAT32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, (cuuint32_t)rank,
                   const_cast<void*>(base), dims, strides_bytes, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
@@ -589,55 +322,31 @@ void pick_rect(int OH, int OW, int stride, int* BH, int* BW) {
   }
 }
 
-template <int BLOCK_N, int PAIR>
-int launch(const CUtensorMap& tx, const CUtensorMap& tw, const CUtensorMap& ty, const CUtensorMap& tx2, const CUtensorMap& tw2,
-           const CUtensorMap& tr, const ConvArgs& a_in, cudaStream_t st) {
-  using C = Cfg<BLOCK_N, PAIR>;
+template <int BLOCK_N, bool SPLIT>
+int launch(const CUtensorMap& tx, const CUtensorMap& tw, const CUtensorMap& tx2, const CUtensorMap& tw2, const ConvArgs& a_in, cudaStream_t st) {
+  using C = Cfg<BLOCK_N, SPLIT>;
   ConvArgs a = a_in;
-  // residual epilogues are HBM-bound: trade A/B pipeline depth for the residual TMA ring (2 groups x kResSlots x 16 KB)
-  constexpr int kRingBytes = 2 * kResSlots * C::kOutStageBytes;
-  constexpr int kFreed = (kRingBytes + C::kStageBytes - 1) / C::kStageBytes;
-  // (split precision keeps every stage for its double-size {hi, lo} tiles: a fused residual is then read coalesced by the epilogue warps)
-  a.res_prefetch = ((a.residual != nullptr) && a.tma_store && a.vec_ok && g_res_prefetch && (C::kStages - kFreed >= 2) && a.passes != 3)
-                       ? (g_res_prefetch == 2 ? 2 : 1) : 0;
-  a.nstages = a.res_prefetch ? C::kStages - kFreed : C::kStages;
-  if (a.passes == 3) a.nstages = C::kStages / 2;                 // split precision: double-size stages holding the hi and lo tiles
+  a.nstages = C::kStages;
   static bool attr = false;
   if (!attr) {
-    cudaError_t e = cudaFuncSetAttribute(conv_fwd_sm100_kernel<BLOCK_N, PAIR>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::kSmemBytes);
+    cudaError_t e = cudaFuncSetAttribute(conv_fwd_sm90_kernel<BLOCK_N, SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::kSmemBytes);
     if (e != cudaSuccess) { set_error("skd_conv2d_fwd_sm100(attr)", e); return 0; }
     attr = true;
   }
-  if constexpr (PAIR == 2) {
-    // one cluster of two CTAs (the two SMs of a TPC) per 256-pixel tile; persistent over at most kNumSMs / 2 pairs
-    int pairs = ((a.m_tiles + 1) / 2) * a.n_tiles * a.splits;
-    if (pairs > kNumSMs / 2) pairs = kNumSMs / 2;
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(2 * pairs); cfg.blockDim = dim3(kThreads); cfg.dynamicSmemBytes = C::kSmemBytes; cfg.stream = st;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeClusterDimension;
-    at[0].val.clusterDim.x = 2; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-    cfg.attrs = at; cfg.numAttrs = 1;
-    cudaError_t e = cudaLaunchKernelEx(&cfg, conv_fwd_sm100_kernel<BLOCK_N, PAIR>, tx, tw, ty, tx2, tw2, tr, a);
-    if (e != cudaSuccess) { set_error("skd_conv2d_fwd_sm100(pair launch)", e); return 0; }
-  } else {
-    int grid = a.m_tiles * a.n_tiles * a.splits;
-    if (grid > kNumSMs) grid = kNumSMs;
-    conv_fwd_sm100_kernel<BLOCK_N, PAIR><<<grid, kThreads, C::kSmemBytes, st>>>(tx, tw, ty, tx2, tw2, tr, a);
-  }
+  int grid = a.m_tiles * a.n_tiles * a.splits;
+  if (grid > kNumSMs) grid = kNumSMs;
+  conv_fwd_sm90_kernel<BLOCK_N, SPLIT><<<grid, kThreads, C::kSmemBytes, st>>>(tx, tw, tx2, tw2, a);
   return finish("skd_conv2d_fwd_sm100");
 }
 
 }  // namespace
 
 extern "C" void skd_set_conv_im2col(int on) { g_conv_im2col = on ? 1 : 0; }
-extern "C" void skd_set_conv_res_prefetch(int mode) { g_res_prefetch = mode < 0 ? 0 : (mode > 2 ? 2 : mode); }
 extern "C" void skd_set_conv_tile_order(int mode) { g_tile_order = mode; g_tile_flip = 0; }
-extern "C" void skd_set_conv_cta_pairs(int mode) { g_cta_pairs = mode & 3; }
 extern "C" void skd_set_conv_k_order(int mode) { g_k_order = mode; }
 
 // ---- split-K for convolutions with few output tiles and a long K loop (the discriminator: 256 .. 4096 output pixels, K up to 4096) ----
-// Without it a 4x8-pixel map at batch 8 is 2 x 2 tiles: 4 of 148 SMs walk 128 K steps each.  Units = tiles x K ranges fill the
+// Without it a 4x8-pixel map at batch 8 is 2 x 2 tiles: 4 of 132 SMs walk 128 K steps each.  Units = tiles x K ranges fill the
 // machine; the raw partial tiles go to a caller-provided workspace and one elementwise pass adds them in fixed order and applies
 // the epilogue (scale / shift / residual / activation).
 static int plan_splits(long long tiles, int k_iters) {
@@ -684,12 +393,6 @@ static int conv_fwd_impl(int N, int H, int W, int Cin, int Cout, int KH, int KW,
   const int OH = oh_req > 0 ? oh_req : (H + 2 * pad - dil * (KH - 1) - 1) / stride + 1;
   const int OW = ow_req > 0 ? ow_req : (W + 2 * pad - dil * (KW - 1) - 1) / stride + 1;
   if (OH <= 0 || OW <= 0 || N <= 0) return 1;
-  // small channel counts, 3x3 / stride 1 / pad 1, dense output, no residual: one halo tile per channel chunk feeds all nine taps
-  // (conv_halo_sm100.cu) instead of nine L2 -> shared-memory passes over the activations
-  if (KH == 3 && KW == 3 && stride == 1 && pad == 1 && dil == 1 && !residual && !sumsq && !no_store && oh_req <= 0 && ow_req <= 0 &&
-      y_row == (long long)OW * ldy && y_img == (long long)OH * OW * ldy && (x_lo == nullptr) == (w_lo == nullptr) &&
-      conv3x3_halo_supported(Cin, Cout, (x_lo && w_lo) ? 3 : 1))
-    return conv3x3_halo_launch(N, H, W, Cin, Cout, x, x_lo, ldx, w, w_lo, y, ldy, scale, shift, act, slope, round_tf32, st);
   ConvArgs a;
   a.Cout = Cout; a.Cin = Cin; a.KH = KH; a.KW = KW; a.stride = stride; a.pad = pad; a.dil = dil;
   a.rOH = OH; a.rOW = OW; a.im2col = 0;
@@ -698,7 +401,7 @@ static int conv_fwd_impl(int N, int H, int W, int Cin, int Cout, int KH, int KW,
   //   im2col : TMA im2col mode walks 128 consecutive OUTPUT pixels across rows and images (halo = hardware zero fill);
   //   rect   : BH x BW rectangles of one image through the tiled TMA mode (ragged edges waste up to ~19% at 65x129).
   // output addressed as y[n*y_img + oy*y_row + ox*ldy + c]; anything but the dense NHWC strides (e.g. an every-other-pixel
-  // sub-grid written by the strided data-gradient) forces rectangular tiles + TMA store
+  // sub-grid written by the strided data-gradient) forces rectangular tiles
   const bool strided_out = (y_row != (long long)OW * ldy) || (y_img != (long long)OH * y_row);
   const bool flat = !strided_out && (KH == 1 && KW == 1 && stride == 1 && pad == 0);
   const long long P = (long long)N * OH * OW;
@@ -718,18 +421,12 @@ static int conv_fwd_impl(int N, int H, int W, int Cin, int Cout, int KH, int KW,
   a.k_chunks = (Cin + kBlockK - 1) / kBlockK;
   a.y = y; a.ldy = ldy; a.scale = scale; a.shift = shift; a.residual = residual; a.ldr = ldr;
   a.act = act; a.slope = slope; a.round_out = round_tf32;
-  a.vec_ok = (ldy % 4 == 0) && !(reinterpret_cast<uintptr_t>(y) & 15) &&
-             (!residual || ((ldr % 4 == 0) && !(reinterpret_cast<uintptr_t>(residual) & 15)));
-  const int bn = Cout > 128 ? 256 : (Cout > 64 ? 128 : (Cout > 32 ? 64 : 32));
+  a.y_row = strided_out ? y_row : (long long)a.OW * ldy; a.y_img = strided_out ? y_img : (long long)a.OH * a.OW * ldy;
+  // N tile: at most 128 channels, so that a consumer thread's fragment (64 fp32, 128 with the split-precision running total) stays in
+  // registers
+  const int bn = Cout > 64 ? 128 : (Cout > 32 ? 64 : 32);
   a.n_tiles = (Cout + bn - 1) / bn;
-  // CTA pairs (measured, tools/pair_bench.py): +5-11% on the 256-wide non-residual tiles; with a fused residual only when the K loop
-  // is long enough (>= 16 chunks) that the two A/B stages the residual ring leaves a single CTA become the limiter
-  // (64- and 128-wide pair tiles exist for completeness / tests: the student's Cin = 64 convolutions measured identical either way --
-  //  they are bound by the 9x re-read of the activations through L2, ~6.5 TB/s aggregate; DESIGN.md "what limits what")
-  const bool pair_ok = bn >= 64 && a.m_tiles >= 2;
   const bool kc_outer = (g_k_order == 2) || (g_k_order == 0 && KH * KW > 1 && Cin >= 2048);
-  const bool auto_pair = bn == 256 && !kc_outer && (!residual || Cin * KH * KW >= 512);
-  bool pair = pair_ok && ((g_cta_pairs & 2) ? true : (g_cta_pairs & 1) ? auto_pair : false);
   // split-K: flat / im2col tile modes only, channel counts and pitches that are whole float4s, a workspace from the caller
   a.splits = 1; a.k_per_split = KH * KW * a.k_chunks; a.split_stride = 0;
   const int ldw = (Cout + 3) / 4 * 4;
@@ -740,10 +437,9 @@ static int conv_fwd_impl(int N, int H, int W, int Cin, int Cout, int KH, int KW,
     splits = plan_splits((long long)a.m_tiles * a.n_tiles, KH * KW * a.k_chunks);
   if (splits > 1 && (long long)splits * P * ldw > split_ws_floats) splits = 1;
   if (splits > 1) {
-    pair = false;
     a.splits = splits; a.k_per_split = (KH * KW * a.k_chunks + splits - 1) / splits; a.split_stride = P * ldw;
-    a.y = split_ws; a.ldy = ldw; a.scale = nullptr; a.shift = nullptr; a.residual = nullptr; a.ldr = 0; a.act = 0; a.round_out = 0;
-    a.vec_ok = 1;
+    a.y = split_ws; a.ldy = ldw; a.y_row = (long long)a.OW * ldw; a.y_img = (long long)a.OH * a.OW * ldw;
+    a.scale = nullptr; a.shift = nullptr; a.residual = nullptr; a.ldr = 0; a.act = 0; a.round_out = 0;
   }
 
   CUtensorMap tx, tw, tx2, tw2;
@@ -770,51 +466,26 @@ static int conv_fwd_impl(int N, int H, int W, int Cin, int Cout, int KH, int KW,
   auto encode_w = [&](CUtensorMap* m, const float* ptr) -> bool {
     cuuint64_t dims[3] = {(cuuint64_t)Cin, (cuuint64_t)(KH * KW), (cuuint64_t)Cout};
     cuuint64_t strides[2] = {(cuuint64_t)Cin * 4, (cuuint64_t)KH * KW * Cin * 4};
-    cuuint32_t box[3] = {(cuuint32_t)kBlockK, 1, (cuuint32_t)(pair ? bn / 2 : bn)};     // pair mode: each CTA stages half the rows
+    cuuint32_t box[3] = {(cuuint32_t)kBlockK, 1, (cuuint32_t)bn};
     cuuint32_t estr[3] = {1, 1, 1};
     return encode(m, 3, ptr, dims, strides, box, estr, who);
   };
   if (!encode_x(&tx, x) || !encode_w(&tw, w)) return 0;
-  tx2 = tx; tw2 = tw; a.passes = 1;
-  if (x_lo && w_lo) {                                          // split-precision operands: three MMAs per K step
+  tx2 = tx; tw2 = tw;
+  const bool split3 = x_lo && w_lo;
+  if (split3) {                                          // split-precision operands: three MMAs per K step
     if ((reinterpret_cast<uintptr_t>(x_lo) | reinterpret_cast<uintptr_t>(w_lo)) & 15) { set_error_msg(who, "x_lo / w_lo not 16-byte aligned"); return 0; }
     if (!encode_x(&tx2, x_lo) || !encode_w(&tw2, w_lo)) return 0;
-    a.passes = 3;
   }
-  CUtensorMap ty = tx;
   a.kc_outer = kc_outer;
   a.reverse = (g_tile_order == 2) ? (g_tile_flip ^= 1) : g_tile_order;
-  a.nstages = 0; a.res_prefetch = 0; a.sumsq = sumsq; a.no_store = no_store;
-  a.tma_store = !no_store && (ldy % 4 == 0) && !(reinterpret_cast<uintptr_t>(y) & 15) && (y_row % 4 == 0) && (y_img % 4 == 0);
-  if (a.splits > 1) a.tma_store = 0;                            // partial tiles: plain row stores into the workspace planes
-  if (strided_out && (!a.tma_store || residual)) { set_error_msg(who, "strided output needs 16-byte aligned strides and no residual"); return 0; }
-  if (a.tma_store) {
-    cuuint64_t dims[4] = {(cuuint64_t)Cout, (cuuint64_t)a.OW, (cuuint64_t)a.OH, (cuuint64_t)a.N};
-    cuuint64_t strides[3] = {(cuuint64_t)ldy * 4, (cuuint64_t)a.OW * ldy * 4, (cuuint64_t)a.OH * a.OW * ldy * 4};
-    if (strided_out) { strides[1] = (cuuint64_t)y_row * 4; strides[2] = (cuuint64_t)y_img * 4; }
-    cuuint32_t box[4] = {32, (cuuint32_t)a.BW, (cuuint32_t)a.BH, 1};
-    cuuint32_t estr[4] = {1, 1, 1, 1};
-    if (!encode(&ty, 4, y, dims, strides, box, estr, who, true)) return 0;
-  }
-  CUtensorMap tr = ty;                                          // residual boxes: same geometry as the output boxes, own pitch
-  if (a.tma_store && residual && a.vec_ok) {
-    cuuint64_t dims[4] = {(cuuint64_t)Cout, (cuuint64_t)a.OW, (cuuint64_t)a.OH, (cuuint64_t)a.N};
-    cuuint64_t strides[3] = {(cuuint64_t)ldr * 4, (cuuint64_t)a.OW * ldr * 4, (cuuint64_t)a.OH * a.OW * ldr * 4};
-    cuuint32_t box[4] = {32, (cuuint32_t)a.BW, (cuuint32_t)a.BH, 1};
-    cuuint32_t estr[4] = {1, 1, 1, 1};
-    if (!encode(&tr, 4, residual, dims, strides, box, estr, who, true)) return 0;      // plain FLOAT32: the residual is not rounded
-  }
-  if (pair) {
-    if (bn == 256) return launch<256, 2>(tx, tw, ty, tx2, tw2, tr, a, st);
-    if (bn == 128) return launch<128, 2>(tx, tw, ty, tx2, tw2, tr, a, st);
-    return launch<64, 2>(tx, tw, ty, tx2, tw2, tr, a, st);
-  }
+  a.nstages = 0; a.sumsq = sumsq; a.no_store = no_store;
+  if (strided_out && residual) { set_error_msg(who, "strided output takes no residual"); return 0; }
   int ok;
   switch (bn) {
-    case 256: ok = launch<256, 1>(tx, tw, ty, tx2, tw2, tr, a, st); break;
-    case 128: ok = launch<128, 1>(tx, tw, ty, tx2, tw2, tr, a, st); break;
-    case 64: ok = launch<64, 1>(tx, tw, ty, tx2, tw2, tr, a, st); break;
-    default: ok = launch<32, 1>(tx, tw, ty, tx2, tw2, tr, a, st); break;
+    case 128: ok = split3 ? launch<128, true>(tx, tw, tx2, tw2, a, st) : launch<128, false>(tx, tw, tx2, tw2, a, st); break;
+    case 64: ok = split3 ? launch<64, true>(tx, tw, tx2, tw2, a, st) : launch<64, false>(tx, tw, tx2, tw2, a, st); break;
+    default: ok = split3 ? launch<32, true>(tx, tw, tx2, tw2, a, st) : launch<32, false>(tx, tw, tx2, tw2, a, st); break;
   }
   if (!ok || a.splits == 1) return ok;
   const long long tot4 = P * (Cout / 4);
@@ -849,8 +520,8 @@ extern "C" int skd_gemm_nt_sm100(int M, int Ncols, int K, const float* A, int ld
 }
 
 // Split-precision ("3xTF32") forward: x = x_hi + x_lo, w = w_hi + w_lo (each part exactly representable in TF32); the kernel
-// accumulates x_hi*w_hi + x_lo*w_hi + x_hi*w_lo in the same TMEM accumulator -> fp32-grade result at 3x the tensor work.
-// Used for the student's stem and layer1, where train-mode BN amplifies operand rounding the most (DESIGN.md "TF32 and parity").
+// accumulates x_hi*w_hi + x_lo*w_hi + x_hi*w_lo per K step and adds the steps with fp32 adds -> fp32-grade result at 3x the tensor work.
+// Used for the student's stem, layer1 and layer2, where train-mode BN amplifies operand rounding the most (DESIGN.md "TF32 and parity").
 extern "C" int skd_conv2d_fwd_sm100_3xtf32(int N, int H, int W, int Cin, int Cout, int KH, int KW, int stride, int pad, int dil,
                                            const float* x_hi, const float* x_lo, int ldx, const float* w_hi, const float* w_lo,
                                            float* y, int ldy, const float* scale, const float* shift, int act, float slope,
@@ -881,7 +552,7 @@ extern "C" long long skd_conv2d_fwd_sm100_splitk_workspace_floats(int N, int H, 
   const int OW = out_w > 0 ? out_w : (W + 2 * pad - dil * (KW - 1) - 1) / stride + 1;
   if (OH <= 0 || OW <= 0 || N <= 0 || Cout % 4) return 0;
   const long long P = (long long)N * OH * OW;
-  const int bn = Cout > 128 ? 256 : (Cout > 64 ? 128 : (Cout > 32 ? 64 : 32));
+  const int bn = Cout > 64 ? 128 : (Cout > 32 ? 64 : 32);
   const long long tiles = ((P + kBlockM - 1) / kBlockM) * ((Cout + bn - 1) / bn);
   const int splits = plan_splits(tiles, KH * KW * ((Cin + kBlockK - 1) / kBlockK));
   return splits > 1 ? (long long)splits * P * Cout : 0;

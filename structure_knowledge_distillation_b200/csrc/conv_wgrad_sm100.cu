@@ -1,27 +1,30 @@
-// tcgen05 weight-gradient convolution for sm_100a (cuDNN wgrad in the reference, reached through autograd of every
+// wgmma weight-gradient convolution for sm_90a (cuDNN wgrad in the reference, reached through autograd of every
 // nn.Conv2d of the student: networks/kd_model.py:150 G_loss.backward()).
 //
 //   dW[co][tap][ci] = sum_{pixels p} dY[p][co] * X[p shifted by tap][ci]
 //
-// GEMM view: M = Cout (128 per tile), N = Cin (<=256 per tile, one filter tap per tile), K = pixels.  Both operands are
-// read exactly as they lie in HBM (NHWC: channels contiguous), i.e. as MN-major UMMA operands: per pipeline stage a
-// K-block is a BHk x BWk rectangle of 32 pixels; TMA drops 32-channel x 32-pixel boxes (128B-swizzled, 4 KB each) side
-// by side, and 4 tcgen05.mma.kind::tf32 (K=8 pixels each) consume them.  Split-K over pixel blocks gives >= 2 waves of
-// work units; fp32 partials go to a workspace and a deterministic reduction adds them in fixed order.
+// GEMM view: M = Cout (128 per tile), N = Cin (<= 128 per tile, one filter tap per tile), K = pixels.  Both operands lie in HBM with
+// the channels contiguous (NHWC), i.e. MN-major, and wgmma takes tf32 operands only K-major.  So per pipeline stage TMA drops
+// 32-channel x 32-pixel boxes (128B-swizzled, one pixel per 128-byte row) of dY and X into a raw stage, the two consumer warpgroups
+// transpose them into K-major 128B-swizzled tiles (one channel per 128-byte row, double-buffered so the transposition of the next
+// K-block overlaps the wgmmas of this one) and release the raw stage at once; each warpgroup then issues 4 x wgmma.m64nNk8.tf32 for
+// its 64 Cout rows.  Split-K over pixel blocks gives >= 2 waves of work units; fp32 partials go to a workspace and a deterministic
+// reduction adds them in fixed order.
 #include <cuda.h>
 
 #include "common.cuh"
 #include "skd.h"
-#include "sm100_ptx.cuh"
+#include "sm90_ptx.cuh"
 
 using namespace skd;
 
 namespace {
 
 constexpr int kBlockM = 128;               // Cout per tile
-// pixels per pipeline stage: 64 for wide channel tiles, 128 for Cin <= 64 (fewer, larger TMA boxes: the producer is box-rate bound)
-__host__ __device__ constexpr int kpix_for(int block_n) { return block_n >= 128 ? 64 : 128; }
-constexpr int kThreads = 192;
+constexpr int kKPix = 32;                  // pixels per pipeline stage (one 128-byte K row of the transposed tiles)
+constexpr int kThreads = 384;              // producer warpgroup + 2 consumer warpgroups
+constexpr int kChunkBytes = 32 * kKPix * 4;        // one 32-channel x 32-pixel box
+constexpr int kMaxStages = 4;
 
 struct WgArgs {
   int N, OH, OW, Cout, Cin, KH, KW, stride, pad, dil;
@@ -29,222 +32,154 @@ struct WgArgs {
   int m_tiles, n_tiles, taps, splits, kb_total, kb_per_split;
   float* ws;                               // [splits][Cout][taps*Cin]
   int linear;                              // K-blocks are 32 consecutive output pixels (dY as a [P][Cout] matrix, X through TMA im2col)
-  // pipeline geometry (run time): with Cout <= 64 the dY operand needs two of its four 32-channel chunks, the stage shrinks and a
-  // third / fourth stage fits (the M = 128 MMA then reads x data as rows 64..127 of A: finite garbage in accumulator rows nobody stores)
-  int a_bytes, stage_bytes, nstages;
 };
-constexpr int kMaxStages = 4;
 
-// PAIR = 2: a cluster of two CTAs (cta_group::2) owns a 256 (Cout) x BLOCK_N (Cin) tile: each CTA stages its own 128 Cout rows of dY
-// and only HALF of the x tile (BLOCK_N / 2 channels), the leader issues M = 256 MMAs.  Per 128 x BLOCK_N of MMA work a CTA then moves
-// 8 TMA boxes instead of 12 (BLOCK_N = 256) -- the producer's box rate, not the tensor pipe, bounded the single-CTA kernel (ncu:
-// tensor pipe 59 % of active cycles on 512 -> 512) -- and the freed shared memory gives a third pipeline stage.
-template <int BLOCK_N, int PAIR = 1>
+template <int BLOCK_N>
 struct WCfg {
-  static constexpr int kKPix = kpix_for(BLOCK_N);
-  static constexpr int kChunkBytes = 32 * kKPix * 4;                 // one 32-channel x kKPix-pixel box
   static constexpr int kABytes = 4 * kChunkBytes;                    // 128 co
-  static constexpr int kBBytes = (BLOCK_N / 32 / PAIR) * kChunkBytes;
-  static constexpr int kStageBytes = kABytes + kBBytes;
-  static constexpr int kStages = (PAIR == 2) ? 3 : ((BLOCK_N >= 256) ? 2 : (BLOCK_N >= 128 ? 3 : 2));
-  static constexpr int kTmemCols = 2 * BLOCK_N;
-  static constexpr int kSmemBytes = kStages * kStageBytes + 1024 + 256;
+  static constexpr int kBBytes = (BLOCK_N / 32) * kChunkBytes;
+  static constexpr int kStageBytes = kABytes + kBBytes;              // raw (pixel-major) stage; the transposed set has the same size
+  static constexpr int kFit = (232448 - 2 * kStageBytes - 1024 - 256) / kStageBytes;
+  static constexpr int kStages = kFit > kMaxStages ? kMaxStages : kFit;
+  static constexpr int kSmemBytes = (kStages + 2) * kStageBytes + 1024 + 256;
+  static_assert(kStages >= 2, "at least two pipeline stages");
 };
 
-template <int BLOCK_N, int PAIR>
+// raw box (pixel rows of 32 channels, 128B swizzle) -> K-major tile (channel rows of 32 pixels, 128B swizzle); unit = 4 pixels x 4 channels
+__device__ __forceinline__ void transpose_tile(const uint8_t* raw, uint8_t* dst, int rows, int t) {
+  for (int u = t; u < rows * 2; u += 256) {
+    const int pg = u & 7, cg = u >> 3;
+    const uint8_t* src = raw + (cg >> 3) * kChunkBytes;
+    float4 r[4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const int p = 4 * pg + i;
+      r[i] = *reinterpret_cast<const float4*>(src + p * 128 + ((((cg & 7) ^ (p & 7))) << 4));
+    }
+    const int c = 4 * cg;
+    *reinterpret_cast<float4*>(dst + (c + 0) * 128 + ((pg ^ ((c + 0) & 7)) << 4)) = make_float4(r[0].x, r[1].x, r[2].x, r[3].x);
+    *reinterpret_cast<float4*>(dst + (c + 1) * 128 + ((pg ^ ((c + 1) & 7)) << 4)) = make_float4(r[0].y, r[1].y, r[2].y, r[3].y);
+    *reinterpret_cast<float4*>(dst + (c + 2) * 128 + ((pg ^ ((c + 2) & 7)) << 4)) = make_float4(r[0].z, r[1].z, r[2].z, r[3].z);
+    *reinterpret_cast<float4*>(dst + (c + 3) * 128 + ((pg ^ ((c + 3) & 7)) << 4)) = make_float4(r[0].w, r[1].w, r[2].w, r[3].w);
+  }
+}
+
+template <int BLOCK_N>
 __global__ void __launch_bounds__(kThreads, 1)
-conv_wgrad_sm100_kernel(const __grid_constant__ CUtensorMap tmap_dy, const __grid_constant__ CUtensorMap tmap_x, const WgArgs a) {
-  using C = WCfg<BLOCK_N, PAIR>;
+conv_wgrad_sm90_kernel(const __grid_constant__ CUtensorMap tmap_dy, const __grid_constant__ CUtensorMap tmap_x, const WgArgs a) {
+  using C = WCfg<BLOCK_N>;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   // keep the pointer in the shared address space (integer round trips make nvcc emit generic LD/ST instead of LDS/STS)
   const uint32_t raw_addr = ptx::smem_u32(smem_raw);
   uint8_t* smem = smem_raw + (((raw_addr + 1023u) & ~1023u) - raw_addr);
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + C::kStages * C::kStageBytes);
+  uint8_t* sets = smem + C::kStages * C::kStageBytes;                // 2 transposed {A, B} sets
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(sets + 2 * C::kStageBytes);
   uint64_t* empty_bar = full_bar + kMaxStages;
-  uint64_t* tmem_full = empty_bar + kMaxStages;
-  uint64_t* tmem_empty = tmem_full + 2;
-  uint32_t* tmem_base_slot = reinterpret_cast<uint32_t*>(tmem_empty + 2);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t cta_rank = (PAIR == 2) ? ptx::cluster_ctarank() : 0u;
-  const int unit0 = (PAIR == 2) ? (int)(blockIdx.x >> 1) : (int)blockIdx.x;
-  const int unit_step = (PAIR == 2) ? (int)(gridDim.x >> 1) : (int)gridDim.x;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     ptx::prefetch_tmap(&tmap_dy); ptx::prefetch_tmap(&tmap_x);
-    for (int s = 0; s < a.nstages; ++s) { ptx::mbar_init(&full_bar[s], 1); ptx::mbar_init(&empty_bar[s], 1); }
-    for (int s = 0; s < 2; ++s) { ptx::mbar_init(&tmem_full[s], 1); ptx::mbar_init(&tmem_empty[s], 4 * PAIR); }
+    for (int s = 0; s < C::kStages; ++s) { ptx::mbar_init(&full_bar[s], 1); ptx::mbar_init(&empty_bar[s], 1); }
     ptx::fence_barrier_init();
   }
-  if (warp == 1) {
-    if constexpr (PAIR == 2) ptx::tmem_alloc_2cta<C::kTmemCols>(tmem_base_slot);
-    else ptx::tmem_alloc<C::kTmemCols>(tmem_base_slot);
-  }
-  ptx::tc_fence_before();
-  if constexpr (PAIR == 2) ptx::cluster_sync(); else __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem_base = *tmem_base_slot;
+  __syncthreads();
 
-  const int m_units = a.m_tiles / PAIR;                    // pair mode: a tile is two consecutive 128-row Cout tiles (Cout % 256 == 0)
-  const int tiles = m_units * a.taps * a.n_tiles;
+  const int tiles = a.m_tiles * a.taps * a.n_tiles;
   const int units = tiles * a.splits;
   const int kb_per_img = a.kb_x * a.kb_y;
 
-  if (warp == 0) {
+  if (warp < 4) {
     // ===================== TMA producer =====================
-    // TMA sustains roughly one box per ~100 cycles per SM whatever its size, so boxes are made as large as the MN-major
-    // swizzle allows (32 channels x 64 pixels = 8 KB) and all-out-of-range channel chunks (Cout or Cin < tile) are not issued.
-    if (lane == 0) {
+    // all-out-of-range channel chunks (Cout or Cin < tile) are not issued
+    if (threadIdx.x == 0) {
       int stage = 0; uint32_t phase = 0;
-      const uint32_t full_bar0 = (PAIR == 2) ? ptx::mapa_shared(&full_bar[0], 0) : 0u;   // the leader's full barriers
-      for (int u = unit0; u < units; u += unit_step) {
+      for (int u = blockIdx.x; u < units; u += gridDim.x) {
         const int split = u / tiles, tile = u - split * tiles;
-        const int mu = tile / (a.taps * a.n_tiles), r = tile - mu * (a.taps * a.n_tiles);
-        const int mt = (PAIR == 2) ? 2 * mu + (int)cta_rank : mu;
+        const int mt = tile / (a.taps * a.n_tiles), r = tile - mt * (a.taps * a.n_tiles);
         const int tap = r / a.n_tiles, nt = r - tap * a.n_tiles;
         const int kh = tap / a.KW, kw = tap - kh * a.KW;
         const int kb0 = split * a.kb_per_split;
         const int kb1 = min(a.kb_total, kb0 + a.kb_per_split);
         const int a_chunks = min(4, (a.Cout - mt * kBlockM + 31) / 32);
-        // pair mode: this CTA stages channels [nt * BLOCK_N + rank * BLOCK_N / 2, +BLOCK_N / 2) of x
-        const int n0 = nt * BLOCK_N + (int)cta_rank * (BLOCK_N / PAIR);
-        const int b_chunks = max(0, min(BLOCK_N / 32 / PAIR, (a.Cin - n0 + 31) / 32));
+        const int b_chunks = max(0, min(BLOCK_N / 32, (a.Cin - nt * BLOCK_N + 31) / 32));
         for (int kb = kb0; kb < kb1; ++kb) {
           ptx::mbar_wait(&empty_bar[stage], phase ^ 1);
-          uint8_t* sa = smem + stage * a.stage_bytes;
-          uint8_t* sb = sa + a.a_bytes;
-          if constexpr (PAIR == 2) {
-            // both CTAs' boxes complete on the LEADER's barrier, which expects the bytes of both (the peer's chunk counts are its own:
-            // Cout % 256 == 0 makes a_chunks 4 in both; the peer's share of x may be ragged)
-            if (cta_rank == 0) {
-              const int peer_b = max(0, min(BLOCK_N / 64, (a.Cin - (nt * BLOCK_N + BLOCK_N / 2) + 31) / 32));
-              ptx::mbar_expect_tx(&full_bar[stage], (uint32_t)((2 * a_chunks + b_chunks + peer_b) * C::kChunkBytes));
-            }
-            const uint32_t fb = full_bar0 + (uint32_t)stage * 8u;
-            const int p0 = kb * C::kKPix;
-            const int img = p0 / (a.OH * a.OW), r2 = p0 - img * (a.OH * a.OW);
-            const int oy = r2 / a.OW, ox = r2 - oy * a.OW;
-            for (int c = 0; c < a_chunks; ++c)
-              ptx::tma_load_4d_2cta(sa + c * C::kChunkBytes, &tmap_dy, fb, mt * kBlockM + c * 32, p0, 0, 0);
-            for (int c = 0; c < b_chunks; ++c)
-              ptx::tma_load_im2col_4d_2cta(sb + c * C::kChunkBytes, &tmap_x, fb, n0 + c * 32, ox * a.stride - a.pad, oy * a.stride - a.pad, img,
-                                           (uint16_t)(kw * a.dil), (uint16_t)(kh * a.dil));
-            if (++stage == a.nstages) { stage = 0; phase ^= 1; }
-            continue;
-          }
-          ptx::mbar_expect_tx(&full_bar[stage], (uint32_t)((a_chunks + b_chunks) * C::kChunkBytes));
+          uint8_t* sa = smem + stage * C::kStageBytes;
+          uint8_t* sb = sa + C::kABytes;
+          ptx::mbar_expect_tx(&full_bar[stage], (uint32_t)((a_chunks + b_chunks) * kChunkBytes));
           if (a.linear) {
-            const int p0 = kb * C::kKPix;
+            const int p0 = kb * kKPix;
             const int img = p0 / (a.OH * a.OW), r2 = p0 - img * (a.OH * a.OW);
             const int oy = r2 / a.OW, ox = r2 - oy * a.OW;
             for (int c = 0; c < a_chunks; ++c)
-              ptx::tma_load_4d(sa + c * C::kChunkBytes, &tmap_dy, &full_bar[stage], mt * kBlockM + c * 32, p0, 0, 0);
+              ptx::tma_load_4d(sa + c * kChunkBytes, &tmap_dy, &full_bar[stage], mt * kBlockM + c * 32, p0, 0, 0);
             for (int c = 0; c < b_chunks; ++c)
-              ptx::tma_load_im2col_4d(sb + c * C::kChunkBytes, &tmap_x, &full_bar[stage], nt * BLOCK_N + c * 32, ox * a.stride - a.pad,
+              ptx::tma_load_im2col_4d(sb + c * kChunkBytes, &tmap_x, &full_bar[stage], nt * BLOCK_N + c * 32, ox * a.stride - a.pad,
                                       oy * a.stride - a.pad, img, (uint16_t)(kw * a.dil), (uint16_t)(kh * a.dil));
           } else {
             const int img = kb / kb_per_img, q = kb - img * kb_per_img;
             const int by = q / a.kb_x, bx = q - by * a.kb_x;
             const int oy0 = by * a.BHk, ox0 = bx * a.BWk;
             for (int c = 0; c < a_chunks; ++c)
-              ptx::tma_load_4d(sa + c * C::kChunkBytes, &tmap_dy, &full_bar[stage], mt * kBlockM + c * 32, ox0, oy0, img);
+              ptx::tma_load_4d(sa + c * kChunkBytes, &tmap_dy, &full_bar[stage], mt * kBlockM + c * 32, ox0, oy0, img);
             for (int c = 0; c < b_chunks; ++c)
-              ptx::tma_load_4d(sb + c * C::kChunkBytes, &tmap_x, &full_bar[stage], nt * BLOCK_N + c * 32,
+              ptx::tma_load_4d(sb + c * kChunkBytes, &tmap_x, &full_bar[stage], nt * BLOCK_N + c * 32,
                                ox0 * a.stride - a.pad + kw * a.dil, oy0 * a.stride - a.pad + kh * a.dil, img);
           }
-          if (++stage == a.nstages) { stage = 0; phase ^= 1; }
+          if (++stage == C::kStages) { stage = 0; phase ^= 1; }
         }
       }
-    }
-  } else if (warp == 1) {
-    constexpr uint32_t idesc = ptx::make_idesc_tf32(kBlockM * PAIR, BLOCK_N, 1, 1);     // both operands MN-major
-    int stage = 0; uint32_t phase = 0; int acc = 0; uint32_t acc_phase = 0;
-    for (int u = unit0; u < units && cta_rank == 0; u += unit_step) {
-      const int split = u / tiles, tile = u - split * tiles;
-      const int kb0 = split * a.kb_per_split;
-      const int nkb = min(a.kb_total, kb0 + a.kb_per_split) - kb0;
-      if (lane == 0) ptx::mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-      __syncwarp();
-      ptx::tc_fence_after();
-      const uint32_t tmem_d = tmem_base + (uint32_t)(acc * BLOCK_N);
-      for (int k = 0; k < nkb; ++k) {
-        if (lane == 0) {
-          ptx::mbar_wait(&full_bar[stage], phase);
-          ptx::tc_fence_after();
-          const uint32_t sa = ptx::smem_u32(smem + stage * a.stage_bytes);
-          const uint32_t sb = sa + (uint32_t)a.a_bytes;
-#pragma unroll
-          for (int kk = 0; kk < C::kKPix / 8; ++kk) {
-            // MN-major tf32 must use the 128B swizzle with 32B atoms (UMMA layout type 1 <-> TMA SWIZZLE_128B_ATOM_32B):
-            // LBO = distance between 32-channel chunks, SBO = distance between 4-pixel groups
-            const uint64_t da = ptx::make_smem_desc(sa + kk * 1024, C::kChunkBytes, 512, 1);   // 8 pixels = 1 KB per MMA K step
-            const uint64_t db = ptx::make_smem_desc(sb + kk * 1024, C::kChunkBytes, 512, 1);
-            if constexpr (PAIR == 2) ptx::mma_tf32_2cta(tmem_d, da, db, idesc, (k | kk) != 0 ? 1u : 0u);
-            else ptx::mma_tf32(tmem_d, da, db, idesc, (k | kk) != 0 ? 1u : 0u);
-          }
-          if constexpr (PAIR == 2) {
-            ptx::mma_commit_2cta(&empty_bar[stage]);
-            if (k == nkb - 1) ptx::mma_commit_2cta(&tmem_full[acc]);
-          } else {
-            ptx::mma_commit(&empty_bar[stage]);
-            if (k == nkb - 1) ptx::mma_commit(&tmem_full[acc]);
-          }
-        }
-        __syncwarp();
-        if (++stage == a.nstages) { stage = 0; phase ^= 1; }
-      }
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
     }
   } else {
-    const int quarter = warp & 3;
-    const int row = quarter * 32 + lane;
+    // ===================== consumers =====================
+    const int t = threadIdx.x - 128;                           // 0..255
+    const int g = t >> 7;                                      // warpgroup: Cout rows 64g .. 64g+63 of the tile
+    const int wq = warp & 3;
+    const int r_lo = g * 64 + wq * 16 + (lane >> 2);
+    const int cq = 2 * (lane & 3);
     const size_t kdim = (size_t)a.taps * a.Cin;
-    int acc = 0; uint32_t acc_phase = 0;
-    const uint32_t tmem_empty0 = (PAIR == 2) ? ptx::mapa_shared(&tmem_empty[0], 0) : 0u;   // the leader's tmem_empty barriers
-    for (int u = unit0; u < units; u += unit_step) {
+    float acc[BLOCK_N / 2];
+    int stage = 0; uint32_t phase = 0; uint32_t it = 0;        // it: K-blocks consumed so far (transposed-set parity)
+    for (int u = blockIdx.x; u < units; u += gridDim.x) {
       const int split = u / tiles, tile = u - split * tiles;
-      const int mu = tile / (a.taps * a.n_tiles), r = tile - mu * (a.taps * a.n_tiles);
-      const int mt = (PAIR == 2) ? 2 * mu + (int)cta_rank : mu;
+      const int mt = tile / (a.taps * a.n_tiles), r = tile - mt * (a.taps * a.n_tiles);
       const int tap = r / a.n_tiles, nt = r - tap * a.n_tiles;
-      const int co = mt * kBlockM + row;
-      float* orow = a.ws + ((size_t)split * a.Cout + co) * kdim + (size_t)tap * a.Cin;
-      ptx::mbar_wait(&tmem_full[acc], acc_phase);
-      ptx::tc_fence_after();
-      const uint32_t taddr = tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(acc * BLOCK_N);
-#pragma unroll 1
-      for (int ch = 0; ch < BLOCK_N / 32; ++ch) {
-        uint32_t v[32];
-        ptx::tmem_ld_32x32(taddr + ch * 32, v);
-        ptx::tmem_ld_wait();
-        const int c0 = nt * BLOCK_N + ch * 32;
-        if (co < a.Cout && c0 < a.Cin) {
+      const int kb0 = split * a.kb_per_split;
+      const int nkb = min(a.kb_total, kb0 + a.kb_per_split) - kb0;
+      for (int k = 0; k < nkb; ++k, ++it) {
+        uint8_t* set = sets + (it & 1) * C::kStageBytes;
+        ptx::mbar_wait(&full_bar[stage], phase);
+        ptx::wgmma_wait<1>();                                  // this warpgroup's wgmmas of two K-blocks ago (same set) are done
+        ptx::named_bar_sync(1, 256);                           // ... and the other warpgroup's
+        const uint8_t* raw = smem + stage * C::kStageBytes;
+        transpose_tile(raw, set, kBlockM, t);
+        transpose_tile(raw + C::kABytes, set + C::kABytes, BLOCK_N, t);
+        ptx::fence_proxy_async();                              // generic-proxy writes -> visible to the wgmma (async proxy) reads
+        ptx::named_bar_sync(1, 256);
+        if (t == 0) ptx::mbar_arrive(&empty_bar[stage]);       // raw stage consumed
+        const uint32_t sa = ptx::smem_u32(set) + (uint32_t)(g * 64 * 128);
+        const uint32_t sb = ptx::smem_u32(set) + (uint32_t)C::kABytes;
+        ptx::wgmma_fence();
 #pragma unroll
-          for (int j = 0; j < 32; j += 4) {
-            const int c = c0 + j;
-            if (c + 3 < a.Cin) {
-              *reinterpret_cast<float4*>(orow + c) = make_float4(__uint_as_float(v[j]), __uint_as_float(v[j + 1]),
-                                                                 __uint_as_float(v[j + 2]), __uint_as_float(v[j + 3]));
-            } else {
+        for (int kk = 0; kk < kKPix / 8; ++kk)
+          ptx::wgmma_tf32<BLOCK_N>(acc, ptx::make_wgmma_desc_sw128(sa + kk * 32), ptx::make_wgmma_desc_sw128(sb + kk * 32), (k | kk) != 0 ? 1u : 0u);
+        ptx::wgmma_commit();
+        if (++stage == C::kStages) { stage = 0; phase ^= 1; }
+      }
+      ptx::wgmma_wait<0>();
+      ptx::fence_regs(acc);
 #pragma unroll
-              for (int t = 0; t < 4; ++t) if (c + t < a.Cin) orow[c + t] = __uint_as_float(v[j + t]);
-            }
-          }
+      for (int h = 0; h < 2; ++h) {
+        const int co = mt * kBlockM + r_lo + 8 * h;
+        if (co >= a.Cout) continue;
+        float* orow = a.ws + ((size_t)split * a.Cout + co) * kdim + (size_t)tap * a.Cin;
+#pragma unroll
+        for (int j = 0; j < BLOCK_N / 8; ++j) {
+          const int ci = nt * BLOCK_N + 8 * j + cq;            // even; Cin % 4 == 0, so ci + 1 < Cin too
+          if (ci < a.Cin) *reinterpret_cast<float2*>(orow + ci) = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
         }
       }
-      ptx::tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        if constexpr (PAIR == 2) ptx::mbar_arrive_cluster(tmem_empty0 + (uint32_t)acc * 8u);
-        else ptx::mbar_arrive(&tmem_empty[acc]);
-      }
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
     }
-  }
-  ptx::tc_fence_before();
-  if constexpr (PAIR == 2) ptx::cluster_sync(); else __syncthreads();
-  if (warp == 1) {
-    ptx::tc_fence_after();
-    if constexpr (PAIR == 2) ptx::tmem_dealloc_2cta<C::kTmemCols>(tmem_base);
-    else ptx::tmem_dealloc<C::kTmemCols>(tmem_base);
   }
 }
 
@@ -273,42 +208,31 @@ EncodeTiledFn get_encode() {
   return fn;
 }
 
-struct Plan { int OH, OW, BHk, BWk, kb_x, kb_y, kb_total, bn, m_tiles, n_tiles, taps, splits, kb_per_split, linear, pair; };
+struct Plan { int OH, OW, BHk, BWk, kb_x, kb_y, kb_total, bn, m_tiles, n_tiles, taps, splits, kb_per_split, linear; };
 
 int g_wgrad_linear = 1;
-int g_wgrad_pairs = 1;            // cta_group::2 pairs for 256-wide Cin tiles with Cout % 256 == 0
 
 Plan make_plan(int N, int H, int W, int Cin, int Cout, int KH, int KW, int stride, int pad, int dil) {
   Plan p;
   p.OH = (H + 2 * pad - dil * (KH - 1) - 1) / stride + 1; p.OW = (W + 2 * pad - dil * (KW - 1) - 1) / stride + 1;
-  const int cand[4][2] = {{8, 8}, {4, 16}, {16, 4}, {2, 32}};        // 64-pixel K blocks in the rectangular fallback mode
+  const int cand[4][2] = {{4, 8}, {8, 4}, {2, 16}, {1, 32}};        // 32-pixel K blocks in the rectangular fallback mode
   long long best = -1;
   for (auto& c : cand) {
     const long long t = (long long)((p.OH + c[0] - 1) / c[0]) * ((p.OW + c[1] - 1) / c[1]);
     if (best < 0 || t < best) { best = t; p.BHk = c[0]; p.BWk = c[1]; }
   }
-  p.bn = Cin > 128 ? 256 : (Cin > 64 ? 128 : (Cin > 32 ? 64 : 32));
-  const int kpix = kpix_for(p.bn);
-  if (kpix == 128) {                                              // 128-pixel rectangles in the fallback mode
-    const int cand2[4][2] = {{8, 16}, {4, 32}, {16, 8}, {2, 64}};
-    best = -1;
-    for (auto& c : cand2) {
-      const long long t = (long long)((p.OH + c[0] - 1) / c[0]) * ((p.OW + c[1] - 1) / c[1]);
-      if (best < 0 || t < best) { best = t; p.BHk = c[0]; p.BWk = c[1]; }
-    }
-  }
+  p.bn = Cin > 64 ? 128 : (Cin > 32 ? 64 : 32);
   p.kb_x = (p.OW + p.BWk - 1) / p.BWk; p.kb_y = (p.OH + p.BHk - 1) / p.BHk;
   p.kb_total = N * p.kb_x * p.kb_y;
   const int up_h = pad - (KH - 1) * dil, up_w = pad - (KW - 1) * dil;
   p.linear = g_wgrad_linear && pad <= 128 && up_h >= -128 && up_w >= -128 && stride <= 8 && (long long)N * p.OH * p.OW < (1LL << 31);
-  if (p.linear) p.kb_total = (int)(((long long)N * p.OH * p.OW + kpix - 1) / kpix);
+  if (p.linear) p.kb_total = (int)(((long long)N * p.OH * p.OW + kKPix - 1) / kKPix);
   p.m_tiles = (Cout + kBlockM - 1) / kBlockM; p.n_tiles = (Cin + p.bn - 1) / p.bn; p.taps = KH * KW;
-  p.pair = (g_wgrad_pairs && p.linear && p.bn == 256 && Cout % 256 == 0) ? 1 : 0;
-  const int tiles = (p.m_tiles / (p.pair ? 2 : 1)) * p.n_tiles * p.taps;
-  const int slots = p.pair ? kNumSMs / 2 : kNumSMs;          // persistent CTAs (or CTA pairs)
+  const int tiles = p.m_tiles * p.n_tiles * p.taps;
+  const int slots = kNumSMs;                                 // persistent CTAs
   // split-K: work units = tiles x K ranges over a persistent grid of kNumSMs CTAs.  Pick the split count whose unit count fills
-  // whole waves best (ncu, round 2: 9 tiles x 33 splits = 297 units = 2 waves + ONE unit -> a third round, 34 % of the SM cycles
-  // idle; 72 tiles x 5 = 360 units = 2.4 waves -> 23 % idle), fewer splits on ties (each split writes a partial dW plane)
+  // whole waves best (a unit count just past a whole number of waves leaves
+  // most SMs idle in the last round), fewer splits on ties (each split writes a partial dW plane)
   int cap = p.kb_total / 16; if (cap < 1) cap = 1;          // at least 16 k-blocks per unit
   int hi = (4 * slots + tiles - 1) / tiles; if (hi > cap) hi = cap; if (hi < 1) hi = 1;
   int best_sp = 1; double best_eff = -1.0;
@@ -327,44 +251,23 @@ Plan make_plan(int N, int H, int W, int Cin, int Cout, int KH, int KW, int strid
   return p;
 }
 
-template <int BLOCK_N, int PAIR>
-int launch(const CUtensorMap& tdy, const CUtensorMap& tx, const WgArgs& a_in, int units, cudaStream_t st) {
-  using C = WCfg<BLOCK_N, PAIR>;
-  WgArgs a = a_in;
-  const int a_chunks_max = (PAIR == 2 || a.Cout > 96) ? 4 : (a.Cout > 64 ? 3 : (a.Cout > 32 ? 2 : 1));
-  a.a_bytes = (PAIR == 2) ? C::kABytes : ((a_chunks_max * C::kChunkBytes + 1023) / 1024) * 1024;
-  a.stage_bytes = a.a_bytes + C::kBBytes;
-  a.nstages = (C::kStages * C::kStageBytes) / a.stage_bytes;
-  if (a.nstages > kMaxStages) a.nstages = kMaxStages;
-  // the M = 128 MMA always reads four A chunks: the last stage's must stay inside the data region
-  while (a.nstages > 1 && (a.nstages - 1) * a.stage_bytes + C::kABytes > C::kStages * C::kStageBytes) --a.nstages;
+template <int BLOCK_N>
+int launch(const CUtensorMap& tdy, const CUtensorMap& tx, const WgArgs& a, int units, cudaStream_t st) {
+  using C = WCfg<BLOCK_N>;
   static bool attr = false;
   if (!attr) {
-    cudaError_t e = cudaFuncSetAttribute(conv_wgrad_sm100_kernel<BLOCK_N, PAIR>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::kSmemBytes);
+    cudaError_t e = cudaFuncSetAttribute(conv_wgrad_sm90_kernel<BLOCK_N>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::kSmemBytes);
     if (e != cudaSuccess) { set_error("skd_conv2d_wgrad_sm100(attr)", e); return 0; }
     attr = true;
   }
-  if constexpr (PAIR == 2) {
-    int pairs = units < kNumSMs / 2 ? units : kNumSMs / 2;
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(2 * pairs); cfg.blockDim = dim3(kThreads); cfg.dynamicSmemBytes = C::kSmemBytes; cfg.stream = st;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeClusterDimension;
-    at[0].val.clusterDim.x = 2; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-    cfg.attrs = at; cfg.numAttrs = 1;
-    cudaError_t e = cudaLaunchKernelEx(&cfg, conv_wgrad_sm100_kernel<BLOCK_N, PAIR>, tdy, tx, a);
-    if (e != cudaSuccess) { set_error("skd_conv2d_wgrad_sm100(pair launch)", e); return 0; }
-  } else {
-    const int grid = units < kNumSMs ? units : kNumSMs;
-    conv_wgrad_sm100_kernel<BLOCK_N, PAIR><<<grid, kThreads, C::kSmemBytes, st>>>(tdy, tx, a);
-  }
+  const int grid = units < kNumSMs ? units : kNumSMs;
+  conv_wgrad_sm90_kernel<BLOCK_N><<<grid, kThreads, C::kSmemBytes, st>>>(tdy, tx, a);
   return finish("skd_conv2d_wgrad_sm100");
 }
 
 }  // namespace
 
 extern "C" void skd_set_wgrad_linear(int on) { g_wgrad_linear = on ? 1 : 0; }
-extern "C" void skd_set_wgrad_cta_pairs(int on) { g_wgrad_pairs = on ? 1 : 0; }
 
 extern "C" long long skd_conv2d_wgrad_sm100_workspace_floats(int N, int H, int W, int Cin, int Cout, int KH, int KW, int stride,
                                                              int pad, int dil) {
@@ -402,10 +305,10 @@ extern "C" int skd_conv2d_wgrad_sm100(int N, int H, int W, int Cin, int Cout, in
     {
       cuuint64_t dims[4] = {(cuuint64_t)Cout, (cuuint64_t)P, 1, 1};
       cuuint64_t strides[3] = {(cuuint64_t)ldy * 4, (cuuint64_t)P * ldy * 4, (cuuint64_t)P * ldy * 4};
-      cuuint32_t box[4] = {32, (cuuint32_t)kpix_for(p.bn), 1, 1};
+      cuuint32_t box[4] = {32, (cuuint32_t)kKPix, 1, 1};
       cuuint32_t es[4] = {1, 1, 1, 1};
       CUresult r = enc(&tdy, dt, 4, const_cast<float*>(dy), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                       CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+                       CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
       if (r != CUDA_SUCCESS) { set_error_msg(who, "cuTensorMapEncodeTiled(dy, linear) failed"); return 0; }
     }
     {
@@ -414,8 +317,8 @@ extern "C" int skd_conv2d_wgrad_sm100(int N, int H, int W, int Cin, int Cout, in
       int lower[2] = {-pad, -pad};
       int upper[2] = {pad - (KW - 1) * dil, pad - (KH - 1) * dil};
       cuuint32_t es[4] = {1, (cuuint32_t)stride, (cuuint32_t)stride, 1};
-      CUresult r = enc_i2c(&tx, dt, 4, const_cast<float*>(x), dims, strides, lower, upper, 32, (cuuint32_t)kpix_for(p.bn), es,
-                           CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+      CUresult r = enc_i2c(&tx, dt, 4, const_cast<float*>(x), dims, strides, lower, upper, 32, (cuuint32_t)kKPix, es,
+                           CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                            CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
       if (r != CUDA_SUCCESS) { set_error_msg(who, "cuTensorMapEncodeIm2col(x) failed"); return 0; }
     }
@@ -426,7 +329,7 @@ extern "C" int skd_conv2d_wgrad_sm100(int N, int H, int W, int Cin, int Cout, in
     cuuint32_t box[4] = {32, (cuuint32_t)p.BWk, (cuuint32_t)p.BHk, 1};
     cuuint32_t es[4] = {1, 1, 1, 1};
     CUresult r = enc(&tdy, dt, 4, const_cast<float*>(dy), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                     CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+                     CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) { set_error_msg(who, "cuTensorMapEncodeTiled(dy) failed"); return 0; }
   }
   {
@@ -435,7 +338,7 @@ extern "C" int skd_conv2d_wgrad_sm100(int N, int H, int W, int Cin, int Cout, in
     cuuint32_t box[4] = {32, (cuuint32_t)(p.BWk * stride), (cuuint32_t)(p.BHk * stride), 1};
     cuuint32_t es[4] = {1, (cuuint32_t)stride, (cuuint32_t)stride, 1};
     CUresult r = enc(&tx, dt, 4, const_cast<float*>(x), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                     CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+                     CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) { set_error_msg(who, "cuTensorMapEncodeTiled(x) failed"); return 0; }
   }
   }
@@ -445,13 +348,12 @@ extern "C" int skd_conv2d_wgrad_sm100(int N, int H, int W, int Cin, int Cout, in
   a.splits = p.splits; a.kb_total = p.kb_total; a.kb_per_split = p.kb_per_split;
   a.ws = p.splits == 1 ? dw : workspace;
   a.linear = p.linear;
-  const int units = (p.m_tiles / (p.pair ? 2 : 1)) * p.n_tiles * p.taps * p.splits;
+  const int units = p.m_tiles * p.n_tiles * p.taps * p.splits;
   int ok;
   switch (p.bn) {
-    case 256: ok = p.pair ? launch<256, 2>(tdy, tx, a, units, st) : launch<256, 1>(tdy, tx, a, units, st); break;
-    case 128: ok = launch<128, 1>(tdy, tx, a, units, st); break;
-    case 64: ok = launch<64, 1>(tdy, tx, a, units, st); break;
-    default: ok = launch<32, 1>(tdy, tx, a, units, st); break;
+    case 128: ok = launch<128>(tdy, tx, a, units, st); break;
+    case 64: ok = launch<64>(tdy, tx, a, units, st); break;
+    default: ok = launch<32>(tdy, tx, a, units, st); break;
   }
   if (!ok) return 0;
   if (p.splits > 1) {

@@ -1,4 +1,4 @@
-// SAGAN discriminator of the holistic (Ho) loss on sm_100a -- everything around its tensor-core convolutions:
+// SAGAN discriminator of the holistic (Ho) loss on sm_90a -- everything around its tensor-core convolutions:
 //
 //   networks/spectral.py:23-35          skd_sn_power_iter / skd_sn_weight_grad   (cluster + DSMEM power iteration)
 //   networks/sagan_models.py:147,157    skd_bn2d_*                               (BatchNorm2d(19), batch statistics)
@@ -7,7 +7,7 @@
 //   utils/criterion.py:98-120           skd_gp_norms / skd_gp_direction          (WGAN-GP)
 //   utils/criterion.py:129-166          skd_adv_loss                             (wgan / hinge adversarial losses)
 //
-// The 4x4 stride-2 spectral-norm convolutions and the 1x1 q/k/v projections run on the tcgen05 implicit-GEMM kernel
+// The 4x4 stride-2 spectral-norm convolutions and the 1x1 q/k/v projections run on the wgmma implicit-GEMM kernel
 // (conv_sm100.cu, split-precision 3xTF32); the data gradient of a 4x4/s2/p1 convolution is ONE 3x3 stride-1 convolution of
 // dy producing the four input-pixel parity classes as 4*Cin channels (weights from skd_disc_dgrad_weight_prep), un-shuffled
 // (and multiplied by the LeakyReLU mask of the layer below) by skd_disc_dgrad_unshuffle.
@@ -21,7 +21,7 @@
 
 #include "common.cuh"
 #include "skd.h"
-#include "sm100_ptx.cuh"
+#include "sm90_ptx.cuh"
 
 namespace cg = cooperative_groups;
 using namespace skd;
@@ -81,7 +81,7 @@ __device__ __forceinline__ void block_gemm(int M, int N, int K, FA a, FB b, FS s
 
 // The same product on the tensor cores: mma.sync m16n8k8 TF32 in split precision (a_lo*b_hi + a_hi*b_lo + a_hi*b_hi, fp32-grade like
 // the 3xTF32 convolutions), operands through the same shared-memory accessors.  Warp tiles of 16 x 8*NT, eight warps round-robin.
-// The attention products are 32..128 positions wide (n x n x d scores, n x C x n values): far below one tcgen05 tile pipeline's
+// The attention products are 32..128 positions wide (n x n x d scores, n x C x n values): far below one wgmma tile pipeline's
 // start-up cost, so the warp-level MMA is the tensor-core path that fits them.
 __device__ __forceinline__ void mma_m16n8k8_tf32(float (&c)[4], const uint32_t (&a)[4], const uint32_t (&b)[2]) {
   asm volatile("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
@@ -219,7 +219,7 @@ sn_power_iter_kernel(int Cout, int taps, int Cin, const float* __restrict__ w, f
 }
 
 // ---- the same iteration for SEVERAL layers at once, spread over the whole GPU (the discriminator's four layers per forward) ----
-// The cluster kernel above keeps one layer on 8 SMs: 197 us for the 512 x 4096 matrix of l4 (two passes over 8 MB through 8 SMs).
+// The cluster kernel above keeps one layer on 8 SMs: the 512 x 4096 matrix of l4 is two passes over 8 MB through 8 SMs.
 // Here every phase is a grid over all layers: (1) partial W^T u per 32-row block, (2) v = normalize(sum of partials) [fixed order],
 // (3) s = W v, one warp per row, (4) u = normalize(s), sigma = u . s.  Deterministic (no atomics): replicas of a data-parallel
 // job keep bit-identical u, v.
@@ -426,7 +426,7 @@ bn2d_reduce_kernel(int N, int C, int HW, const float* __restrict__ x, long long 
   double s1 = 0.0, s2 = 0.0, s3 = 0.0;
   if (lane < C) {
     const float m = MODE ? mean[lane] : 0.f, r = MODE ? rstd[lane] : 0.f;
-    // four pixels per iteration: 4-12 independent loads in flight per lane (one pixel per iteration was latency-bound: 50 us for 67 080 pixels)
+    // four pixels per iteration: 4-12 independent loads in flight per lane (one pixel per iteration is latency-bound)
     const long long step = (long long)gridDim.x * 8;
     for (long long p0 = (long long)blockIdx.x * 8 + warp; p0 < P; p0 += 4 * step) {
       float xv[4], av[4], bv[4];

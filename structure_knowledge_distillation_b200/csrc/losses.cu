@@ -1,8 +1,8 @@
-// Distillation / task losses for sm_100a (HBM- or latency-bound: SIMT, coalesced, fused; no tensor cores here).
+// Distillation / task losses for sm_90a (HBM- or latency-bound: SIMT, coalesced, fused; no tensor cores here).
 //   * pixel-wise (Pi):  utils/criterion.py:211-226   softmax(T) . log_softmax(S), batch-summed, / (W*H)
 //   * pair-wise  (Pa):  utils/criterion.py:228-245 + utils/utils.py:170-183 (ceil-mode max-pool, detached L2 norm,
 //                       node affinity, squared difference) -- SIMT path for <= ~1.2k nodes; the 8 385-node regime is
-//                       the tcgen05 kernel in pairwise_sm100.cu
+//                       the wgmma kernel in pairwise_sm100.cu
 //   * DSN cross entropy: utils/criterion.py:168-188   bilinear(align_corners) upsample + log-softmax + NLL(ignore)
 //                       fused so the 2 x 318 MB upsampled logits are never materialised.
 // Tensors are addressed with explicit element strides (sn, sc, sp) over (image, channel, pixel) so both NCHW
@@ -335,7 +335,7 @@ pa_pool_kernel(const float* __restrict__ F, Strides st, int C, int H, int W, int
 }
 
 // NHWC variant: 16 channel quads (float4) x 16 window lanes per block -- 4x the loads in flight of the scalar kernel above, which
-// walks a 32 x 64 pixel window (pool_scale 0.5) with 4 lanes of dependent scalar loads (0.21 ms per 8 x 512 x 65 x 129 tensor)
+// walks a 32 x 64 pixel window (pool_scale 0.5) with 4 lanes of dependent scalar loads
 __global__ void __launch_bounds__(256)
 pa_pool_nhwc_kernel(const float* __restrict__ F, long long sn, int pitch, int C, int H, int W, int ph, int pw, int nh, int nw,
                     float* __restrict__ pooled, int* __restrict__ argmax) {

@@ -3,7 +3,7 @@
 
 #include "common.cuh"
 #include "skd.h"
-#include "sm100_ptx.cuh"
+#include "sm90_ptx.cuh"
 
 namespace skd {
 static thread_local char g_err[256] = "";
@@ -44,7 +44,7 @@ int blocks_for(long long n) { long long b = (n + 255) / 256; if (b > kNumSMs * 1
 }  // namespace
 
 extern "C" const char* skd_last_error(void) { return skd::g_err; }
-extern "C" int skd_version(void) { return 100; }
+extern "C" int skd_version(void) { return 90; }
 extern "C" long long skd_kernel_launches(void) { return (long long)skd::g_kernel_launches; }
 extern "C" void skd_set_tf32_tma_type(int use_tfloat32_type) { skd::g_tf32_tma_type = use_tfloat32_type ? 1 : 0; }
 

@@ -1,4 +1,4 @@
-// Pair-wise affinity loss at large node counts (pool_scale -> 1/65: 8 385 nodes per image) on tcgen05.
+// Pair-wise affinity loss at large node counts (pool_scale -> 1/65: 8 385 nodes per image) on wgmma.
 //   utils/utils.py:173-183:  A = f^T f / (|f_m| |f_n|) per image,  loss = sum (A_T - A_S)^2 / nodes^2 / N
 // Formulation: with X = [ fT*rT | fS*rS ] and W = [ fT*rT | -fS*rS ] (K = C_T + C_S) the difference matrix is ONE K-major
 // GEMM  E = X W^T, so the tensor-core kernel of conv_sm100.cu is used as a plain NT GEMM (skd_gemm_nt_sm100) with the L2

@@ -1,4 +1,4 @@
-// NHWC pooling / resampling / optimizer kernels for sm_100a (all HBM- or latency-bound; float4 over channels).
+// NHWC pooling / resampling / optimizer kernels for sm_90a (all HBM- or latency-bound; float4 over channels).
 //   * 3x3 s2 p1 ceil-mode max-pool of the ResNet stem          networks/pspnet_combine.py:130
 //   * AdaptiveAvgPool2d(1/2/3/6) of the PSP module               networks/pspnet_combine.py:103
 //   * bilinear(align_corners) upsampling of the PSP priors, written straight into their channel slice of the
@@ -40,8 +40,7 @@ __device__ __forceinline__ void max4(float4& best, int4& bi, const float4 v, int
 }
 
 // One block per (output row, slice of the row): the (n, y) decomposition is done once per block and the inner index is 32-bit (the
-// flat 64-bit i -> (n, y, x, c4) chain of divisions cost more issue slots than the memory traffic: ncu put these kernels at 40-60 % of
-// the HBM rate of a plain copy).
+// flat 64-bit i -> (n, y, x, c4) chain of divisions costs more issue slots than the memory traffic).
 __global__ void __launch_bounds__(256)
 maxpool_fwd_kernel(const float* __restrict__ x, float* __restrict__ y, unsigned char* __restrict__ arg, int N, int H, int W,
                    int C4, int OH, int OW) {
@@ -119,7 +118,7 @@ constexpr int kMaxXBins = 16, kMaxXSegs = 32;
 struct XBins { int n, nseg; int seg_lo[kMaxXSegs + 1]; int fs[kMaxXBins]; int ls[kMaxXBins]; };
 
 // block = 64 channel quads (float4) x 4 x-lanes (adjacent threads: a warp reads 4 pixels x 128 contiguous bytes); lanes are folded
-// with two shuffles per segment.  (The first version walked a row with scalar loads and 12 compares per value: 1.3 TB/s.)
+// with two shuffles per segment.  (Walking a row with scalar loads and 12 compares per value is issue-bound.)
 __global__ void __launch_bounds__(256)
 psp_rowbins_kernel(const float* __restrict__ x, int pitch, int C, int H, int W, XBins xb, float* __restrict__ rowbins) {
   const int y = blockIdx.x, n = blockIdx.y, xl = threadIdx.x & 3, cq = threadIdx.x >> 2;
@@ -168,7 +167,7 @@ psp_colbins_kernel(const float* __restrict__ rowbins, int C, int H, int W, Pyram
 }
 
 // dx[n][y][x][c] = sum over bins containing (y,x) of dpooled/area.  Bin extents come from tables in the kernel parameters (the version
-// that re-derived them with integer divisions per element and candidate bin spent ~3 600 instructions per float4: 0.43 ms for 137 MB).
+// that re-derived them with integer divisions per element and candidate bin spent ~3 600 instructions per float4).
 struct PyrBins { int levels; int size[4]; int first_bin[4]; int lo_y[4][6], hi_y[4][6], lo_x[4][6], hi_x[4][6]; };
 
 __global__ void __launch_bounds__(256)

@@ -1,5 +1,5 @@
 """Cityscapes training loader with the augmentation on the GPU -- host-side mirror of `dataset/datasets.py::CSDataSet`
-(/root/reference/dataset/datasets.py:121-210) for the callers of the hot path (`train_and_eval.py:13-17` builds the loaders whose batches
+(reference dataset/datasets.py:121-210) for the callers of the hot path (`train_and_eval.py:13-17` builds the loaders whose batches
 go to `NetModel.set_input`).
 
 Split of the work:

@@ -1,4 +1,4 @@
-"""torch.autograd.Functions over the sm_100a kernels (the reference's libs/functions.py role, for the whole hot path).
+"""torch.autograd.Functions over the sm_90a kernels (the reference's libs/functions.py role, for the whole hot path).
 
 Conventions kept from the reference (libs/functions.py:70-162): ctx.save_for_backward for tensors, non-tensor
 arguments get None gradients, backward is once-differentiable (no double backward through hand-written kernels).
@@ -29,7 +29,7 @@ class PixelWiseLoss(torch.autograd.Function):
 class PairWiseLoss(torch.autograd.Function):
     """CriterionPairWiseforWholeFeatAfterPool math (utils/criterion.py:236-245, utils/utils.py:170-183)."""
 
-    TCGEN05_MIN_NODES = 1024      # below: one SIMT tile kernel (the default pool_scale 0.5 has 9 nodes); above: tcgen05 GEMM
+    TCGEN05_MIN_NODES = 1024      # below: one SIMT tile kernel (the default pool_scale 0.5 has 9 nodes); above: wgmma GEMM
 
     @staticmethod
     def forward(ctx, feat_S, feat_T, ph, pw):
@@ -95,7 +95,7 @@ def _padded_weight(w_ohwi, cout_p, cin_p):
 
 
 def conv_forward_padded(x, weight, bias, stride, pad, dil, **epi):
-    """tcgen05 forward for any channel count: Cin / Cout that are not multiples of 4 (3-channel image, 19 classes) are
+    """wgmma forward for any channel count: Cin / Cout that are not multiples of 4 (3-channel image, 19 classes) are
     zero-padded to the next multiple so that every pixel row is 16-byte aligned for TMA.  Returns a (N,Cout,OH,OW) view."""
     w = ops.weight_ohwi(weight)
     cout, kh, kw, cin = w.shape
@@ -122,7 +122,7 @@ def _small_cin(weight):
 
 
 def conv_forward_small_cin(x, weight, stride, pad, dil, precise=False, **epi):
-    """Tiny-Cin convolution (3-channel stem) as explicit im2col + one dense K=32 GEMM step on tcgen05."""
+    """Tiny-Cin convolution (3-channel stem) as explicit im2col + one dense K=32 GEMM step on wgmma."""
     cout, cin, kh, kw = weight.shape
     k = kh * kw * cin
     kp = (k + 31) // 32 * 32
@@ -162,7 +162,7 @@ def _sync_mean(t):
 class WgradOverlap:
     """Weight-gradient kernels on a side stream.  In the backward pass only the data-gradient chain (dgrad -> ABN backward -> dgrad
     ...) is sequential; a layer's weight gradient needs (x, dy) and feeds nothing but the optimizer.  Issued on a second stream the
-    tcgen05 wgrad kernels (12 K registers, no co-residency conflict) overlap the HBM-bound ABN backward passes of the chain instead
+    wgmma wgrad kernels (12 K registers, no co-residency conflict) overlap the HBM-bound ABN backward passes of the chain instead
     of queueing between them.  NetModel opens a window around G_loss.backward(); tensors a side-stream kernel reads are kept alive
     until the window's join, so the caching allocator cannot hand their memory to a main-stream kernel early (valid in eager
     mode and under CUDA-graph capture alike -- no record_stream)."""
@@ -203,7 +203,7 @@ def _grad_written(param):
 
 
 class Conv2d(torch.autograd.Function):
-    """nn.Conv2d forward / dgrad / wgrad on tcgen05.  x is NHWC-stored; weight is the (Cout,Cin,KH,KW) parameter held in
+    """nn.Conv2d forward / dgrad / wgrad on wgmma.  x is NHWC-stored; weight is the (Cout,Cin,KH,KW) parameter held in
     channels-last (OHWI) storage."""
 
     @staticmethod

@@ -1,5 +1,5 @@
 """InPlace-ABN module facade with the reference's constructor surface (libs/bn.py:48-193), backed by the fused NHWC
-sm_100a kernels (csrc/abn.cu).  State-dict names are the reference's: weight, bias, running_mean, running_var.
+sm_90a kernels (csrc/abn.cu).  State-dict names are the reference's: weight, bias, running_mean, running_var.
 
 `InPlaceABNSync` keeps its name and arguments; with one process per GPU the statistics are per-rank by default (what
 the reference's own launch script runs: 1 GPU, run_train_val.sh:8-15).

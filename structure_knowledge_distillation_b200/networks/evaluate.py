@@ -1,5 +1,5 @@
 """`evaluate_main` of the reference (networks/evaluate.py:162-206) on the frozen-path kernels: eval-mode BN folded into the
-tcgen05 convolution epilogues, class scores up-sampled / accumulated / arg-maxed and the confusion matrix counted on the GPU
+wgmma convolution epilogues, class scores up-sampled / accumulated / arg-maxed and the confusion matrix counted on the GPU
 (csrc/eval.cu); only the num_classes x num_classes counts come back to the host.
 
 Kept: whole-image prediction at 1024x2048 (`whole=True`, predict_multiscale with scale 1.0, no flip) and sliding 1/3-overlap

@@ -1,4 +1,4 @@
-"""`NetModel` -- the reference's training-step entry point (networks/kd_model.py:27-193), B200-native underneath.
+"""`NetModel` -- the reference's training-step entry point (networks/kd_model.py:27-193), H100-native underneath.
 
 Kept surface: NetModel(args), .set_input(data), .forward(), .student_backward(), .discriminator_backward(),
 .optimize_parameters(), .adjust_learning_rate(base_lr, optimizer, i_iter), .lr_poly, .print_info, .save_ckpt,
@@ -63,7 +63,7 @@ class NetModel():
         self.args = args
         device = torch.device(_arg(args, "device", "cuda"))
         if device.type != "cuda":
-            raise RuntimeError("NetModel runs on CUDA (sm_100a) only; there is no CPU path")
+            raise RuntimeError("NetModel runs on CUDA (sm_90a) only; there is no CPU path")
         self.device = device
         self.world = dist.get_world_size() if dist.is_available() and dist.is_initialized() else 1
 
@@ -84,7 +84,7 @@ class NetModel():
             p.requires_grad_(False)
         self.parallel_teacher = self.teacher
 
-        # SAGAN discriminator on the sm_100a kernels (networks/sagan_engine.py): tcgen05 spectral-norm convolutions, fused
+        # SAGAN discriminator on the sm_90a kernels (networks/sagan_engine.py): wgmma spectral-norm convolutions, fused
         # attention, and the WGAN-GP penalty by a tangent + joint reverse pass instead of autograd's double backward
         D_model = Discriminator(args.preprocess_GAN_mode, args.classes_num, args.batch_size, args.imsize_for_adv, args.adv_conv_dim)
         load_D_model(args, D_model, False)
@@ -246,7 +246,7 @@ class NetModel():
         """One step up to (not including) the two optimizer updates, with the discriminator phase (kd_model.py:153-163 without the
         D step) on its own stream UNDER the student's backward pass.  The D phase needs the logits of forward() and the D state left
         by the generator pass's D(S) (one power iteration) -- not the student's gradients or its updated weights -- and its ~370
-        launches are tiny grids (4x8 .. 32x64 maps): alone they leave the GPU mostly idle for ~4 ms, beside the student's
+        launches are tiny grids (4x8 .. 32x64 maps): alone they leave the GPU mostly idle, beside the student's
         backward kernels they cost nothing.  It starts once the generator pass's adjoint through D has been issued (event recorded
         by DiscriminatorFn.backward) and is joined before the optimizer updates."""
         self.forward()

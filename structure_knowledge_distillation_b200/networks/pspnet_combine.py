@@ -1,9 +1,9 @@
 """PSPNet / dilated ResNet with the reference's public surface (networks/pspnet_combine.py): `Res_pspnet(block, layers,
 num_classes)`, `BasicBlock`, `Bottleneck`, `PSPModule`, identical state-dict names and the 7-tensor output list
-`[x, x_dsn, x_feat_after_psp, x4, x3, x2, x1]` (:189) -- computed by the sm_100a kernels of libskd_b200.
+`[x, x_dsn, x_feat_after_psp, x4, x3, x2, x1]` (:189) -- computed by the sm_90a kernels of libskd_b200.
 
 Two execution paths over the same parameters:
-  * training (student): torch.autograd.Functions, conv (tcgen05) -> fused ABN(+ReLU / +residual+ReLU / +Dropout2d);
+  * training (student): torch.autograd.Functions, conv (wgmma) -> fused ABN(+ReLU / +residual+ReLU / +Dropout2d);
   * frozen  (teacher: eval() under no_grad, networks/kd_model.py:121-122): no autograd, eval-mode ABN folded into the
     convolution epilogue (scale/shift/activation/residual in registers), layer4 writes straight into the PSP concat
     buffer -- one kernel per conv, nothing else touches HBM.
@@ -25,14 +25,14 @@ BatchNorm2d = functools.partial(InPlaceABNSync, activation='none')          # ps
 
 class Conv2d(nn.Module):
     """nn.Conv2d stand-in (same constructor arguments, parameter names and default init) whose weight lives in OHWI
-    (channels-last) storage, the K-major layout the tcgen05 kernels read."""
+    (channels-last) storage, the K-major layout the wgmma kernels read."""
 
     def __init__(self, in_channels, out_channels, kernel_size, stride=1, padding=0, dilation=1, bias=True):
         super().__init__()
         k = kernel_size if isinstance(kernel_size, int) else kernel_size[0]
         self.in_channels, self.out_channels, self.kernel_size = in_channels, out_channels, (k, k)
         self.stride, self.padding, self.dilation = stride, padding, dilation
-        self.precise = False              # training forward in split-precision 3xTF32 (set for the student's stem + layer1)
+        self.precise = False              # training forward in split-precision 3xTF32 (set for the student's stem, layer1 and layer2)
         w = torch.empty(out_channels, in_channels, k, k)
         nn.init.kaiming_uniform_(w, a=math.sqrt(5))                         # nn.Conv2d.reset_parameters
         self.weight = nn.Parameter(w.contiguous(memory_format=torch.channels_last))
@@ -206,10 +206,11 @@ class ResNet(nn.Module):
         self.set_precise_early_layers(True)
 
     def set_precise_early_layers(self, on=True):
-        """Training-mode forward of the stem and layer1 in split-precision 3xTF32 (fp32-grade): with batch statistics the
-        operand rounding of these first layers is what the rest of the network amplifies (measured: student-logit error
-        9e-3 -> 2.6e-3, DESIGN.md).  No effect on the frozen / eval path; ~+4 ms per step at batch 8, 512x1024."""
-        for m in [self.conv1, self.conv2, self.conv3] + [c for c in self.layer1.modules() if isinstance(c, Conv2d)]:
+        """Training-mode forward of the stem, layer1 and layer2 in split-precision 3xTF32 (fp32-grade): with batch statistics the
+        operand rounding of these first layers is what the rest of the network amplifies (DESIGN.md "TF32 and parity").  No effect
+        on the frozen / eval path."""
+        early = [c for layer in (self.layer1, self.layer2) for c in layer.modules() if isinstance(c, Conv2d)]
+        for m in [self.conv1, self.conv2, self.conv3] + early:
             m.precise = bool(on)
 
     def _make_layer(self, block, planes, blocks, stride=1, dilation=1, multi_grid=1):

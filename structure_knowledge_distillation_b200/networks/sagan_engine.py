@@ -1,4 +1,4 @@
-"""Execution engine of the SAGAN discriminator on the sm_100a kernels (csrc/disc.cu + the tcgen05 convolutions).
+"""Execution engine of the SAGAN discriminator on the sm_90a kernels (csrc/disc.cu + the wgmma convolutions).
 
 Three passes over the same parameters, none of them through torch operators or autograd:
 
@@ -10,8 +10,8 @@ Three passes over the same parameters, none of them through torch operators or a
                         graph, which for the bilinear layers is the ordinary backward over a [primal | tangent] batch of 2B.
                         oracle/gp_dual.py states the same operation sequence in torch and is pinned against autograd.
 
-Activations are NHWC rows.  The 4x4/s2 spectral-norm convolutions and the q/k/v projections run on the tcgen05 implicit-GEMM
-kernel in split precision (3xTF32); weight gradients on the tcgen05 wgrad kernel (TF32); 1/sigma rides in the convolution
+Activations are NHWC rows.  The 4x4/s2 spectral-norm convolutions and the q/k/v projections run on the wgmma implicit-GEMM
+kernel in split precision (3xTF32); weight gradients on the wgmma wgrad kernel (TF32); 1/sigma rides in the convolution
 epilogue's per-channel scale, so no normalised weight tensor is ever materialised.
 """
 import ctypes
@@ -563,7 +563,7 @@ class AdvLossFn(torch.autograd.Function):
 # ---------------------------------------------------------------------------------------------------- stand-alone layers
 class SNConvFn(torch.autograd.Function):
     """SpectralNorm(conv).forward used on its own (networks/spectral.py:66-68): one power iteration, then
-    y = conv(x, w_bar) / sigma + bias on tcgen05; backward = tcgen05 dgrad / wgrad + the sigma term of spectral.py:34-35."""
+    y = conv(x, w_bar) / sigma + bias on wgmma; backward = wgmma dgrad / wgrad + the sigma term of spectral.py:34-35."""
 
     @staticmethod
     def forward(ctx, m, x, w_bar, bias):

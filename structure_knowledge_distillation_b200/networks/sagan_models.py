@@ -1,6 +1,6 @@
 """SAGAN discriminator of the holistic (Ho) loss -- same classes, constructor arguments, state-dict names and [out, p1, p2]
-output as networks/sagan_models.py:9-41,105-168, executed by hand-written sm_100a kernels (networks/sagan_engine.py,
-csrc/disc.cu, tcgen05 convolutions): no torch operator, cuDNN or cuBLAS call on the forward, backward or WGAN-GP path.
+output as networks/sagan_models.py:9-41,105-168, executed by hand-written sm_90a kernels (networks/sagan_engine.py,
+csrc/disc.cu, wgmma convolutions): no torch operator, cuDNN or cuBLAS call on the forward, backward or WGAN-GP path.
 
 The modules below are parameter containers with the reference's names; `Discriminator.forward` is one autograd node
 (`DiscriminatorFn`).  Differences that are visible to a caller:
@@ -20,7 +20,7 @@ from .spectral import SpectralNorm
 
 class Self_Attn(nn.Module):
     """Self attention layer: softmax(Q^T K) without 1/sqrt(d), out = gamma * (V A^T) + x, gamma initialised to 0
-    (sagan_models.py:9-41).  query/key/value 1x1 convolutions are one (2d+C) x C GEMM on tcgen05; the core is csrc/disc.cu."""
+    (sagan_models.py:9-41).  query/key/value 1x1 convolutions are one (2d+C) x C GEMM on wgmma; the core is csrc/disc.cu."""
 
     def __init__(self, in_dim, activation=None):
         super().__init__()

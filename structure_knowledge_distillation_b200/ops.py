@@ -9,7 +9,7 @@ from ._cabi import lib
 
 ACT = {"none": 0, "leaky_relu": 1, "elu": 2, "relu": 3}
 
-# bench.py sets this to a list to time every tcgen05 conv launch with CUDA events: (start, end, algorithmic FLOP)
+# bench.py sets this to a list to time every wgmma conv launch with CUDA events: (start, end, algorithmic FLOP)
 CONV_EVENT_LOG = None
 
 
@@ -234,7 +234,7 @@ def conv2d_fwd_3xtf32(x, w_ohwi, stride, pad, dil, shift=None):
 
 
 def conv2d_dgrad(dy, w_ohwi, x_shape, stride, pad, dil, round_tf32=False, force_direct=False):
-    """dx for y = conv(x, w).  stride 1: forward tcgen05 kernel on dy with the flipped/transposed weights."""
+    """dx for y = conv(x, w).  stride 1: forward wgmma kernel on dy with the flipped/transposed weights."""
     n, cin, h, w = x_shape
     cout, kh, kw, _ = w_ohwi.shape
     L = lib()
@@ -503,7 +503,7 @@ def pairwise_bwd(E, pS, rS, arg, grad_out, feat_like):
 
 
 def pairwise_affinity_sm100(pS, pT, rS, rT, want_E):
-    """tcgen05 large-node path: loss (0-dim) and E (N, nodes, ldE) or None."""
+    """wgmma large-node path: loss (0-dim) and E (N, nodes, ldE) or None."""
     n, nodes, cs = pS.shape
     ct = pT.shape[2]
     L = lib()

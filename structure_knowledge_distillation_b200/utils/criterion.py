@@ -1,5 +1,5 @@
 """Loss API of the reference (utils/criterion.py), same class names, constructor arguments, list-indexed inputs,
-0-dim fp32 outputs with autograd history and error behaviour -- computed by hand-written sm_100a kernels.
+0-dim fp32 outputs with autograd history and error behaviour -- computed by hand-written sm_90a kernels.
 
   CriterionPixelWise                          utils/criterion.py:211-226
   CriterionPairWiseforWholeFeatAfterPool      utils/criterion.py:228-245   (alias: CriterionPairWise, the name the

@@ -28,7 +28,7 @@ def test_reference_native_abi_names_are_mirrored():
 
 def test_lib_object_and_version():
     L = _cabi.lib()
-    assert L.skd_version() == 100
+    assert L.skd_version() == 90
     assert L.skd_pool_out_size_ceil(256, 3, 2, 1) == 129       # ceil-mode stem max-pool (pspnet_combine.py:130)
     assert L.skd_pool_out_size_ceil(129, 3, 2, 1) == 65
     assert L.skd_abn_num_splits(67080, 512) >= 1

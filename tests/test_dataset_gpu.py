@@ -1,6 +1,7 @@
 """GPU: `skd_cs_augment_batch` (csrc/augment.cu) through `DeviceAugment` / `CSDataLoader` against (1) the outputs of the UNMODIFIED
-reference loader stored in tests/golden/dataset.pt and (2) the oracle restatement on seeded full-size inputs (1024 x 2048 -> 512 x 1024,
+reference loader stored in tests/golden/dataset.pt.gz and (2) the oracle restatement on seeded full-size inputs (1024 x 2048 -> 512 x 1024,
 all 15 scale factors).  Integer / table work and one float32 subtraction: the bar is bit-exact."""
+import gzip
 import os
 import random
 
@@ -11,7 +12,7 @@ import torch
 from oracle import dataset_port as dp
 
 pytestmark = pytest.mark.gpu
-GOLD = os.path.join(os.path.dirname(__file__), "golden", "dataset.pt")
+GOLD = os.path.join(os.path.dirname(__file__), "golden", "dataset.pt.gz")
 
 
 def _augs(img, crop, scale, mirror, n):
@@ -21,7 +22,7 @@ def _augs(img, crop, scale, mirror, n):
 
 def test_device_augment_matches_reference_loader_golden():
     from structure_knowledge_distillation_b200.dataset.datasets import DeviceAugment
-    gold = torch.load(GOLD, weights_only=False)
+    gold = torch.load(gzip.open(GOLD), weights_only=False)
     mean = gold["mean"].numpy()
     total = 0
     for case in gold["cases"]:

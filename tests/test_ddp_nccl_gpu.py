@@ -1,6 +1,6 @@
 """Data-parallel semantics over NCCL on 2 GPUs (utils/parallel.py:54-63,155: loss per GPU on its shard, mean over GPUs):
 replicas are identical after construction whatever the per-rank RNG state, the all-reduced flat gradient is the SUM of the
-per-rank gradients, and FlatSGD.step applies their MEAN.  Skipped on a single-GPU box (run with `gpurun --gpus 2`)."""
+per-rank gradients, and FlatSGD.step applies their MEAN.  Skipped on a machine with fewer than two GPUs."""
 import os
 
 import pytest
@@ -80,7 +80,7 @@ def _worker(rank, world, port, out):
 
 def test_two_rank_nccl_gradient_average_through_flat_sgd():
     if torch.cuda.device_count() < 2:
-        pytest.skip("needs 2 GPUs (gpurun --gpus 2)")
+        pytest.skip("needs 2 GPUs")
     import torch.multiprocessing as mp
     ctx = mp.get_context("spawn")
     q = ctx.Queue()
@@ -134,7 +134,7 @@ def test_sync_bn_two_ranks_equals_full_batch():
     combined mean / variance, running statistics with the global count, edz / eydz averaged over ranks) == the whole batch on one GPU:
     outputs, input gradients, summed parameter gradients, running statistics."""
     if torch.cuda.device_count() < 2:
-        pytest.skip("needs 2 GPUs (gpurun --gpus 2)")
+        pytest.skip("needs 2 GPUs")
     import torch.multiprocessing as mp
     ctx = mp.get_context("spawn")
     q = ctx.Queue()
@@ -212,7 +212,7 @@ def test_nvls_fused_sgd_two_ranks():
     equals p - lr * (mu * v + mean_over_ranks(g) + wd * p) over two steps, replicas bit-identical, and a whole distillation step equals
     the NCCL path's."""
     if torch.cuda.device_count() < 2:
-        pytest.skip("needs 2 GPUs (gpurun --gpus 2)")
+        pytest.skip("needs 2 GPUs")
     import torch.multiprocessing as mp
     ctx = mp.get_context("spawn")
     q = ctx.Queue()

@@ -1,8 +1,8 @@
-"""Discriminator (SAGAN, Ho loss) on the B200: every kernel of csrc/disc.cu through the C ABI against a float64 torch statement
+"""Discriminator (SAGAN, Ho loss) on the H100: every kernel of csrc/disc.cu through the C ABI against a float64 torch statement
 of the same operation (oracle/gp_dual.py where it has one), and the whole module + adversarial criteria + WGAN-GP against the
 golden fixture produced by the UNMODIFIED reference (tests/golden/discriminator.pt, oracle/make_golden.py).
 
-Tolerances: fp32 SIMT kernels 1e-5; tcgen05 convolutions 3xTF32 (fp32-grade) forward / data gradient, TF32 weight gradients
+Tolerances: fp32 SIMT kernels 1e-5; wgmma convolutions 3xTF32 (fp32-grade) forward / data gradient, TF32 weight gradients
 (3e-3 per tensor, rel-L2)."""
 import os
 
@@ -176,7 +176,7 @@ def _attention_case(L, B, n, C, d):
     attn, o, y, y_lo = torch.empty(B, n, n, device="cuda"), torch.empty(B * n, C, device="cuda"), torch.empty(B * n, C, device="cuda"), torch.empty(B * n, C, device="cuda")
     L.skd_attn_fwd(B, n, C, d, _p(qkv), ldq, _p(x), _p(gamma), _p(attn), _p(o), _p(y), _p(y_lo), _st())
     assert rel(attn, a_ref) < 2e-5 and rel(o, o_ref) < 2e-5 and rel(y, y_ref) < 2e-5
-    assert 0 < float(y_lo.abs().max()) <= float(y.abs().max()) * 2 ** -10        # the TF32 lo part: y - rna_tf32(y)
+    assert 0 < float(y_lo.abs().max()) <= float(y.abs().max()) * 2 ** -10        # the TF32 lo part: y - rn_tf32(y)
     ty_ref, ds_ref, da_ref, do_ref = gp_dual.attn_tangent(q, k, v, a_ref, tq, tk, tv, D(tx), gamma.double())
     dattn, to, ty = torch.empty(B, n, n, device="cuda"), torch.empty(B * n, C, device="cuda"), torch.empty(B * n, C, device="cuda")
     L.skd_attn_tangent_fwd(B, n, C, d, _p(qkv), _p(tqkv), ldq, _p(attn), _p(tx), _p(gamma), _p(dattn), _p(to), _p(ty), None, _st())
@@ -257,7 +257,7 @@ def test_conv_split_k_matches_fp64(L, B, H, W, cin, cout, k, stride, pad, precis
         ref = ref + r.permute(0, 3, 1, 2).double()
     ref = F.leaky_relu(ref, 0.1)
     e = rel(y.permute(0, 3, 1, 2), ref)
-    assert e < (5e-5 if precise else 1e-3), e            # 3xTF32, K up to 4096: the TMEM fp32 accumulation truncates (~1e-5 per 1000 K steps)
+    assert e < (5e-5 if precise else 1e-3), e            # 3xTF32, K up to 4096: the tensor-core fp32 accumulation truncates (~1e-5 per 1000 K steps)
     # and the un-split launch of the same convolution agrees (different summation order only)
     y2 = torch.empty_like(y)
     L.skd_conv2d_fwd_sm100_ex(B, H, W, cin, cout, k, k, stride, pad, 1, _p(x), _p(x_lo) if precise else None, cin, _p(w), _p(w_lo) if precise else None,

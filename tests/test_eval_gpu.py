@@ -1,4 +1,4 @@
-"""Evaluation path and eval/train mode switching on the B200: evaluate_main (networks/evaluate.py:162-206) against a torch
+"""Evaluation path and eval/train mode switching on the H100: evaluate_main (networks/evaluate.py:162-206) against a torch
 restatement of the reference's numpy pipeline on the same class scores; the student's eval logits after training steps (the
 folded BN of a TRAINABLE module must not be cached: ADVICE r1); eval-mode ABN backward (libs/functions.py:144-147)."""
 import numpy as np

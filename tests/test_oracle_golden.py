@@ -1,5 +1,5 @@
 """CPU: the oracle (oracle/port.py) against the golden fixtures produced by the UNMODIFIED reference
-(oracle/make_golden.py, run in the build container where /root/reference exists)."""
+(oracle/make_golden.py, run against a checkout of the reference)."""
 import os
 
 import pytest
@@ -31,8 +31,8 @@ def test_criteria_match_reference():
         pi = port.pixelwise_loss(S[0], T[0]); pa = port.pairwise_loss(S[2], T[2], scale); ce = port.dsn_ce_loss(S, labels)
         assert _rel(pi, G["pi"]) < 1e-6 and _rel(pa, G["pa"]) < 1e-5 and _rel(ce, G["ce"]) < 1e-6
         (pi + pa + ce).backward()
-        assert torch.allclose(S[0].grad, G["d_pi"] + G["d_ce0"], rtol=1e-4, atol=1e-8)
-        assert torch.allclose(S[2].grad, G["d_pa"], rtol=1e-3, atol=1e-9)
+        assert torch.allclose(*cases.at_stored(S[0].grad, cases.stored_sum(G["d_pi"], G["d_ce0"])), rtol=1e-4, atol=1e-8)
+        assert torch.allclose(*cases.at_stored(S[2].grad, G["d_pa"]), rtol=1e-3, atol=1e-9)
     adv = gold["adv"]
     for kind in ("wgan-gp", "hinge"):
         assert _rel(port.adv_loss_d([adv["dS"]], [adv["dT"]], kind), adv[kind]["d"]) < 1e-6

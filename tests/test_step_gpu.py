@@ -1,4 +1,4 @@
-"""Step-level parity on the B200: NetModel (our kernels) against the golden fixtures produced by the UNMODIFIED
+"""Step-level parity on the H100: NetModel (our kernels) against the golden fixtures produced by the UNMODIFIED
 reference modules driven in networks/kd_model.py:119-173 order (oracle/make_golden.py).  Contract (BASELINE.json):
 every loss within 1e-3 relative; student gradients: relative L2 of each parameter's gradient norm reported, <= 3e-2
 (TF32 operands through a 100-layer teacher / 18-layer student, fp32 accumulation)."""
