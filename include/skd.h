@@ -101,6 +101,29 @@ int skd_dsn_ce_fwd_train(int N, int C, int h, int w, int H, int W, const float* 
 int skd_dsn_ce_bwd_cols(int N, int C, int h, int w, int H, const float* rows_ws, long long a_sn, long long a_sc, long long a_sp,
                         long long b_sn, long long b_sc, long long b_sp, int heads, float w0, float w1, const float* grad_out,
                         const float* count, float* d0, float* d1, cudaStream_t);
+/* OhemCrossEntropy2d / CriterionOhemDSN (utils/criterion.py:11-90, 190-209), with no host round trip.
+   skd_ohem_grid_sample replaces find_threshold's scipy zooms (criterion.py:20-35): for every point of the gh x gw grid (Python
+   round(H / factor), round(W / factor)) it writes the zoomed probability of the zoomed label (+inf where that label is
+   ignore_index) to pred[N*gh*gw], the zoomed label to grid_labels (may be NULL) and the number of valid points to *nvalid.
+   The probabilities come from the low-resolution logits (align_corners upsample to (H, W), fp32 softmax). */
+int skd_ohem_grid_sample(int N, int C, int h, int w, int H, int W, int gh, int gw, const float* logits, long long sn, long long sc,
+                         long long sp, const long long* labels, int ignore_index, float* pred, long long* grid_labels, int* nvalid,
+                         cudaStream_t);
+/* criterion.py:36-47 (np.partition): threshold = 1 when min_kept >= *nvalid, else thresh raised to the (min_kept-1)-th smallest
+   pred when that is larger and min_kept > 0 (min_kept = the reference's min_kept // factor^2).  Exact radix select on the device. */
+long long skd_ohem_threshold_workspace_ints(void);
+int skd_ohem_threshold(long long n, const float* pred, const int* nvalid, int min_kept, float thresh, float* threshold,
+                       int* workspace, cudaStream_t);
+/* criterion.py:65-90 + 203-209: w0 * CE over the valid pixels with p[label] <= *threshold (head 0) + w1 * CE over the valid
+   pixels (head 1, logits1 may be NULL), each mean over its own count, fused with the backward's row phase like
+   skd_dsn_ce_fwd_train.  counts[4]: kept, valid (head 1), and the two denominators skd_ohem_dsn_ce_bwd_cols reads. */
+int skd_ohem_dsn_ce_fwd_train(int N, int C, int h, int w, int H, int W, const float* logits0, long long a_sn, long long a_sc,
+                              long long a_sp, const float* logits1, long long b_sn, long long b_sc, long long b_sp,
+                              const long long* labels, int ignore_index, float w0, float w1, const float* threshold, float* loss,
+                              float* counts, double* partials, float* rows_ws, cudaStream_t);
+int skd_ohem_dsn_ce_bwd_cols(int N, int C, int h, int w, int H, const float* rows_ws, long long a_sn, long long a_sc, long long a_sp,
+                             long long b_sn, long long b_sc, long long b_sp, int heads, float w0, float w1, const float* grad_out,
+                             const float* counts, float* d0, float* d1, cudaStream_t);
 /* CriterionPairWiseforWholeFeatAfterPool.forward (utils/criterion.py:236-245) + sim_dis_compute (utils/utils.py:170-183):
    pool: ceil-mode max pool kernel=stride=(ph,pw) -> pooled[N][nodes][C], argmax (pixel index, may be NULL), rnorm[N][nodes] */
 int skd_pairwise_pool(int N, int C, int H, int W, const float* F, long long sn, long long sc, long long sp, int ph, int pw,

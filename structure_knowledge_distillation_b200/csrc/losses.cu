@@ -35,6 +35,33 @@ __global__ void finalize_sum_kernel(const double* __restrict__ part, int n, doub
   }
 }
 
+// OHEM DSN: loss = sum_0 / count_0 + sum_1 / count_1 (the weights are already in the partials), each head summed in a fixed
+// order over its `per_head` partials.  counts: kept (head 0), valid (head 1), then the two backward denominators, where an
+// empty head divides by +inf so that its gradient is 0 while its loss is NaN (torch's cross entropy over no target)
+__global__ void ohem_finalize_kernel(const double* __restrict__ part_loss, const double* __restrict__ part_cnt, int per_head,
+                                     int heads, float* __restrict__ loss, float* __restrict__ counts) {
+  __shared__ double sh[4][32];
+  double a[2] = {0.0, 0.0}, b[2] = {0.0, 0.0};
+  for (int hd = 0; hd < heads; ++hd)
+    for (int i = threadIdx.x; i < per_head; i += blockDim.x) { a[hd] += part_loss[hd * per_head + i]; b[hd] += part_cnt[hd * per_head + i]; }
+  for (int o = 16; o > 0; o >>= 1)
+    for (int hd = 0; hd < 2; ++hd) { a[hd] += __shfl_xor_sync(0xffffffffu, a[hd], o); b[hd] += __shfl_xor_sync(0xffffffffu, b[hd], o); }
+  if ((threadIdx.x & 31) == 0) {
+    const int wid = threadIdx.x >> 5;
+    sh[0][wid] = a[0]; sh[1][wid] = b[0]; sh[2][wid] = a[1]; sh[3][wid] = b[1];
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double t[4] = {0.0, 0.0, 0.0, 0.0};
+    for (int i = 0; i < (int)(blockDim.x >> 5); ++i) for (int q = 0; q < 4; ++q) t[q] += sh[q][i];
+    double l = t[0] / t[1];
+    if (heads == 2) l += t[2] / t[3];
+    loss[0] = (float)l;
+    counts[0] = (float)t[1]; counts[1] = (float)t[3];
+    counts[2] = t[1] > 0.0 ? (float)t[1] : INFINITY; counts[3] = t[3] > 0.0 ? (float)t[3] : INFINITY;
+  }
+}
+
 __device__ __forceinline__ double block_sum_d(double v, double* sh) {
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
   __syncthreads();
@@ -184,12 +211,16 @@ dsn_ce_fwd_kernel(const float* __restrict__ L0, const float* __restrict__ L1, St
 // the two source rows of the logits are blended ONCE per block into shared memory (row[x][c] = ly0 * L[y0][x][c] + ly1 * L[y1][x][c]),
 // so a pixel is 2 x C shared-memory reads instead of 4 x C global ones, and the softmax reuses exp(v - max) for the gradient (C
 // exponentials per pixel instead of 2 C).  CT: compile-time class bound (19 for Cityscapes; 32 generic).
+// OHEM = true (OhemCrossEntropy2d, utils/criterion.py:65-90): head 0 keeps a valid pixel only when its softmax probability of the
+// label is <= *ohem_thr (the device threshold of ohem.cu); dropped pixels contribute neither loss, gradient nor count.  Each head
+// then writes its own count partials (the two heads have different denominators).
 constexpr int kRowsThreads = 512;
-template <bool LOSS, int CT>
+template <bool LOSS, int CT, bool OHEM = false>
 __global__ void __launch_bounds__(kRowsThreads, 2)
 dsn_ce_bwd_rows_kernel(const float* __restrict__ L0, const float* __restrict__ L1, Strides s0, Strides s1,
                        const long long* __restrict__ labels, int N, int C, int h, int w, int H, int W, int ignore,
-                       float* __restrict__ T1, int chunk, double* __restrict__ part_loss, double* __restrict__ part_cnt, float w0, float w1) {
+                       float* __restrict__ T1, int chunk, double* __restrict__ part_loss, double* __restrict__ part_cnt, float w0, float w1,
+                       const float* __restrict__ ohem_thr = nullptr) {
   __shared__ double shd[32];
   double loss_acc = 0.0, cnt_acc = 0.0;
   extern __shared__ float G[];                                 // [C][chunk|1], wa[chunk], wb[chunk], first[w+2], row[w][C]
@@ -203,6 +234,7 @@ dsn_ce_bwd_rows_kernel(const float* __restrict__ L0, const float* __restrict__ L
   const Strides st = head == 0 ? s0 : s1;
   const float sy = H > 1 ? (float)(h - 1) / (float)(H - 1) : 0.f, sx = W > 1 ? (float)(w - 1) / (float)(W - 1) : 0.f;
   const Bilin by = bilin(Y, sy, h);
+  const float thr = (OHEM && head == 0) ? __ldg(ohem_thr) : 0.f;
   float* out = T1 + (((size_t)head * N + n) * H + Y) * (size_t)C * w;
   {
     const float* b0 = L + n * st.sn + (long long)by.i0 * w * st.sp;
@@ -244,9 +276,21 @@ dsn_ce_bwd_rows_kernel(const float* __restrict__ L0, const float* __restrict__ L
 #pragma unroll
         for (int c = 0; c < CT; ++c) if (c < C) { v[c] = __expf(v[c] - m); z += v[c]; }
         const float rz = 1.f / z;
+        bool keep = true;
+        if (OHEM && head == 0) {
+          float e = 0.f;
 #pragma unroll
-        for (int c = 0; c < CT; ++c) if (c < C) G[c * pitch + j] = v[c] * rz - (c == (int)lab ? 1.f : 0.f);
-        if (LOSS) { loss_acc += (double)(m + __logf(z) - pick); cnt_acc += 1.0; }
+          for (int c = 0; c < CT; ++c) if (c == (int)lab) e = v[c];
+          keep = e * rz <= thr;
+        }
+        if (keep) {
+#pragma unroll
+          for (int c = 0; c < CT; ++c) if (c < C) G[c * pitch + j] = v[c] * rz - (c == (int)lab ? 1.f : 0.f);
+          if (LOSS) { loss_acc += (double)(m + __logf(z) - pick); cnt_acc += 1.0; }
+        } else {
+#pragma unroll
+          for (int c = 0; c < CT; ++c) if (c < C) G[c * pitch + j] = 0.f;
+        }
       }
     }
     __syncthreads();
@@ -265,7 +309,7 @@ dsn_ce_bwd_rows_kernel(const float* __restrict__ L0, const float* __restrict__ L
     if (threadIdx.x == 0) {
       const size_t idx = ((size_t)head * N + n) * H + Y;
       part_loss[idx] = tl * (double)(head == 0 ? w0 : w1);
-      part_cnt[idx] = head == 0 ? tc : 0.0;
+      part_cnt[idx] = (OHEM || head == 0) ? tc : 0.0;
     }
   }
 }
@@ -532,7 +576,7 @@ extern "C" long long skd_dsn_ce_bwd_workspace_floats(int N, int C, int w, int H,
 
 static int dsn_rows_launch(bool with_loss, int N, int C, int h, int w, int H, int W, const float* L0, Strides a, const float* L1, Strides b,
                            const long long* labels, int ignore_index, float w0, float w1, float* T1, double* part_loss, double* part_cnt,
-                           cudaStream_t st, const char* who) {
+                           cudaStream_t st, const char* who, const float* ohem_thr = nullptr) {
   const int heads = L1 ? 2 : 1;
   int chunk = W < 1024 ? W : 1024;
   const size_t smem = ((size_t)C * (chunk | 1) + 2 * (size_t)chunk + (size_t)w + 2 + (size_t)w * C) * sizeof(float);
@@ -543,9 +587,20 @@ static int dsn_rows_launch(bool with_loss, int N, int C, int h, int w, int H, in
     cudaFuncSetAttribute(dsn_ce_bwd_rows_kernel<true, 19>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
     cudaFuncSetAttribute(dsn_ce_bwd_rows_kernel<false, kMaxClasses>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
     cudaFuncSetAttribute(dsn_ce_bwd_rows_kernel<true, kMaxClasses>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+    cudaFuncSetAttribute(dsn_ce_bwd_rows_kernel<true, 19, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+    cudaFuncSetAttribute(dsn_ce_bwd_rows_kernel<true, kMaxClasses, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
     attr_done = true;
   }
   const dim3 grid(H, N, heads);
+  if (ohem_thr) {
+    if (C <= 19)
+      dsn_ce_bwd_rows_kernel<true, 19, true><<<grid, kRowsThreads, smem, st>>>(L0, L1, a, b, labels, N, C, h, w, H, W, ignore_index, T1,
+                                                                             chunk, part_loss, part_cnt, w0, w1, ohem_thr);
+    else
+      dsn_ce_bwd_rows_kernel<true, kMaxClasses, true><<<grid, kRowsThreads, smem, st>>>(L0, L1, a, b, labels, N, C, h, w, H, W, ignore_index,
+                                                                                      T1, chunk, part_loss, part_cnt, w0, w1, ohem_thr);
+    return 1;
+  }
 #define SKD_DSN_ROWS(LOSSF, CTV, PL, PC) \
   dsn_ce_bwd_rows_kernel<LOSSF, CTV><<<grid, kRowsThreads, smem, st>>>(L0, L1, a, b, labels, N, C, h, w, H, W, ignore_index, T1, chunk, PL, PC, w0, w1)
   if (with_loss) { if (C <= 19) SKD_DSN_ROWS(true, 19, part_loss, part_cnt); else SKD_DSN_ROWS(true, kMaxClasses, part_loss, part_cnt); }
@@ -593,6 +648,35 @@ extern "C" int skd_dsn_ce_bwd_cols(int N, int C, int h, int w, int H, const floa
   dsn_ce_bwd_cols_kernel<<<red_blocks(tot), 256, 0, st>>>(rows_ws, d0, heads == 2 ? d1 : nullptr, Strides{a_sn, a_sc, a_sp},
                                                          Strides{b_sn, b_sc, b_sp}, N, C, h, w, H, grad_out, count, w0, w1);
   return finish("skd_dsn_ce_bwd_cols");
+}
+
+// CriterionOhemDSN / OhemCrossEntropy2d training forward: head 0 masked by the device threshold (ohem.cu), head 1 plain CE, each
+// divided by its own count.  counts: 4 floats (kept, valid of head 1, and the two backward denominators); partials and rows_ws
+// are sized as for skd_dsn_ce_fwd_train
+extern "C" int skd_ohem_dsn_ce_fwd_train(int N, int C, int h, int w, int H, int W, const float* L0, long long a_sn, long long a_sc,
+                                         long long a_sp, const float* L1, long long b_sn, long long b_sc, long long b_sp,
+                                         const long long* labels, int ignore_index, float w0, float w1, const float* threshold,
+                                         float* loss, float* counts, double* partials, float* rows_ws, cudaStream_t st) {
+  if (C > kMaxClasses) { set_error_msg("skd_ohem_dsn_ce_fwd_train", "C > 32 classes unsupported"); return 0; }
+  const int heads = L1 ? 2 : 1;
+  const int np = heads * N * H;
+  if (!dsn_rows_launch(true, N, C, h, w, H, W, L0, Strides{a_sn, a_sc, a_sp}, L1, Strides{b_sn, b_sc, b_sp}, labels, ignore_index, w0, w1,
+                       rows_ws, partials, partials + np, st, "skd_ohem_dsn_ce_fwd_train", threshold)) return 0;
+  ohem_finalize_kernel<<<1, 256, 0, st>>>(partials, partials + np, N * H, heads, loss, counts);
+  return finish("skd_ohem_dsn_ce_fwd_train", 2);
+}
+
+// Backward after skd_ohem_dsn_ce_fwd_train: the column phase once per head, each with its own denominator (counts + 2)
+extern "C" int skd_ohem_dsn_ce_bwd_cols(int N, int C, int h, int w, int H, const float* rows_ws, long long a_sn, long long a_sc,
+                                        long long a_sp, long long b_sn, long long b_sc, long long b_sp, int heads, float w0, float w1,
+                                        const float* grad_out, const float* counts, float* d0, float* d1, cudaStream_t st) {
+  const long long per = (long long)N * h * C * w;
+  const Strides a{a_sn, a_sc, a_sp}, b{b_sn, b_sc, b_sp};
+  dsn_ce_bwd_cols_kernel<<<red_blocks(per), 256, 0, st>>>(rows_ws, d0, nullptr, a, a, N, C, h, w, H, grad_out, counts + 2, w0, w0);
+  if (heads == 2)
+    dsn_ce_bwd_cols_kernel<<<red_blocks(per), 256, 0, st>>>(rows_ws + (size_t)N * H * C * w, d1, nullptr, b, b, N, C, h, w, H, grad_out,
+                                                           counts + 3, w1, w1);
+  return finish("skd_ohem_dsn_ce_bwd_cols", heads);
 }
 
 extern "C" int skd_pairwise_pool(int N, int C, int H, int W, const float* F, long long sn, long long sc, long long sp,

@@ -84,6 +84,32 @@ class DsnCrossEntropy(torch.autograd.Function):
         return d0, d1, None, None, None, None
 
 
+class OhemDsnCrossEntropy(torch.autograd.Function):
+    """OhemCrossEntropy2d (utils/criterion.py:11-90) on head 0, plain CE on head 1 (l1 may be None), as CriterionOhemDSN
+    (:200-209) combines them: w0 * OHEM-CE(up(l0)) + w1 * CE(up(l1)).  The threshold pass (1/factor grid + exact radix select)
+    and the masked cross entropy run on the device, so there is no host sync.  Returns (loss, threshold, kept count); only the
+    loss carries a gradient."""
+
+    @staticmethod
+    def forward(ctx, l0, l1, labels, ignore_index, thresh, min_kept, factor, w0, w1):
+        pred, _, nvalid = ops.ohem_grid_sample(l0, labels, factor, ignore_index)
+        thr = ops.ohem_threshold(pred, nvalid, min_kept // (factor * factor), thresh)
+        loss, counts, rows = ops.ohem_dsn_ce_fwd_train(l0, l1, labels, ignore_index, w0, w1, thr)
+        ctx.save_for_backward(l0, l1, rows, counts)
+        ctx.cfg = (labels.shape[1], w0, w1)
+        kept = counts[0].clone()
+        ctx.mark_non_differentiable(thr, kept)
+        return loss, thr, kept
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g, g_thr, g_kept):
+        l0, l1, rows, counts = ctx.saved_tensors
+        H, w0, w1 = ctx.cfg
+        d0, d1 = ops.ohem_dsn_ce_bwd_cols(l0, l1, rows, H, w0, w1, g.contiguous(), counts)
+        return d0, d1, None, None, None, None, None, None, None
+
+
 # ------------------------------------------------------------------------------------------------ layers
 def _padded_weight(w_ohwi, cout_p, cin_p):
     cout, kh, kw, cin = w_ohwi.shape

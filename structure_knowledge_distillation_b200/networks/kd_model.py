@@ -24,7 +24,7 @@ import torch.distributed as dist
 from .. import functions as Fn
 from .. import ops
 from ..optim import FlatSGD
-from ..utils.criterion import (CriterionAdditionalGP, CriterionAdv, CriterionAdvForG, CriterionDSN,
+from ..utils.criterion import (CriterionAdditionalGP, CriterionAdv, CriterionAdvForG, CriterionDSN, CriterionOhemDSN,
                                CriterionPairWiseforWholeFeatAfterPool, CriterionPixelWise)
 from ..utils.utils import load_D_model, load_S_model, load_T_model
 from .evaluate import evaluate_main
@@ -110,7 +110,10 @@ class NetModel():
             elif int(_arg(args, "allreduce_buckets", 4)) > 0:      # 0: one all-reduce after the backward pass
                 self.G_solver.enable_overlap(int(_arg(args, "allreduce_buckets", 4)))
 
-        self.criterion = CriterionDSN()
+        if _arg(args, "ohem", False):                             # OHEM task loss (the reference imports CriterionOhemDSN, kd_model.py:18)
+            self.criterion = CriterionOhemDSN(thresh=_arg(args, "ohem_thres", 0.7), min_kept=_arg(args, "ohem_keep", 100000))
+        else:
+            self.criterion = CriterionDSN()
         self.criterion_pixel_wise = CriterionPixelWise()
         self.criterion_pair_wise_for_interfeat = CriterionPairWiseforWholeFeatAfterPool(scale=args.pool_scale, feat_ind=-5)
         self.criterion_adv = CriterionAdv(args.adv_loss_type)

@@ -455,6 +455,66 @@ def dsn_ce_bwd_cols(l0, l1, rows, H, w0, w1, grad_out, count):
     return d0, d1
 
 
+def ohem_grid_shape(H, W, factor):
+    """Size of OhemCrossEntropy2d's threshold grid: scipy.ndimage.zoom's output shape, Python round(H * (1 / factor))
+    (half to even: 36 / 8 -> 4, 44 / 8 -> 6)."""
+    return int(round(H * (1.0 / factor))), int(round(W * (1.0 / factor)))
+
+
+def ohem_grid_sample(logits, labels, factor, ignore_index, want_labels=False):
+    """-> (pred (N, gh, gw) fp32 with +inf at ignored points, grid labels (N, gh, gw) int64 or None, valid count (1,) int32)."""
+    _f32(logits)
+    n, c, h, w = logits.shape
+    H, W = labels.shape[1:]
+    if labels.dtype != torch.int64 or not labels.is_contiguous():
+        raise ValueError("labels must be contiguous int64")
+    gh, gw = ohem_grid_shape(H, W, factor)
+    pred = torch.empty((n, gh, gw), device=logits.device, dtype=torch.float32)
+    glab = torch.empty((n, gh, gw), device=logits.device, dtype=torch.int64) if want_labels else None
+    nvalid = torch.empty(1, device=logits.device, dtype=torch.int32)
+    lib().skd_ohem_grid_sample(n, c, h, w, H, W, gh, gw, _p(logits), *pixel_strides(logits), _p(labels), ignore_index, _p(pred),
+                               _p(glab), _p(nvalid), _st())
+    return pred, glab, nvalid
+
+
+def ohem_threshold(pred, nvalid, min_kept, thresh):
+    """Device threshold (0-dim fp32) from the grid values: 1 if min_kept >= valid, else max(thresh, (min_kept-1)-th smallest)."""
+    L = lib()
+    ws = torch.empty(L.skd_ohem_threshold_workspace_ints(), device=pred.device, dtype=torch.int32)
+    thr = torch.empty((), device=pred.device, dtype=torch.float32)
+    L.skd_ohem_threshold(pred.numel(), _p(pred), _p(nvalid), int(min(min_kept, 2 ** 31 - 1)), float(thresh), _p(thr), _p(ws), _st())
+    return thr
+
+
+def ohem_dsn_ce_fwd_train(l0, l1, labels, ignore_index, w0, w1, threshold):
+    """-> (loss 0-dim, counts (4,): kept, valid of head 1, backward denominators) and the backward's row-phase workspace."""
+    _f32(l0, l1)
+    n, c, h, w = l0.shape
+    H, W = labels.shape[1:]
+    if labels.dtype != torch.int64 or not labels.is_contiguous():
+        raise ValueError("labels must be contiguous int64")
+    L = lib()
+    heads = 2 if l1 is not None else 1
+    loss = torch.empty((), device=l0.device, dtype=torch.float32)
+    counts = torch.empty(4, device=l0.device, dtype=torch.float32)
+    parts = torch.empty(L.skd_dsn_ce_train_partials(n, H, heads), device=l0.device, dtype=torch.float64)
+    rows = torch.empty(L.skd_dsn_ce_bwd_workspace_floats(n, c, w, H, heads), device=l0.device, dtype=torch.float32)
+    s1 = pixel_strides(l1) if l1 is not None else (0, 0, 0)
+    L.skd_ohem_dsn_ce_fwd_train(n, c, h, w, H, W, _p(l0), *pixel_strides(l0), _p(l1), *s1, _p(labels), ignore_index, w0, w1,
+                                _p(threshold), _p(loss), _p(counts), _p(parts), _p(rows), _st())
+    return loss, counts, rows
+
+
+def ohem_dsn_ce_bwd_cols(l0, l1, rows, H, w0, w1, grad_out, counts):
+    n, c, h, w = l0.shape
+    d0 = torch.empty_strided(l0.shape, l0.stride(), device=l0.device, dtype=torch.float32)
+    d1 = torch.empty_strided(l1.shape, l1.stride(), device=l1.device, dtype=torch.float32) if l1 is not None else None
+    s1 = pixel_strides(l1) if l1 is not None else (0, 0, 0)
+    lib().skd_ohem_dsn_ce_bwd_cols(n, c, h, w, H, _p(rows), *pixel_strides(l0), *s1, 2 if l1 is not None else 1, w0, w1, _p(grad_out),
+                                   _p(counts), _p(d0), _p(d1), _st())
+    return d0, d1
+
+
 def dsn_ce_bwd(l0, l1, labels, ignore_index, w0, w1, grad_out, count):
     n, c, h, w = l0.shape
     H, W = labels.shape[1:]

@@ -5,8 +5,18 @@
   CriterionPairWiseforWholeFeatAfterPool      utils/criterion.py:228-245   (alias: CriterionPairWise, the name the
                                               north star uses; it does not exist in the reference tree)
   CriterionDSN                                utils/criterion.py:168-188
+  OhemCrossEntropy2d                          utils/criterion.py:11-90
+  CriterionOhemDSN                            utils/criterion.py:190-209
   CriterionAdv / CriterionAdvForG             utils/criterion.py:122-166
   CriterionAdditionalGP                       utils/criterion.py:92-120
+
+The OHEM criteria follow the reference's threshold rule (scipy's zoom to a 1/factor grid with its exact arithmetic, the order
+statistic, pixels with p[label] <= threshold kept) but compute it on the device, without the reference's host round trip.
+Differences, on purpose:
+  * no `Labels: <kept> <threshold>` print per call; the criterion keeps `last_threshold` and `last_kept` as device tensors;
+  * `weight` is ignored (so is it in the reference);
+  * with several ranks each rank thresholds its own shard (the reference's per-replica criterion semantics);
+  * when no pixel is kept the loss is NaN, as torch's cross entropy returns, and the gradient is zero.
 """
 import torch
 import torch.nn as nn
@@ -54,6 +64,49 @@ class CriterionDSN(nn.Module):
 
     def forward(self, preds, target):
         return Fn.DsnCrossEntropy.apply(preds[0], preds[1], target, self.ignore_index, 1.0, 0.4)
+
+
+class OhemCrossEntropy2d(nn.Module):
+    """Cross entropy over the hard pixels only: those whose softmax probability of the label is <= a threshold found on a
+    1/`factor` grid (at least ~`min_kept` pixels, never fewer than those under `thresh`).  `predict` is (n, c, H, W) at label
+    resolution.  Limit: the fused loss kernel holds one row of `predict` in shared memory, so W may be at most 1 483 columns with
+    19 classes (about 760 with 32); wider inputs (full-size 1024x2048 Cityscapes maps) raise RuntimeError ("source width too
+    large").  CriterionOhemDSN has no such limit in practice: it reads the low-resolution logits (65x129 at 512x1024)."""
+
+    def __init__(self, ignore_label=255, thresh=0.7, min_kept=100000, factor=8):
+        super().__init__()
+        self.ignore_label = ignore_label
+        self.thresh = float(thresh)
+        self.min_kept = int(min_kept)
+        self.factor = factor
+        self.last_threshold = None
+        self.last_kept = None
+
+    def forward(self, predict, target, weight=None):
+        assert not target.requires_grad
+        loss, self.last_threshold, self.last_kept = Fn.OhemDsnCrossEntropy.apply(
+            predict, None, target, self.ignore_label, self.thresh, self.min_kept, self.factor, 1.0, 0.0)
+        return loss
+
+
+class CriterionOhemDSN(nn.Module):
+    """DSN with OHEM on the main head: OhemCrossEntropy2d(up(preds[0])) + 0.4 * CE(up(preds[1])), bilinear align_corners to the
+    label size, fused so that neither upsampled logit map is materialised."""
+
+    def __init__(self, ignore_index=255, thresh=0.7, min_kept=100000, use_weight=True, reduce=True):
+        super().__init__()
+        self.ignore_index = ignore_index
+        self.criterion1 = OhemCrossEntropy2d(ignore_index, thresh, min_kept)
+        self.last_threshold = None
+        self.last_kept = None
+
+    def forward(self, preds, target):
+        assert not target.requires_grad
+        c = self.criterion1
+        loss, self.last_threshold, self.last_kept = Fn.OhemDsnCrossEntropy.apply(
+            preds[0], preds[1], target, self.ignore_index, c.thresh, c.min_kept, c.factor, 1.0, 0.4)
+        c.last_threshold, c.last_kept = self.last_threshold, self.last_kept
+        return loss
 
 
 class CriterionAdvForG(nn.Module):

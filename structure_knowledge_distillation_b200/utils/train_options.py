@@ -11,7 +11,8 @@ DEFAULTS = dict(
     student_pretrain_model_imgnet='None', pi=True, pa=True, ho=True, adv_loss_type='wgan-gp', imsize_for_adv=65,
     adv_conv_dim=64, lambda_gp=10.0, lambda_d=0.1, lambda_pi=10.0, lambda_pa=0.5, pool_scale=0.5, preprocess_GAN_mode=1,
     lr_g=1e-2, lr_d=4e-4, best_mean_IU=0.0, gpu_num=1,
-    cuda_graph=False)        # ours: capture the step into CUDA graphs after 3 eager steps (NetModel.enable_cuda_graphs)
+    cuda_graph=False,        # ours: capture the step into CUDA graphs after 3 eager steps (NetModel.enable_cuda_graphs)
+    ohem=False, ohem_thres=0.7, ohem_keep=100000)   # ours: CriterionOhemDSN(thresh=ohem_thres, min_kept=ohem_keep) as the CE term
 
 
 def make_args(**overrides):
