@@ -321,6 +321,25 @@ int skd_eval_upsample_accumulate(int C, int h, int w, const float* logits, long 
                                  int valid_w, float* full, int W, int y1, int x1, cudaStream_t);
 int skd_eval_argmax_confusion(int H, int W, int C, const float* full, const long long* gt, long long gt_row, int valid_h, int valid_w,
                               int ignore_index, long long* confusion, unsigned char* pred, cudaStream_t);
+/* predict_multiscale (networks/evaluate.py:115-134), whole-image tiles placed at (0, 0):
+   skd_eval_zoom_image replaces scipy.ndimage.zoom(image, (1, 1, s, s), order=1, prefilter=False) (:127) bit for bit, including mode
+   'constant''s zero line where a rounded source coordinate passes the last row / column; image is float32 (1, 3, H, W) contiguous,
+   out_h / out_w = round(H * s), round(W * s); out is the 4-channel NHWC network input [1 + flip][out_h][out_w][4] (channel 3 zero),
+   item 1 the mirror image[:, :, :, ::-1] (:130) when flip != 0.
+   skd_eval_upsample_accumulate_ms: full += weight * up(L0) (paired = 0) or full += weight * 0.5f * (up(L0)[y][x] + up(L1)[y][tile_w-1-x])
+   (paired = 1, :131), L1 = batch item 1 of the logits (sn floats after L0); weight = 1 / len(scales) (:133). */
+int skd_eval_zoom_image(int H, int W, const float* image, int out_h, int out_w, int flip, float* out, cudaStream_t);
+int skd_eval_upsample_accumulate_ms(int C, int h, int w, const float* logits, long long sn, long long sc, long long sp, int tile_h,
+                                    int tile_w, int valid_h, int valid_w, float* full, int W, float weight, int paired, cudaStream_t);
+/* arg-max of the whole score buffer into pred [pred_h][pred_w] (evaluate.py:187-191, before the `size` crop of :194), through the
+   256-entry device table lut when given (train id -> Cityscapes label id for type='test', :188); confusion += over the valid region
+   only, as skd_eval_argmax_confusion.  gt / pred may be NULL. */
+int skd_eval_argmax_confusion_lut(int H, int W, int C, const float* full, const long long* gt, long long gt_row, int valid_h, int valid_w,
+                                  int ignore_index, long long* confusion, unsigned char* pred, int pred_h, int pred_w,
+                                  const unsigned char* lut, cudaStream_t);
+/* HOST tables, 256 entries each: label id -> train id (dataset/datasets.py:146-151, the table skd_cs_augment_batch applies) and its
+   reverse, train id -> label id, as id2trainId(..., reverse=True) builds it (evaluate.py:30-38, 188) */
+int skd_cityscapes_id_tables(unsigned char* to_train, unsigned char* to_label);
 
 /* ---- Cityscapes training augmentation on the device (csrc/augment.cu) --------------------------------------------------------------
    Replaces the per-sample CPU work of `CSDataSet.__getitem__` after cv2.imread (reference dataset/datasets.py:175-206):
@@ -341,6 +360,10 @@ typedef struct skd_cs_sample {
 } skd_cs_sample;
 int skd_cs_augment_batch(int n, const skd_cs_sample* samples, int crop_h, int crop_w, const float* mean_bgr, int ignore_label,
                          float* images, void* labels, int labels_int64, cudaStream_t);
+/* `CSDataTestSet.__getitem__` after cv2.imread (dataset/datasets.py:234-250): image (device, uint8 H x W x 3 BGR) -> out (device,
+   float32 [3][out_h][out_w]), value (float)((double)x - mean_bgr[c]) -- the reference subtracts a tuple of Python floats, i.e. in
+   double -- and zero padding on the bottom / right; out_h = max(H, crop_h), out_w = max(W, crop_w) (no crop).  mean_bgr: HOST, 3. */
+int skd_cs_test_preprocess(int H, int W, const unsigned char* image, const double* mean_bgr, int out_h, int out_w, float* out, cudaStream_t);
 
 #ifdef __cplusplus
 }

@@ -30,8 +30,7 @@ struct DevSample {
 struct DevBatch { DevSample s[kMaxSamples]; float mean[3]; int ignore_label; };
 
 // datasets.py:143-149 (ids 0..33; everything else passes through)
-__constant__ unsigned char kTrainId[34] = {255, 255, 255, 255, 255, 255, 255, 0, 1, 255, 255, 2, 3, 4, 255, 255, 255, 5, 255, 6, 7, 8, 9, 10, 11, 12,
-                                           13, 14, 15, 255, 255, 16, 17, 18};
+__constant__ unsigned char kTrainId[kCityscapesIds] = SKD_CITYSCAPES_TRAINID;
 
 __device__ __forceinline__ void linear_coef(int d, double inv, int size, bool reset_at_border, int& s, int& c0, int& c1) {
   float f = __double2float_rn(__dadd_rn(__dmul_rn(__dadd_rn((double)d, 0.5), inv), -0.5));

@@ -54,6 +54,44 @@ __device__ __forceinline__ float4 ld_stream(const float4* p) {   // read-once da
   return r;
 }
 
+// scipy.ndimage.zoom(order=1, prefilter=False, mode='constant') along one axis (ohem.cu's threshold grid, eval.cu's multi-scale
+// image): ratio (in - 1) / (out - 1) first (1 for a single output point), source coordinate o * ratio in double, both
+// neighbours and their weights.  A coordinate past in - 1 -- rounding can put the last output point there, e.g.
+// 767 * (1023 / 767) = 1023.0000000000001 -- lies outside the input, and mode 'constant' reads 0 for it.
+struct ZoomAxis {
+  double c, t, w0;     // coordinate, weight of i1 (c - i0), weight of i0 (1 - t)
+  int i0, i1;
+  bool outside;
+};
+__host__ __device__ __forceinline__ double zoom_ratio(int n_in, int n_out) {
+  return n_out > 1 ? (double)(n_in - 1) / (double)(n_out - 1) : 1.0;
+}
+__device__ __forceinline__ ZoomAxis zoom_axis(int o, double ratio, int n_in) {
+  ZoomAxis a;
+  a.c = __dmul_rn((double)o, ratio);
+  a.outside = a.c > (double)(n_in - 1);
+  a.i0 = (int)floor(a.c);
+  a.i1 = min(a.i0 + 1, n_in - 1);
+  a.t = __dsub_rn(a.c, (double)a.i0);
+  a.w0 = __dsub_rn(1.0, a.t);
+  return a;
+}
+// value * w_y * w_x, summed neighbour by neighbour in scipy's order (NI_ZoomShift); no FMA contraction
+__device__ __forceinline__ double zoom_lerp(double p00, double p01, double p10, double p11, const ZoomAxis& y, const ZoomAxis& x) {
+  double a = __dmul_rn(__dmul_rn(p00, y.w0), x.w0);
+  a = __dadd_rn(a, __dmul_rn(__dmul_rn(p01, y.w0), x.t));
+  a = __dadd_rn(a, __dmul_rn(__dmul_rn(p10, y.t), x.w0));
+  a = __dadd_rn(a, __dmul_rn(__dmul_rn(p11, y.t), x.t));
+  return a;
+}
+
+// Cityscapes label id -> train id (reference dataset/datasets.py:146-151, ids 0..33; everything else passes through).  The one
+// copy of the table: augment.cu maps labels with it, skd_cityscapes_id_tables derives the reverse (train id -> label id) map
+// that evaluation writes test-split predictions with.
+#define SKD_CITYSCAPES_TRAINID {255, 255, 255, 255, 255, 255, 255, 0, 1, 255, 255, 2, 3, 4, 255, 255, 255, 5, 255, 6, 7, 8, 9, 10, \
+                                11, 12, 13, 14, 15, 255, 255, 16, 17, 18}
+constexpr int kCityscapesIds = 34;
+
 enum Act : int { ACT_NONE = 0, ACT_LEAKY = 1, ACT_ELU = 2, ACT_RELU = 3 };
 
 __device__ __forceinline__ float act_fwd(float z, int act, float slope) {

@@ -50,19 +50,18 @@ __global__ void __launch_bounds__(256)
 ohem_grid_kernel(const float* __restrict__ L, long long sn, long long sc, long long sp, const long long* __restrict__ labels,
                  int N, int C, int h, int w, int H, int W, int gh, int gw, int ignore, float* __restrict__ pred,
                  long long* __restrict__ glabels, int* __restrict__ nvalid) {
-  // scipy: zoom = (in - 1) / (out - 1) first (1 for a single output point), coordinate = o * zoom
-  const double ry = gh > 1 ? (double)(H - 1) / (double)(gh - 1) : 1.0;
-  const double rx = gw > 1 ? (double)(W - 1) / (double)(gw - 1) : 1.0;
+  // scipy's zoom arithmetic (common.cuh: zoom_ratio / zoom_axis / zoom_lerp)
+  const double ry = zoom_ratio(H, gh), rx = zoom_ratio(W, gw);
   const float sy = H > 1 ? (float)(h - 1) / (float)(H - 1) : 0.f, sx = W > 1 ? (float)(w - 1) / (float)(W - 1) : 0.f;
   const long long total = (long long)N * gh * gw;
   int valid = 0;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
     const int gx = (int)(i % gw); const long long r = i / gw; const int gy = (int)(r % gh), n = (int)(r / gh);
-    const double cy = __dmul_rn((double)gy, ry), cx = __dmul_rn((double)gx, rx);
-    const bool outside = cy > (double)(H - 1) || cx > (double)(W - 1);       // mode 'constant', cval 0
+    const ZoomAxis ay = zoom_axis(gy, ry, H), ax = zoom_axis(gx, rx, W);
+    const bool outside = ay.outside || ax.outside;                             // mode 'constant', cval 0
     long long lab = 0;
     if (!outside) {
-      int iy = (int)floor(__dadd_rn(cy, 0.5)), ix = (int)floor(__dadd_rn(cx, 0.5));
+      int iy = (int)floor(__dadd_rn(ay.c, 0.5)), ix = (int)floor(__dadd_rn(ax.c, 0.5));
       iy = min(iy, H - 1); ix = min(ix, W - 1);
       lab = labels[((long long)n * H + iy) * W + ix];
     }
@@ -72,19 +71,12 @@ ohem_grid_kernel(const float* __restrict__ L, long long sn, long long sc, long l
       ++valid;
       v = 0.f;
       if (!outside) {
-        const int y0 = (int)floor(cy), x0 = (int)floor(cx);
-        const int y1 = min(y0 + 1, H - 1), x1 = min(x0 + 1, W - 1);
-        const double ty = __dsub_rn(cy, (double)y0), tx = __dsub_rn(cx, (double)x0);
-        const double wy0 = __dsub_rn(1.0, ty), wx0 = __dsub_rn(1.0, tx);
         const int lb = (int)lab;
-        const double p00 = up_prob(L, sn, sc, sp, n, C, h, w, sy, sx, y0, x0, lb), p01 = up_prob(L, sn, sc, sp, n, C, h, w, sy, sx, y0, x1, lb);
-        const double p10 = up_prob(L, sn, sc, sp, n, C, h, w, sy, sx, y1, x0, lb), p11 = up_prob(L, sn, sc, sp, n, C, h, w, sy, sx, y1, x1, lb);
-        // value * w_y * w_x, summed neighbour by neighbour (scipy's NI_ZoomShift order); no FMA contraction
-        double a = __dmul_rn(__dmul_rn(p00, wy0), wx0);
-        a = __dadd_rn(a, __dmul_rn(__dmul_rn(p01, wy0), tx));
-        a = __dadd_rn(a, __dmul_rn(__dmul_rn(p10, ty), wx0));
-        a = __dadd_rn(a, __dmul_rn(__dmul_rn(p11, ty), tx));
-        v = (float)a;                                                          // the zoomed array has the input's dtype
+        const double p00 = up_prob(L, sn, sc, sp, n, C, h, w, sy, sx, ay.i0, ax.i0, lb);
+        const double p01 = up_prob(L, sn, sc, sp, n, C, h, w, sy, sx, ay.i0, ax.i1, lb);
+        const double p10 = up_prob(L, sn, sc, sp, n, C, h, w, sy, sx, ay.i1, ax.i0, lb);
+        const double p11 = up_prob(L, sn, sc, sp, n, C, h, w, sy, sx, ay.i1, ax.i1, lb);
+        v = (float)zoom_lerp(p00, p01, p10, p11, ay, ax);                     // the zoomed array has the input's dtype
       }
     }
     pred[i] = v;

@@ -1,1 +1,2 @@
-from .datasets import CSDataSet, CSDataLoader, DeviceAugment, draw_augmentation, Augmentation  # noqa: F401
+from .datasets import CSDataSet, CSDataLoader, CSDataTestSet, DeviceAugment, DeviceTestPreprocess, draw_augmentation, Augmentation  # noqa: F401
+from .datasets import cityscapes_id_tables  # noqa: F401

@@ -9,6 +9,9 @@ Split of the work:
   * the GPU (`DeviceAugment` -> `skd_cs_augment_batch`, csrc/augment.cu): one kernel per batch produces the float32 CHW crop and the
     label crop directly from the raw uint8 files, bit-exact with the reference's cv2 pipeline (tests/test_dataset_gpu.py).
 `CSDataLoader` chains the two and yields `(images, labels, size, name)` batches resident on the device, i.e. what `set_input` takes.
+The test split (`CSDataTestSet`, reference datasets.py:212-250) works the same way: raw files from the workers, mean subtraction and
+padding on the GPU (`DeviceTestPreprocess` -> `skd_cs_test_preprocess`), and `CSDataLoader` yields `(images, size, name)`, the
+batches `evaluate_main(type='test')` unpacks.
 There is no CPU fallback: without libskd_b200.so `DeviceAugment` raises at import of the ops.
 """
 import collections
@@ -80,6 +83,76 @@ class CSDataSet(data.Dataset):
         return (torch.from_numpy(image), torch.from_numpy(label), torch.tensor(aug, dtype=torch.float64), np.array(image.shape), f["name"])
 
 
+def cityscapes_id_tables():
+    """-> (to_train, to_label): uint8[256] numpy tables label id -> train id (reference datasets.py:146-151, what the training
+    loader applies) and train id -> label id (evaluate.py:188, id2trainId(..., reverse=True)), both from the library's one copy."""
+    from .. import _cabi
+    to_train, to_label = np.zeros(256, np.uint8), np.zeros(256, np.uint8)
+    _cabi.lib().skd_cityscapes_id_tables(to_train.ctypes.data, to_label.ctypes.data)
+    return to_train, to_label
+
+
+class CSDataTestSet(data.Dataset):
+    """Same constructor as the reference (datasets.py:213).  `__getitem__` returns the RAW decoded file, its shape and its name:
+    (image uint8 H x W x 3 BGR, size int[3], name).  The mean subtraction and padding to crop_size run on the GPU
+    (`DeviceTestPreprocess`, through `CSDataLoader`).  Like the reference, it subtracts the BGR ImageNet mean whatever `mean` says."""
+
+    MEAN = (104.00698793, 116.66876762, 122.67891434)       # datasets.py:217
+
+    def __init__(self, root, list_path, crop_size=(505, 505), mean=(128, 128, 128)):
+        self.root, self.list_path = root, list_path
+        self.crop_h, self.crop_w = crop_size
+        self.mean = self.MEAN
+        self.img_ids = [i_id.strip().split() for i_id in open(list_path)]
+        self.files = [{"img": osp.join(self.root, item[0]), "name": osp.splitext(osp.basename(item[0]))[0]} for item in self.img_ids]
+
+    def __len__(self):
+        return len(self.files)
+
+    def __getitem__(self, index):
+        import cv2
+        f = self.files[index]
+        image = cv2.imread(f["img"], cv2.IMREAD_COLOR)
+        if image is None:
+            raise IOError("cannot read %s" % f["img"])
+        return torch.from_numpy(image), np.array(image.shape), f["name"]
+
+
+class DeviceTestPreprocess:
+    """raw test images -> float32 [B, 3, max(H, crop_h), max(W, crop_w)] on the device: (float)((double)x - mean[c]) with zero
+    padding on the bottom / right and no crop (datasets.py:239-249), one kernel launch per image."""
+
+    def __init__(self, crop_size, mean, device=None):
+        from .. import _cabi
+        self._lib = _cabi.lib()
+        self.crop_h, self.crop_w = crop_size
+        self.mean = np.array([float(m) for m in mean], dtype=np.float64)
+        self.device = torch.device("cuda") if device is None else torch.device(device)
+
+    def __call__(self, images):
+        """images: uint8 [B,H,W,3] tensor or list of [H,W,3] (the batch's padded sizes must agree, as default collation needs)."""
+        dev = [t.to(self.device, non_blocking=True).contiguous() for t in images]
+        for t in dev:
+            if t.dtype != torch.uint8 or t.dim() != 3 or t.shape[2] != 3:
+                raise ValueError("raw image must be uint8 H x W x 3")
+        shapes = {(max(int(t.shape[0]), self.crop_h), max(int(t.shape[1]), self.crop_w)) for t in dev}
+        if len(shapes) != 1:
+            raise ValueError("test images of one batch pad to different sizes %s: use batch_size=1" % sorted(shapes))
+        (oh, ow), = shapes
+        out = torch.empty((len(dev), 3, oh, ow), dtype=torch.float32, device=self.device)
+        for i, t in enumerate(dev):
+            self._lib.skd_cs_test_preprocess(int(t.shape[0]), int(t.shape[1]), t.data_ptr(), self.mean.ctypes.data, oh, ow, out[i].data_ptr(),
+                                             torch.cuda.current_stream().cuda_stream)
+        self._keep = dev                                                     # raw buffers stay referenced until the next batch
+        return out
+
+
+def _collate_test(batch):
+    imgs, sizes, names = zip(*batch)
+    same = all(i.shape == imgs[0].shape for i in imgs)
+    return torch.stack(imgs) if same else list(imgs), torch.from_numpy(np.stack(sizes)), list(names)
+
+
 class _Sample(ctypes.Structure):          # include/skd.h: skd_cs_sample
     _fields_ = [("image", ctypes.c_void_p), ("label", ctypes.c_void_p), ("src_h", ctypes.c_int), ("src_w", ctypes.c_int),
                 ("f_scale", ctypes.c_double), ("scaled_h", ctypes.c_int), ("scaled_w", ctypes.c_int), ("h_off", ctypes.c_int),
@@ -142,19 +215,28 @@ def _collate(batch):
 
 class CSDataLoader:
     """Drop-in for `data.DataLoader(CSDataSet(...), batch_size=..., shuffle=True, num_workers=4, pin_memory=True)` of
-    train_and_eval.py:13-15: iterating it yields `(images, labels, size, name)` with images / labels already augmented and on the GPU."""
+    train_and_eval.py:13-15: iterating it yields `(images, labels, size, name)` with images / labels already augmented and on the GPU.
+    With a `CSDataTestSet` (test.py:9-10) it yields `(images, size, name)`, images mean-subtracted and padded on the GPU."""
 
     def __init__(self, dataset, batch_size=1, shuffle=False, num_workers=0, pin_memory=True, drop_last=False, label_dtype=torch.int64,
                  device=None):
         self.dataset = dataset
+        self.test = isinstance(dataset, CSDataTestSet)
         self.loader = data.DataLoader(dataset, batch_size=batch_size, shuffle=shuffle, num_workers=num_workers, pin_memory=pin_memory,
-                                      drop_last=drop_last, collate_fn=_collate)
-        self.augment = DeviceAugment((dataset.crop_h, dataset.crop_w), dataset.mean, dataset.ignore_label, label_dtype, device)
+                                      drop_last=drop_last, collate_fn=_collate_test if self.test else _collate)
+        if self.test:
+            self.augment = DeviceTestPreprocess((dataset.crop_h, dataset.crop_w), dataset.mean, device)
+        else:
+            self.augment = DeviceAugment((dataset.crop_h, dataset.crop_w), dataset.mean, dataset.ignore_label, label_dtype, device)
 
     def __len__(self):
         return len(self.loader)
 
     def __iter__(self):
+        if self.test:
+            for images, sizes, names in self.loader:
+                yield self.augment(images), sizes, names
+            return
         for images, labels, augs, sizes, names in self.loader:
             out_i, out_l = self.augment(images, labels, augs)
             yield out_i, out_l, sizes, names
