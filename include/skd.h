@@ -365,6 +365,49 @@ int skd_cs_augment_batch(int n, const skd_cs_sample* samples, int crop_h, int cr
    double -- and zero padding on the bottom / right; out_h = max(H, crop_h), out_w = max(W, crop_w) (no crop).  mean_bgr: HOST, 3. */
 int skd_cs_test_preprocess(int H, int W, const unsigned char* image, const double* mean_bgr, int out_h, int out_w, float* out, cudaStream_t);
 
+/* ---- H. ESPNet-C student (networks/espnet.py, csrc/espnet.cu).  NHWC rows [P = N*H*W][...] with explicit row pitches in floats;
+        a channel slice of a concat buffer is passed as a pointer to its first channel.  Plain affine BatchNorm2d (gamma = w, not
+        ABN's |w| + eps) followed by a per-channel PReLU (y = z if z > 0 else alpha * z).  Fixed-order reductions throughout. ---- */
+long long skd_bnprelu_workspace_doubles(long long P, int C);   /* workspace of the statistics / backward reductions below */
+/* replaces nn.BatchNorm2d's training-mode statistics: mean, biased var; running_mean / running_var (may be NULL) updated with momentum
+   and the unbiased variance n / (n - 1); *num_batches_tracked += 1 (may be NULL) */
+int skd_bnprelu_stats(long long P, int C, const float* x, int ldx, float momentum, float* running_mean, float* running_var,
+                      long long* num_batches_tracked, float* mean, float* var, double* workspace, cudaStream_t);
+/* replaces ESPNet's torch.cat([d1, a1, a2, a3, a4], 1) (+ input) with a1 = d2, a2 = a1 + d4, a3 = a2 + d8, a4 = a3 + d16: writes the
+   combine [P][n1 + 4n] to out and, when mean != NULL, the BatchNorm statistics of it in the same pass (as skd_bnprelu_stats).
+   d1 has pitch ld1, d2..d16 pitch ldn, residual (may be NULL) pitch ldr */
+int skd_esp_combine(long long P, int n1, int n, const float* d1, int ld1, const float* d2, const float* d4, const float* d8,
+                    const float* d16, int ldn, const float* residual, int ldr, float* out, int ldo, float momentum,
+                    float* running_mean, float* running_var, long long* num_batches_tracked, float* mean, float* var,
+                    double* workspace, cudaStream_t);
+/* replaces BatchNorm2d + PReLU forward: out = prelu((x - mean) * w * rsqrt(var + eps) + b) for C channels, zeros in channels
+   C .. out_channels - 1 (the channel padding the next convolution reads).  Eval mode passes the running statistics. */
+int skd_bnprelu_apply(long long P, int C, const float* x, int ldx, const float* mean, const float* var, const float* weight,
+                      const float* bias, const float* alpha, float eps, float* out, int ldo, int out_channels, cudaStream_t);
+/* backward reduce pass: dweight = sum dz * xhat, dbias = sum dz, dalpha = sum_{z <= 0} z * dout (each may be NULL), dz = dout * prelu'(z);
+   coef[2C] = (mean dz, mean dz * xhat) for the dx pass */
+int skd_bnprelu_bwd_reduce(long long P, int C, const float* x, int ldx, const float* dout, int ldd, const float* mean, const float* var,
+                           const float* weight, const float* bias, const float* alpha, float eps, float* dweight, float* dbias,
+                           float* dalpha, float* coef, double* workspace, cudaStream_t);
+/* dx pass: dx = w * rsqrt(var + eps) * (dz - coef[c] - xhat * coef[C + c]) (training) or w * rsqrt(var + eps) * dz (running
+   statistics); channels C .. dx_channels - 1 are written as zeros */
+int skd_bnprelu_bwd_dx(long long P, int C, const float* x, int ldx, const float* dout, int ldd, const float* mean, const float* var,
+                       const float* weight, const float* bias, const float* alpha, float eps, int training, const float* coef, float* dx,
+                       int lddx, int dx_channels, cudaStream_t);
+/* the same dx pass over an ESP combine (x = the combine, C = n1 + 4n), written as the branch gradients: dd1 = g[0:n1],
+   dd16 = g4, dd8 = g3 + g4, dd4 = g2 + g3 + g4, dd2 = g1 + ... + g4 (suffix sums of the HFF slices g1..g4), pad channels up to the
+   pitches zero; dres (may be NULL) = g, the gradient of the residual input */
+int skd_esp_bwd_dx(long long P, int n1, int n, const float* x, int ldx, const float* dout, int ldd, const float* mean, const float* var,
+                   const float* weight, const float* bias, const float* alpha, float eps, int training, const float* coef, float* dd1,
+                   int ld1, float* dd2, float* dd4, float* dd8, float* dd16, int ldn, float* dres, int ldr, cudaStream_t);
+/* replaces ESPNet's InputProjectionA step nn.AvgPool2d(3, stride=2, padding=1) (count_include_pad): src [N][H][W] pitch lds, C
+   channels -> dst [N][(H+1)/2][(W+1)/2] pitch ldd; forward only (the image needs no gradient) */
+int skd_avgpool3x3s2(int N, int H, int W, int C, const float* src, int lds, float* dst, int ldd, cudaStream_t);
+/* replaces F.interpolate(t, (H, W), mode='bilinear', align_corners=True) of the teacher's logits / feature (NetModel puts them on
+   the student's grid): src (N, C, h, w) with element strides (sn, sc, sp) -> out dense NHWC [N][H][W][C]; forward only */
+int skd_resample_bilinear_nhwc(int N, int C, int h, int w, const float* src, long long sn, long long sc, long long sp, int H, int W,
+                               float* out, cudaStream_t);
+
 #ifdef __cplusplus
 }
 #endif

@@ -85,6 +85,18 @@ __device__ __forceinline__ double zoom_lerp(double p00, double p01, double p10, 
   return a;
 }
 
+// bilinear (align_corners) value of one plane p (pixel stride sp, h x w) at (y, x) of the up-/down-sampled grid, ry = (h - 1) / (H - 1):
+// ATen's source-index rule (eval.cu's score accumulation, espnet.cu's teacher resample)
+__device__ __forceinline__ float up_at(const float* __restrict__ p, long long sp, int h, int w, float ry, float rx, int y, int x) {
+  const float fy = y * ry, fx = x * rx;
+  const int y0 = min((int)fy, h - 1), x0 = min((int)fx, w - 1);
+  const int y1i = min(y0 + 1, h - 1), x1i = min(x0 + 1, w - 1);
+  const float ly = fy - y0, lx = fx - x0;
+  const float v00 = __ldg(p + ((long long)y0 * w + x0) * sp), v01 = __ldg(p + ((long long)y0 * w + x1i) * sp);
+  const float v10 = __ldg(p + ((long long)y1i * w + x0) * sp), v11 = __ldg(p + ((long long)y1i * w + x1i) * sp);
+  return (1.f - ly) * ((1.f - lx) * v00 + lx * v01) + ly * ((1.f - lx) * v10 + lx * v11);
+}
+
 // Cityscapes label id -> train id (reference dataset/datasets.py:146-151, ids 0..33; everything else passes through).  The one
 // copy of the table: augment.cu maps labels with it, skd_cityscapes_id_tables derives the reverse (train id -> label id) map
 // that evaluation writes test-split predictions with.

@@ -14,17 +14,6 @@ using namespace skd;
 
 namespace {
 
-// bilinear (align_corners) value of one class plane p at (y, x) of the tile: ATen's source-index rule
-__device__ __forceinline__ float up_at(const float* __restrict__ p, long long sp, int h, int w, float ry, float rx, int y, int x) {
-  const float fy = y * ry, fx = x * rx;
-  const int y0 = min((int)fy, h - 1), x0 = min((int)fx, w - 1);
-  const int y1i = min(y0 + 1, h - 1), x1i = min(x0 + 1, w - 1);
-  const float ly = fy - y0, lx = fx - x0;
-  const float v00 = __ldg(p + ((long long)y0 * w + x0) * sp), v01 = __ldg(p + ((long long)y0 * w + x1i) * sp);
-  const float v10 = __ldg(p + ((long long)y1i * w + x0) * sp), v11 = __ldg(p + ((long long)y1i * w + x1i) * sp);
-  return (1.f - ly) * ((1.f - lx) * v00 + lx * v01) + ly * ((1.f - lx) * v10 + lx * v11);
-}
-
 enum AccMode : int { kPlain = 0, kWeighted = 1, kWeightedPair = 2 };
 
 // full[(y1+y)*W + x1+x][c] += bilinear(logits)[c][y][x] for y < vh, x < vw (the tile may be padded beyond the image: only the valid

@@ -345,6 +345,172 @@ class ABN(torch.autograd.Function):
         return dx, dw, db, None, None, None, None, None, None, None, dres, None, None
 
 
+# ------------------------------------------------------------------------------------------------ ESPNet-C (networks/espnet.py)
+# Activations between ESPNet-C layers are dense NHWC tensors whose channel count is padded to a multiple of 4 (19 -> 20, 25 -> 28,
+# 131 -> 132) with zero pad channels, so every convolution reads them in place; weights are zero-padded to match.
+def _esp_conv(x, w_ohwi, stride, pad, dil, precise):
+    """Forward convolution of a channel-padded input with channel-padded OHWI weights; 3xTF32 when `precise`."""
+    if precise:
+        return ops.conv2d_fwd_3xtf32(x, w_ohwi, stride, pad, dil)
+    return ops.conv2d_fwd(x, w_ohwi, stride, pad, dil)
+
+
+def _esp_wgrad(x, dy, weight, stride, pad, dil):
+    """(Cout, Cin, KH, KW)-shaped weight gradient (a view of the channel-padded OHWI result).  Main stream: autograd accumulates the
+    returned view into .grad right away."""
+    cout, cin, kh, kw = weight.shape
+    dw = ops.conv2d_wgrad(x, dy, (kh, kw), stride, pad, dil)
+    return dw[:cout, :, :, :cin].permute(0, 3, 1, 2)
+
+
+def _esp_weight(weight, cin_p):
+    w = ops.weight_ohwi(weight)
+    return _padded_weight(w, ops.pad4(w.shape[0]), cin_p)
+
+
+class EspConv(torch.autograd.Function):
+    """One convolution between channel-padded NHWC tensors (ESPNet-C's classifier): (N, pad4(Cout), OH, OW) out, zero pad channels."""
+
+    @staticmethod
+    def forward(ctx, x, weight, stride, pad, dil, precise):
+        wp = _esp_weight(weight, x.shape[1])
+        y = _esp_conv(x, wp, stride, pad, dil, precise)
+        ctx.save_for_backward(x, wp, weight)
+        ctx.cfg = (stride, pad, dil)
+        return y
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, dy):
+        x, wp, weight = ctx.saved_tensors
+        stride, pad, dil = ctx.cfg
+        dy = ops.to_nhwc(dy)
+        dx = ops.conv2d_dgrad(dy, wp, tuple(x.shape), stride, pad, dil) if ctx.needs_input_grad[0] else None
+        dw = _esp_wgrad(x, dy, weight, stride, pad, dil) if ctx.needs_input_grad[1] else None
+        return dx, dw, None, None, None, None
+
+
+def _bn_stats(x, training, momentum, rm, rv, nbt):
+    if training:
+        return ops.bnprelu_stats(x, momentum, rm, rv, nbt)
+    return torch.stack([rm, rv])
+
+
+class EspBnPrelu(torch.autograd.Function):
+    """BatchNorm2d(eps) + PReLU over the channel concatenation of `pieces` (and, with `image`, its average pooling `ipa_times` times,
+    the InputProjectionA channels): ESPNet-C's CBR after its convolution and the BR blocks b1 / b2 / b3.  The concatenation is one
+    channel-padded NHWC buffer; the pooled image is written straight into its slice (forward only: the image has no gradient).
+    Returns the channel-padded output and, for b1, the pooled image slice that b2's projection pools once more."""
+
+    @staticmethod
+    def forward(ctx, image, ipa, weight, bias, alpha, running_mean, running_var, nbt, training, momentum, eps, *pieces):
+        n, _, h, w = pieces[0].shape
+        widths = [p.shape[1] for p in pieces]
+        c = sum(widths) + (3 if image is not None else 0)
+        cp = ops.pad4(c)
+        if len(pieces) == 1 and image is None and ops.nhwc_meta(pieces[0])[4] == c:
+            x = pieces[0]
+        else:
+            x = ops.empty_nhwc(n, c, h, w, pieces[0].device, pitch=cp)
+            off = 0
+            for p, k in zip(pieces, widths):
+                ops.slice_copy(p, 0, x, off, k)
+                off += k
+            if image is not None:
+                src = image
+                for _ in range(ipa):
+                    hh, ww = (src.shape[2] + 1) // 2, (src.shape[3] + 1) // 2
+                    dst = x[:, off:off + 3] if (hh, ww) == (h, w) else ops.empty_nhwc(n, 3, hh, ww, x.device)
+                    ops.avgpool3x3s2(src, dst)
+                    src = dst
+        st = _bn_stats(x, training, momentum, running_mean, running_var, nbt)
+        y = ops.bnprelu_apply(x, st[0], st[1], weight, bias, alpha, eps, out_channels=cp)
+        ctx.save_for_backward(x, st, weight, bias, alpha)
+        ctx.cfg = (training, eps, widths)
+        projected = x[:, c - 3:c] if image is not None else None
+        if projected is not None:
+            ctx.mark_non_differentiable(projected)
+        return y, projected
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, dy, _dproj):
+        x, st, weight, bias, alpha = ctx.saved_tensors
+        training, eps, widths = ctx.cfg
+        dy = ops.to_nhwc(dy)
+        dw, db, da, coef = ops.bnprelu_bwd_reduce(x, dy, st[0], st[1], weight, bias, alpha, eps)
+        dx = ops.bnprelu_bwd_dx(x, dy, st[0], st[1], weight, bias, alpha, eps, training, coef, dx_channels=ops.pad4(x.shape[1]))
+        dpieces, off = [], 0
+        if len(widths) == 1 and dx.shape[1] == widths[0]:
+            dpieces = [dx]
+        else:
+            n, _, h, w = dx.shape
+            for k in widths:
+                d = ops.empty_nhwc(n, k, h, w, dx.device)
+                ops.slice_copy(dx, off, d, 0, k)
+                dpieces.append(d)
+                off += k
+        return (None, None, dw, db, da, None, None, None, None, None, None) + tuple(dpieces)
+
+
+class EspBlock(torch.autograd.Function):
+    """One ESP module of ESPNet-C -- DownSamplerB (`c1` 3x3 / stride 2) or DilatedParllelResidualBlockB (`c1` 1x1, residual `add`):
+    reduce -> five dilated 3x3 branches (d = 1, 2, 4, 8, 16) -> hierarchical feature fusion + concatenation (+ input) -> BatchNorm ->
+    PReLU.  Forward: six wgmma convolutions (3xTF32 when `precise`), then one pass that forms the combine and its batch statistics,
+    then the BN + PReLU apply.  Backward: one reduce pass and one pass that writes every branch's gradient (suffix sums of the fused
+    slices) and the residual's; the five branch data gradients are summed into d(c1 out) through the convolution epilogue's residual
+    input, in a fixed order."""
+
+    @staticmethod
+    def forward(ctx, x, w_c1, w_d1, w_d2, w_d4, w_d8, w_d16, bn_w, bn_b, alpha, running_mean, running_var, nbt, stride, add, training,
+                momentum, eps, precise):
+        n_red, n1 = w_d2.shape[0], w_d1.shape[0]
+        k = w_c1.shape[2]
+        wc1 = _esp_weight(w_c1, x.shape[1])
+        t = _esp_conv(x, wc1, stride, (k - 1) // 2, 1, precise)                         # (N, pad4(n), H', W')
+        wbr = [_esp_weight(wd, t.shape[1]) for wd in (w_d1, w_d2, w_d4, w_d8, w_d16)]
+        outs = [_esp_conv(t, wb, 1, d, d, precise) for wb, d in zip(wbr, (1, 2, 4, 8, 16))]
+        branches = [outs[0][:, :n1]] + [o[:, :n_red] for o in outs[1:]]
+        N, _, h, w = t.shape
+        c = n1 + 4 * n_red
+        comb = ops.empty_nhwc(N, c, h, w, x.device)
+        if training:
+            st = ops.esp_combine(branches, x if add else None, comb, momentum, running_mean, running_var, nbt)
+        else:
+            ops.esp_combine(branches, x if add else None, comb, stats=False)
+            st = torch.stack([running_mean, running_var])
+        y = ops.bnprelu_apply(comb, st[0], st[1], bn_w, bn_b, alpha, eps)
+        ctx.save_for_backward(x, t, comb, st, wc1, *wbr, w_c1, w_d1, w_d2, w_d4, w_d8, w_d16, bn_w, bn_b, alpha)
+        ctx.cfg = (stride, add, training, eps, n1, n_red)
+        return y
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, dy):
+        x, t, comb, st, wc1, *rest = ctx.saved_tensors
+        wbr, params = rest[:5], rest[5:]
+        w_c1, w_d1, w_d2, w_d4, w_d8, w_d16, bn_w, bn_b, alpha = params
+        stride, add, training, eps, n1, n_red = ctx.cfg
+        dy = ops.to_nhwc(dy)
+        dbw, dbb, da, coef = ops.bnprelu_bwd_reduce(comb, dy, st[0], st[1], bn_w, bn_b, alpha, eps)
+        dds, dres = ops.esp_bwd_dx(comb, dy, st[0], st[1], bn_w, bn_b, alpha, eps, training, coef, n1, n_red,
+                                   add and ctx.needs_input_grad[0])
+        dt = None
+        for dd, wb, d in zip(dds, wbr, (1, 2, 4, 8, 16)):                # d(c1 out) = sum of the branch data gradients, in order
+            dt = ops.conv2d_dgrad(dd, wb, tuple(t.shape), 1, d, d, residual=dt)
+        k = w_c1.shape[2]
+        dx = None
+        if ctx.needs_input_grad[0]:
+            if stride == 1:
+                dx = ops.conv2d_dgrad(dt, wc1, tuple(x.shape), 1, (k - 1) // 2, 1, residual=dres)
+            else:
+                dx = ops.conv2d_dgrad(dt, wc1, tuple(x.shape), stride, (k - 1) // 2, 1)
+                assert dres is None
+        dws = [_esp_wgrad(t, dd, wd, 1, d, d) for dd, wd, d in zip(dds, (w_d1, w_d2, w_d4, w_d8, w_d16), (1, 2, 4, 8, 16))]
+        dwc1 = _esp_wgrad(x, dt, w_c1, stride, (k - 1) // 2, 1)
+        return (dx, dwc1, *dws, dbw, dbb, da) + (None,) * 9
+
+
 class MaxPool3x3s2(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x):

@@ -24,9 +24,10 @@ import torch.distributed as dist
 from .. import functions as Fn
 from .. import ops
 from ..optim import FlatSGD
-from ..utils.criterion import (CriterionAdditionalGP, CriterionAdv, CriterionAdvForG, CriterionDSN, CriterionOhemDSN,
-                               CriterionPairWiseforWholeFeatAfterPool, CriterionPixelWise)
+from ..utils.criterion import (CriterionAdditionalGP, CriterionAdv, CriterionAdvForG, CriterionCrossEntropy, CriterionDSN,
+                               CriterionOhemDSN, CriterionPairWiseforWholeFeatAfterPool, CriterionPixelWise)
 from ..utils.utils import load_D_model, load_S_model, load_T_model
+from .espnet import ESPNet_C
 from .evaluate import evaluate_main
 from .pspnet_combine import BasicBlock, Bottleneck, Res_pspnet
 from .sagan_models import Discriminator
@@ -67,7 +68,15 @@ class NetModel():
         self.device = device
         self.world = dist.get_world_size() if dist.is_available() and dist.is_initialized() else 1
 
-        student = Res_pspnet(BasicBlock, [2, 2, 2, 2], num_classes=args.classes_num)
+        self.student_kind = str(_arg(args, "student", "resnet18"))
+        if self.student_kind == "resnet18":
+            student = Res_pspnet(BasicBlock, [2, 2, 2, 2], num_classes=args.classes_num)
+        elif self.student_kind == "espnet_c":
+            if _arg(args, "sync_bn", False):
+                raise ValueError("sync_bn is not available with the ESPNet-C student (its BatchNorm statistics are per rank)")
+            student = ESPNet_C(args.classes_num, _arg(args, "espnet_p", 2), _arg(args, "espnet_q", 8))
+        else:
+            raise ValueError("student must be 'resnet18' or 'espnet_c' (got %r)" % self.student_kind)
         load_S_model(args, student, False)                         # ImageNet init or S_resume (utils/utils.py:93-127)
         self.student = student.float().to(device).train()
         if _arg(args, "sync_bn", False):                          # cross-rank batch statistics (the reference's InPlaceABNSync semantics)
@@ -111,7 +120,10 @@ class NetModel():
                 self.G_solver.enable_overlap(int(_arg(args, "allreduce_buckets", 4)))
 
         if _arg(args, "ohem", False):                             # OHEM task loss (the reference imports CriterionOhemDSN, kd_model.py:18)
+            # (ESPNet-C: head 0 only, preds[1] is None)
             self.criterion = CriterionOhemDSN(thresh=_arg(args, "ohem_thres", 0.7), min_kept=_arg(args, "ohem_keep", 100000))
+        elif self.student_kind == "espnet_c":                     # no auxiliary head: single-head cross entropy
+            self.criterion = CriterionCrossEntropy()
         else:
             self.criterion = CriterionDSN()
         self.criterion_pixel_wise = CriterionPixelWise()
@@ -187,6 +199,7 @@ class NetModel():
             with torch.no_grad():
                 self.preds_T = self.parallel_teacher.eval()(images)
             self.preds_S = self.parallel_student.train()(images)
+            self._resample_teacher()
             return
         # the frozen teacher and the student are independent until the losses: the teacher's forward goes to a second stream, so the
         # student's HBM-bound passes (ABN statistics / apply, pooling) run under the teacher's tensor-bound convolutions (one
@@ -200,6 +213,19 @@ class NetModel():
             self.preds_T = self.parallel_teacher.eval()(images)
         self.preds_S = self.parallel_student.train()(images)
         cur.wait_stream(side)
+        self._resample_teacher()
+
+    def _resample_teacher(self):
+        """Students on another grid than the teacher (ESPNet-C: 45x60 at 360x480, PSPNet's ceil-mode pool: 46x61): the two teacher
+        tensors the distillation terms read, preds_T[0] and preds_T[-5], are resized onto the student's grid (bilinear,
+        align_corners=True; forward only, the teacher is frozen).  Equal grids (the ResNet18 student): nothing runs."""
+        size = tuple(self.preds_S[0].shape[2:])
+        if tuple(self.preds_T[0].shape[2:]) == size:
+            return
+        preds = list(self.preds_T)
+        for i in (0, len(preds) - 5):
+            preds[i] = ops.resample_nhwc(preds[i], *size)
+        self.preds_T = preds
 
     def student_backward(self):
         args = self.args
@@ -225,7 +251,9 @@ class NetModel():
             # the ONE collective of the path (teacher frozen): bucketed NCCL all-reduce of the flat student gradient, issued from
             # inside the backward pass as each range of parameters completes (utils/parallel.py:54-63,155 semantics: mean over ranks)
             self.G_solver.begin_overlapped_reduce(self.world)
-        if self.overlap_streams:
+        if self.overlap_streams and self.student_kind == "resnet18":
+            # (ESPNet-C issues its weight gradients on the main stream: no side-stream window, so no join on an idle stream, which
+            # a CUDA-graph capture would reject)
             Fn.WgradOverlap.begin()
             if Fn.WgradOverlap.stream not in self.G_solver.producer_streams:
                 self.G_solver.producer_streams.append(Fn.WgradOverlap.stream)

@@ -233,14 +233,20 @@ def conv2d_fwd_3xtf32(x, w_ohwi, stride, pad, dil, shift=None):
     return out
 
 
-def conv2d_dgrad(dy, w_ohwi, x_shape, stride, pad, dil, round_tf32=False, force_direct=False):
-    """dx for y = conv(x, w).  stride 1: forward wgmma kernel on dy with the flipped/transposed weights."""
+def conv2d_dgrad(dy, w_ohwi, x_shape, stride, pad, dil, round_tf32=False, force_direct=False, residual=None):
+    """dx for y = conv(x, w).  stride 1: forward wgmma kernel on dy with the flipped/transposed weights.  `residual` (stride-1
+    wgmma path only): dx + residual, added by the kernel's epilogue -- the fixed-order sum of several data gradients into one
+    tensor (ESPNet-C's branches)."""
     n, cin, h, w = x_shape
     cout, kh, kw, _ = w_ohwi.shape
     L = lib()
     dn, dc, doh, dow, ldy = nhwc_meta(dy)
     dx = empty_nhwc(n, cin, h, w, dy.device)
-    if stride == 1 and not force_direct and cout % 4 == 0 and ldy % 4 == 0:
+    wgmma = stride == 1 and not force_direct and cout % 4 == 0 and ldy % 4 == 0
+    if residual is not None and not (wgmma and cin % 4 == 0):
+        raise ValueError("conv2d_dgrad: a residual needs the stride-1 wgmma path (channel counts padded to multiples of 4)")
+    ldr = nhwc_meta(residual)[4] if residual is not None else 0
+    if wgmma:
         wt = torch.empty((cin, kh, kw, cout), device=dy.device, dtype=torch.float32)
         L.skd_weight_flip_transpose(cout, cin, kh, kw, _p(w_ohwi), _p(wt), 0, _st())
         log = CONV_EVENT_LOG
@@ -248,7 +254,7 @@ def conv2d_dgrad(dy, w_ohwi, x_shape, stride, pad, dil, round_tf32=False, force_
             ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             ev0.record()
         L.skd_conv2d_fwd_sm100(n, doh, dow, cout, cin, kh, kw, 1, dil * (kh - 1) - pad, dil, _p(dy), ldy, _p(wt), _p(dx), cin,
-                               None, None, None, 0, 0, 0.0, int(round_tf32), _st())
+                               None, None, _p(residual), ldr, 0, 0.0, int(round_tf32), _st())
         if log is not None:
             ev1.record()
             log.append((ev0, ev1, 2.0 * n * h * w * cin * cout * kh * kw, ("dgrad", n, cout, doh, dow, cin, kh, 1, dil)))
@@ -587,6 +593,108 @@ def pairwise_affinity_bwd_sm100(E, pS, rS, arg, grad_out, feat_like):
         if feat_like.dim() == 4 and feat_like.stride(1) == 1 else torch.zeros_like(feat_like)
     L.skd_pairwise_scatter(n, nodes, cs, _p(dpooled), _p(arg), _p(dF), *pixel_strides(dF), _st())
     return dF
+
+
+# ------------------------------------------------------------------------------------------------ ESPNet-C (csrc/espnet.cu)
+def _rows(t):
+    """-> (P, C, pitch) of an NHWC-stored (possibly channel-sliced) tensor."""
+    n, c, h, w, pitch = nhwc_meta(t)
+    return n * h * w, c, pitch
+
+
+def bnprelu_stats(x, momentum, running_mean, running_var, num_batches_tracked):
+    """Batch mean / biased variance of x's channels; running statistics and the batch counter updated in place (may be None)."""
+    _f32(x)
+    P, c, ldx = _rows(x)
+    st = torch.empty(2, c, device=x.device)
+    ws = torch.empty(lib().skd_bnprelu_workspace_doubles(P, c), device=x.device, dtype=torch.float64)
+    lib().skd_bnprelu_stats(P, c, _p(x), ldx, momentum, _p(running_mean), _p(running_var), _p(num_batches_tracked), _p(st[0]), _p(st[1]),
+                            _p(ws), _st())
+    return st
+
+
+def esp_combine(branches, residual, out, momentum=0.0, running_mean=None, running_var=None, num_batches_tracked=None, stats=True):
+    """ESP combine of the five branch outputs (d1, d2, d4, d8, d16: NHWC tensors, channel-padded) plus the optional residual into `out`
+    ((N, n1 + 4n, H, W) NHWC); -> batch statistics (2, C) or None."""
+    d1, d2, d4, d8, d16 = branches
+    P, n1, ld1 = _rows(d1)
+    _, n, ldn = _rows(d2)
+    for t in (d4, d8, d16):
+        if _rows(t)[2] != ldn:
+            raise ValueError("Non-contiguous input")
+    _, c, ldo = _rows(out)
+    ldr = _rows(residual)[2] if residual is not None else 0
+    L = lib()
+    st = torch.empty(2, c, device=out.device) if stats else None
+    ws = torch.empty(L.skd_bnprelu_workspace_doubles(P, c), device=out.device, dtype=torch.float64) if stats else None
+    L.skd_esp_combine(P, n1, n, _p(d1), ld1, _p(d2), _p(d4), _p(d8), _p(d16), ldn, _p(residual), ldr, _p(out), ldo, momentum,
+                      _p(running_mean), _p(running_var), _p(num_batches_tracked), _p(st[0]) if stats else None,
+                      _p(st[1]) if stats else None, _p(ws), _st())
+    return st
+
+
+def bnprelu_apply(x, mean, var, weight, bias, alpha, eps, out=None, out_channels=None):
+    """prelu(bn(x)) -> `out` (default: a fresh NHWC tensor with `out_channels` >= C channels, the extra ones zero)."""
+    _f32(x)
+    n, c, h, w, ldx = nhwc_meta(x)
+    cw = out_channels or c
+    if out is None:
+        out = empty_nhwc(n, cw, h, w, x.device)
+    ldo = nhwc_meta(out)[4]
+    lib().skd_bnprelu_apply(n * h * w, c, _p(x), ldx, _p(mean), _p(var), _p(weight), _p(bias), _p(alpha), eps, _p(out), ldo, cw, _st())
+    return out
+
+
+def bnprelu_bwd_reduce(x, dout, mean, var, weight, bias, alpha, eps):
+    """-> (dweight, dbias, dalpha) and the (2, C) coefficients of the dx pass."""
+    P, c, ldx = _rows(x)
+    ldd = _rows(dout)[2]
+    L = lib()
+    red = torch.empty(5, c, device=x.device)             # dweight, dbias, dalpha, mean dz, mean dz*xhat
+    ws = torch.empty(L.skd_bnprelu_workspace_doubles(P, c), device=x.device, dtype=torch.float64)
+    L.skd_bnprelu_bwd_reduce(P, c, _p(x), ldx, _p(dout), ldd, _p(mean), _p(var), _p(weight), _p(bias), _p(alpha), eps, _p(red[0]),
+                             _p(red[1]), _p(red[2]), _p(red[3]), _p(ws), _st())
+    return red[0], red[1], red[2], red[3:5]
+
+
+def bnprelu_bwd_dx(x, dout, mean, var, weight, bias, alpha, eps, training, coef, dx_channels=None):
+    n, c, h, w, ldx = nhwc_meta(x)
+    ldd = nhwc_meta(dout)[4]
+    cw = dx_channels or c
+    dx = empty_nhwc(n, cw, h, w, x.device)
+    lib().skd_bnprelu_bwd_dx(n * h * w, c, _p(x), ldx, _p(dout), ldd, _p(mean), _p(var), _p(weight), _p(bias), _p(alpha), eps,
+                             int(training), _p(coef), _p(dx), cw, cw, _st())
+    return dx
+
+
+def esp_bwd_dx(x, dout, mean, var, weight, bias, alpha, eps, training, coef, n1, n, want_dres):
+    """-> (dd1, dd2, dd4, dd8, dd16) (channel-padded to multiples of 4, pad channels zero) and dres (or None)."""
+    N, c, h, w, ldx = nhwc_meta(x)
+    ldd = nhwc_meta(dout)[4]
+    dev = x.device
+    dd1 = empty_nhwc(N, pad4(n1), h, w, dev)
+    dds = [empty_nhwc(N, pad4(n), h, w, dev) for _ in range(4)]
+    dres = empty_nhwc(N, c, h, w, dev) if want_dres else None
+    lib().skd_esp_bwd_dx(N * h * w, n1, n, _p(x), ldx, _p(dout), ldd, _p(mean), _p(var), _p(weight), _p(bias), _p(alpha), eps,
+                         int(training), _p(coef), _p(dd1), pad4(n1), *[_p(t) for t in dds], pad4(n), _p(dres), c, _st())
+    return (dd1, *dds), dres
+
+
+def avgpool3x3s2(src, out):
+    """nn.AvgPool2d(3, 2, 1) of src (N, C, H, W) NHWC(-pitched) into out (N, C, (H+1)//2, (W+1)//2) NHWC(-pitched), in place."""
+    n, c, h, w, lds = nhwc_meta(src)
+    ldd = nhwc_meta(out)[4]
+    lib().skd_avgpool3x3s2(n, h, w, c, _p(src), lds, _p(out), ldd, _st())
+    return out
+
+
+def resample_nhwc(t, h, w):
+    """Bilinear (align_corners=True) resize of an (N, C, H', W') tensor to (N, C, h, w), NHWC output; forward only."""
+    _f32(t)
+    n, c = t.shape[:2]
+    out = torch.empty((n, h, w, c), device=t.device, dtype=torch.float32)
+    lib().skd_resample_bilinear_nhwc(n, c, t.shape[2], t.shape[3], _p(t), *pixel_strides(t), h, w, _p(out), _st())
+    return out.permute(0, 3, 1, 2)
 
 
 def sgd_step_nvls(lo, hi, param_mc, grad_mc, param_local, buf, lr_dev, momentum, weight_decay, grad_scale):

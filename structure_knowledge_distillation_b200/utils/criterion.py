@@ -5,6 +5,7 @@
   CriterionPairWiseforWholeFeatAfterPool      utils/criterion.py:228-245   (alias: CriterionPairWise, the name the
                                               north star uses; it does not exist in the reference tree)
   CriterionDSN                                utils/criterion.py:168-188
+  CriterionCrossEntropy                       named at kd_model.py:79 (single head: the ESPNet-C student's task loss)
   OhemCrossEntropy2d                          utils/criterion.py:11-90
   CriterionOhemDSN                            utils/criterion.py:190-209
   CriterionAdv / CriterionAdvForG             utils/criterion.py:122-166
@@ -64,6 +65,18 @@ class CriterionDSN(nn.Module):
 
     def forward(self, preds, target):
         return Fn.DsnCrossEntropy.apply(preds[0], preds[1], target, self.ignore_index, 1.0, 0.4)
+
+
+class CriterionCrossEntropy(nn.Module):
+    """Single-head cross entropy, CE(up(preds[0])) with bilinear align_corners to the label size, mean over the valid pixels (the
+    class the reference names for students without an auxiliary head, kd_model.py:79): the task loss of the ESPNet-C student."""
+
+    def __init__(self, ignore_index=255, use_weight=True, reduce=True):
+        super().__init__()
+        self.ignore_index = ignore_index
+
+    def forward(self, preds, target):
+        return Fn.DsnCrossEntropy.apply(preds[0], None, target, self.ignore_index, 1.0, 0.0)
 
 
 class OhemCrossEntropy2d(nn.Module):

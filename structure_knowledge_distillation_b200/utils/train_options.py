@@ -12,7 +12,8 @@ DEFAULTS = dict(
     adv_conv_dim=64, lambda_gp=10.0, lambda_d=0.1, lambda_pi=10.0, lambda_pa=0.5, pool_scale=0.5, preprocess_GAN_mode=1,
     lr_g=1e-2, lr_d=4e-4, best_mean_IU=0.0, gpu_num=1,
     cuda_graph=False,        # ours: capture the step into CUDA graphs after 3 eager steps (NetModel.enable_cuda_graphs)
-    ohem=False, ohem_thres=0.7, ohem_keep=100000)   # ours: CriterionOhemDSN(thresh=ohem_thres, min_kept=ohem_keep) as the CE term
+    ohem=False, ohem_thres=0.7, ohem_keep=100000,   # ours: CriterionOhemDSN(thresh=ohem_thres, min_kept=ohem_keep) as the CE term
+    student='resnet18', espnet_p=2, espnet_q=8)     # ours: 'resnet18' (ResNet18-PSP) or 'espnet_c' (ESPNet-C with p / q ESP blocks)
 
 
 def make_args(**overrides):
