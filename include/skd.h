@@ -182,6 +182,10 @@ int skd_conv2d_fwd_sm100_splitk(int N, int H, int W, int Cin, int Cout, int KH, 
 int skd_conv2d_fwd_sm100_strided(int N, int H, int W, int Cin, int Cout, int KH, int KW, int stride, int pad, int dil, const float* x,
                                  int ldx, const float* w, float* y, long long y_pix, long long y_row, long long y_img, int out_h, int out_w,
                                  int round_tf32, cudaStream_t);   /* out_h/out_w > 0 override the output extent (far-end zero padding) */
+/* the strided-output form with split-precision operands (x_lo, w_lo required; skd_split_tf32 makes them) */
+int skd_conv2d_fwd_sm100_strided_3xtf32(int N, int H, int W, int Cin, int Cout, int KH, int KW, int stride, int pad, int dil,
+                                        const float* x_hi, const float* x_lo, int ldx, const float* w_hi, const float* w_lo, float* y,
+                                        long long y_pix, long long y_row, long long y_img, cudaStream_t);
 /* wgmma weight gradient: dw[Cout][KH][KW][Cin] = sum_pixels dy[p][co] * x[p+tap][ci]; workspace from the size query */
 long long skd_conv2d_wgrad_sm100_workspace_floats(int N, int H, int W, int Cin, int Cout, int KH, int KW, int stride, int pad, int dil);
 int skd_conv2d_wgrad_sm100(int N, int H, int W, int Cin, int Cout, int KH, int KW, int stride, int pad, int dil, const float* x,
@@ -222,6 +226,7 @@ int skd_psp_upsample_fwd(int N, int H, int W, int C, int s, const float* src, in
 long long skd_psp_upsample_bwd_workspace_floats(int N, int H, int C, int s);
 int skd_psp_upsample_bwd(int N, int H, int W, int C, int s, const float* dout, int dout_pitch, int chan_off, float* dsrc,
                          int nbins_total, int first_bin, float* workspace, cudaStream_t);
+/* dst[r][dst_off + c] = src[r][src_off + c], c < C; float4 accesses when every count / offset / pitch is a multiple of 4, else scalar */
 int skd_slice_copy(long long rows, int C, const float* src, int src_pitch, int src_off, float* dst, int dst_pitch, int dst_off, cudaStream_t);
 /* G_solver.step (networks/kd_model.py:74,171): v = mu*v + (g*grad_scale + wd*p); p -= lr*v; lr read from device memory */
 int skd_sgd_step(long long n, float* param, const float* grad, float* momentum_buf, const float* lr, float momentum,
@@ -380,6 +385,8 @@ int skd_esp_combine(long long P, int n1, int n, const float* d1, int ld1, const 
                     const float* d16, int ldn, const float* residual, int ldr, float* out, int ldo, float momentum,
                     float* running_mean, float* running_var, long long* num_batches_tracked, float* mean, float* var,
                     double* workspace, cudaStream_t);
+/* alpha == NULL in the apply, backward reduce and dx passes below is plain BatchNorm2d without the PReLU (the full ESPNet's `br`):
+   slope 1, no dalpha.  Non-NULL alpha computes exactly what it did before this mode existed. */
 /* replaces BatchNorm2d + PReLU forward: out = prelu((x - mean) * w * rsqrt(var + eps) + b) for C channels, zeros in channels
    C .. out_channels - 1 (the channel padding the next convolution reads).  Eval mode passes the running statistics. */
 int skd_bnprelu_apply(long long P, int C, const float* x, int ldx, const float* mean, const float* var, const float* weight,
@@ -407,6 +414,10 @@ int skd_avgpool3x3s2(int N, int H, int W, int C, const float* src, int lds, floa
    the student's grid): src (N, C, h, w) with element strides (sn, sc, sp) -> out dense NHWC [N][H][W][C]; forward only */
 int skd_resample_bilinear_nhwc(int N, int C, int h, int w, const float* src, long long sn, long long sc, long long sp, int H, int W,
                                float* out, cudaStream_t);
+/* adjoint of skd_resample_bilinear_nhwc: dsrc (N, C, h, w; NHWC, pixel pitch lds) = the transpose of the resize applied to dout
+   (dense NHWC [N][H][W][C]).  A gather in fixed order (no atomics): two calls give bit-identical results.  The full ESPNet's
+   discriminator input is its logits resized onto the teacher's grid; this is the gradient of that resize. */
+int skd_resample_bilinear_adjoint_nhwc(int N, int C, int h, int w, const float* dout, int H, int W, float* dsrc, int lds, cudaStream_t);
 
 #ifdef __cplusplus
 }

@@ -511,6 +511,16 @@ extern "C" int skd_conv2d_fwd_sm100_strided(int N, int H, int W, int Cin, int Co
                        0, 0.f, round_tf32, st);
 }
 
+// The strided-output form with split-precision operands (ESPNet's 2x2 / stride-2 transposed convolution: a 1x1 GEMM per output-row
+// parity written straight onto the every-other-row sub-grid, fp32-grade like skd_conv2d_fwd_sm100_3xtf32).
+extern "C" int skd_conv2d_fwd_sm100_strided_3xtf32(int N, int H, int W, int Cin, int Cout, int KH, int KW, int stride, int pad, int dil,
+                                                   const float* x_hi, const float* x_lo, int ldx, const float* w_hi, const float* w_lo,
+                                                   float* y, long long y_pix, long long y_row, long long y_img, cudaStream_t st) {
+  if (!x_lo || !w_lo) { set_error_msg("skd_conv2d_fwd_sm100_strided_3xtf32", "x_lo and w_lo are required"); return 0; }
+  return conv_fwd_impl(N, H, W, Cin, Cout, KH, KW, stride, pad, dil, x_hi, x_lo, ldx, w_hi, w_lo, y, (int)y_pix, y_row, y_img, 0, 0, nullptr, 0,
+                       nullptr, nullptr, nullptr, 0, 0, 0.f, 0, st);
+}
+
 // GEMM view of the same kernel for the pair-wise affinity (utils/utils.py:173-183): D[M][Ncols] = A[M][K] * B[Ncols][K]^T with both
 // operands K-major; optional output, optional fused sum of squares.
 extern "C" int skd_gemm_nt_sm100(int M, int Ncols, int K, const float* A, int lda, const float* B, float* D, int ldd, double* sumsq,

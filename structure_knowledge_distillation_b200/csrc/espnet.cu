@@ -2,6 +2,8 @@
 // through an offset pointer), the ESP module's combine (hierarchical feature fusion + concatenation + residual) fused with the
 // BatchNorm statistics, its backward fused with the BatchNorm + PReLU input-gradient pass, and the input projection (3x3 / stride 2
 // average pooling of the image straight into a concat buffer's channel slice), and the teacher's resample onto the student's grid.
+// The full ESPNet's decoder adds plain BatchNorm (the BN + PReLU kernels with alpha == NULL) and the adjoint of the bilinear resample
+// (the discriminator sees the full-resolution student logits resized onto the teacher's grid).
 //
 // Every reduction adds in a fixed order (row splits fixed by (P, C), partials in double, split order in the finalize pass), so
 // two runs of a step give bit-identical results.  The kernels are scalar per channel: ESPNet-C's channel counts (19, 25, 131, ...)
@@ -41,6 +43,9 @@ __device__ __forceinline__ float esp_combine_at(const EspSrc& s, long long row, 
 }
 
 __device__ __forceinline__ float bn_invstd(float var, float eps) { return 1.f / sqrtf(var + eps); }
+
+// PReLU slope of channel c; alpha == NULL is plain BatchNorm (slope 1: every product below with it is exact, so z and dz pass unchanged)
+__device__ __forceinline__ float slope_of(const float* __restrict__ alpha, int c) { return alpha ? alpha[c] : 1.f; }
 
 // BatchNorm output before the PReLU, z = (x - mean) * invstd * w + b, rounded step by step so that the apply pass and the backward
 // passes (which recompute z for the PReLU mask) agree bit for bit
@@ -122,7 +127,7 @@ apply_kernel(long long P, int C, int Cw, const float* __restrict__ x, int ldx, c
     float y = 0.f;
     if (c < C) {
       const float z = bn_z(x[r * ldx + c], mean[c], bn_invstd(var[c], eps), w[c], b[c]);
-      y = z > 0.f ? z : __fmul_rn(alpha[c], z);
+      y = z > 0.f ? z : __fmul_rn(slope_of(alpha, c), z);
     }
     out[r * ldo + c] = y;
   }
@@ -137,7 +142,7 @@ bwd_partial_kernel(long long P, int C, const float* __restrict__ x, int ldx, con
   const Tile t = tile_of(P, C);
   double s1 = 0.0, s2 = 0.0, s3 = 0.0;
   if (t.active) {
-    const float m = mean[t.c], is = bn_invstd(var[t.c], eps), wc = w[t.c], bc = b[t.c], a = alpha[t.c];
+    const float m = mean[t.c], is = bn_invstd(var[t.c], eps), wc = w[t.c], bc = b[t.c], a = slope_of(alpha, t.c);
     for (long long r = t.r0 + t.ty; r < t.r1; r += t.tr) {
       const float xv = x[r * ldx + t.c], g = dout[r * ldd + t.c];
       const float z = bn_z(xv, m, is, wc, bc);
@@ -182,7 +187,7 @@ __device__ __forceinline__ float bn_dx_at(const BnArgs& a, long long r, int c) {
   const float xv = a.x[r * a.ldx + c], g = a.dout[r * a.ldd + c];
   const float m = a.mean[c], is = bn_invstd(a.var[c], a.eps), wc = a.w[c];
   const float z = bn_z(xv, m, is, wc, a.b[c]);
-  const float dz = z > 0.f ? g : a.alpha[c] * g;
+  const float dz = z > 0.f ? g : slope_of(a.alpha, c) * g;
   if (!a.training) return dz * (wc * is);
   const float xhat = (xv - m) * is;
   return (dz - a.coef[c] - xhat * a.coef[a.C + c]) * (wc * is);
@@ -265,6 +270,44 @@ resample_kernel(int N, int C, int h, int w, const float* __restrict__ src, long 
     const int x = (int)(r % W); r /= W;
     const int y = (int)(r % H); const int n = (int)(r / H);
     out[i] = up_at(src + n * sn + c * sc, sp, h, w, ry, rx, y, x);
+  }
+}
+
+// Adjoint of resample_kernel (d src from d out), as a gather: one thread per source element (n, y, x, c) sums, in ascending (oy, ox)
+// order, wy * wx * dout over the output pixels whose four taps include (y, x).  The weights are resample_kernel's, recomputed with
+// its arithmetic (up_at); a clamped tap (y0 == y1 at the last row / column) receives both of its weights.  No atomics: the result
+// does not depend on scheduling.  dout is dense NHWC [N][H][W][C]; dsrc is NHWC with pixel pitch lds.
+__device__ __forceinline__ float adj_weight(int o, float r, int n, int i) {
+  const float f = o * r;
+  const int i0 = min((int)f, n - 1), i1 = min(i0 + 1, n - 1);
+  const float l = f - i0;
+  return (i0 == i ? 1.f - l : 0.f) + (i1 == i ? l : 0.f);
+}
+
+__global__ void __launch_bounds__(kThreads)
+resample_adjoint_kernel(int N, int C, int h, int w, const float* __restrict__ dout, int H, int W, float* __restrict__ dsrc, int lds) {
+  const long long total = (long long)N * h * w * C;
+  const float ry = H > 1 ? (float)(h - 1) / (float)(H - 1) : 0.f, rx = W > 1 ? (float)(w - 1) / (float)(W - 1) : 0.f;
+  for (long long i = (long long)blockIdx.x * kThreads + threadIdx.x; i < total; i += (long long)gridDim.x * kThreads) {
+    const int c = (int)(i % C); long long r = i / C;
+    const int x = (int)(r % w); r /= w;
+    const int y = (int)(r % h); const int n = (int)(r / h);
+    // output rows / columns that can reach y / x: o * ry in (y - 1, y + 1], widened by one for the float rounding of o * ry
+    const int oy0 = ry > 0.f ? max(0, (int)floorf((y - 1) / ry) - 1) : 0, oy1 = ry > 0.f ? min(H - 1, (int)ceilf((y + 1) / ry) + 1) : H - 1;
+    const int ox0 = rx > 0.f ? max(0, (int)floorf((x - 1) / rx) - 1) : 0, ox1 = rx > 0.f ? min(W - 1, (int)ceilf((x + 1) / rx) + 1) : W - 1;
+    float acc = 0.f;
+    for (int oy = oy0; oy <= oy1; ++oy) {
+      const float wy = adj_weight(oy, ry, h, y);
+      if (wy == 0.f) continue;
+      const float* row = dout + (((long long)n * H + oy) * W) * C + c;
+      float s = 0.f;
+      for (int ox = ox0; ox <= ox1; ++ox) {
+        const float wx = adj_weight(ox, rx, w, x);
+        if (wx != 0.f) s = __fadd_rn(s, __fmul_rn(wx, row[(long long)ox * C]));
+      }
+      acc = __fadd_rn(acc, __fmul_rn(wy, s));
+    }
+    dsrc[(((long long)n * h + y) * w + x) * lds + c] = acc;
   }
 }
 
@@ -363,6 +406,15 @@ extern "C" int skd_resample_bilinear_nhwc(int N, int C, int h, int w, const floa
   if (N <= 0 || C <= 0 || h <= 0 || w <= 0 || H <= 0 || W <= 0) { set_error_msg("skd_resample_bilinear_nhwc", "bad shape"); return 0; }
   resample_kernel<<<ew_grid((long long)N * H * W * C), kThreads, 0, st>>>(N, C, h, w, src, sn, sc, sp, H, W, out);
   return finish("skd_resample_bilinear_nhwc");
+}
+
+extern "C" int skd_resample_bilinear_adjoint_nhwc(int N, int C, int h, int w, const float* dout, int H, int W, float* dsrc, int lds,
+                                                  cudaStream_t st) {
+  if (N <= 0 || C <= 0 || h <= 0 || w <= 0 || H <= 0 || W <= 0 || lds < C) {
+    set_error_msg("skd_resample_bilinear_adjoint_nhwc", "bad shape"); return 0;
+  }
+  resample_adjoint_kernel<<<ew_grid((long long)N * h * w * C), kThreads, 0, st>>>(N, C, h, w, dout, H, W, dsrc, lds);
+  return finish("skd_resample_bilinear_adjoint_nhwc");
 }
 
 extern "C" int skd_avgpool3x3s2(int N, int H, int W, int C, const float* src, int lds, float* dst, int ldd, cudaStream_t st) {

@@ -297,6 +297,17 @@ slice_copy_kernel(const float* __restrict__ src, int spitch4, int soff4, float* 
   }
 }
 
+// the same copy one float at a time, for channel counts / offsets that are not whole float4s (the full ESPNet's 19-class slices)
+__global__ void __launch_bounds__(256)
+slice_copy_scalar_kernel(const float* __restrict__ src, int spitch, int soff, float* __restrict__ dst, int dpitch, int doff, long long rows,
+                         int C) {
+  const long long total = rows * C;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const long long r = i / C; const int c = (int)(i - r * C);
+    dst[r * dpitch + doff + c] = src[r * spitch + soff + c];
+  }
+}
+
 // v = mu*v + (g + wd*p) ; p -= lr*v   (torch.optim.SGD, dampening 0, first step v = g + wd*p)
 __global__ void __launch_bounds__(256)
 sgd_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ v, long long n4, long long n,
@@ -454,7 +465,11 @@ extern "C" int skd_psp_upsample_bwd(int N, int H, int W, int C, int s, const flo
 
 extern "C" int skd_slice_copy(long long rows, int C, const float* src, int src_pitch, int src_off, float* dst, int dst_pitch,
                               int dst_off, cudaStream_t st) {
-  if ((C | src_pitch | src_off | dst_pitch | dst_off) % 4) { set_error_msg("skd_slice_copy", "multiples of 4 channels only"); return 0; }
+  if (C <= 0 || src_pitch < src_off + C || dst_pitch < dst_off + C) { set_error_msg("skd_slice_copy", "bad shape"); return 0; }
+  if ((C | src_pitch | src_off | dst_pitch | dst_off) % 4 || ((reinterpret_cast<uintptr_t>(src) | reinterpret_cast<uintptr_t>(dst)) & 15)) {
+    slice_copy_scalar_kernel<<<ew_blocks(rows * C), 256, 0, st>>>(src, src_pitch, src_off, dst, dst_pitch, dst_off, rows, C);
+    return finish("skd_slice_copy");
+  }
   slice_copy_kernel<<<ew_blocks(rows * (C / 4)), 256, 0, st>>>(src, src_pitch / 4, src_off / 4, dst, dst_pitch / 4, dst_off / 4,
                                                               rows, C / 4);
   return finish("skd_slice_copy");

@@ -479,7 +479,7 @@ class EspBlock(torch.autograd.Function):
         else:
             ops.esp_combine(branches, x if add else None, comb, stats=False)
             st = torch.stack([running_mean, running_var])
-        y = ops.bnprelu_apply(comb, st[0], st[1], bn_w, bn_b, alpha, eps)
+        y = ops.bnprelu_apply(comb, st[0], st[1], bn_w, bn_b, alpha, eps, out_channels=ops.pad4(c))
         ctx.save_for_backward(x, t, comb, st, wc1, *wbr, w_c1, w_d1, w_d2, w_d4, w_d8, w_d16, bn_w, bn_b, alpha)
         ctx.cfg = (stride, add, training, eps, n1, n_red)
         return y
@@ -509,6 +509,87 @@ class EspBlock(torch.autograd.Function):
         dws = [_esp_wgrad(t, dd, wd, 1, d, d) for dd, wd, d in zip(dds, (w_d1, w_d2, w_d4, w_d8, w_d16), (1, 2, 4, 8, 16))]
         dwc1 = _esp_wgrad(x, dt, w_c1, stride, (k - 1) // 2, 1)
         return (dx, dwc1, *dws, dbw, dbb, da) + (None,) * 9
+
+
+class EspConvTranspose(torch.autograd.Function):
+    """nn.ConvTranspose2d(Cin, Cout, 2, stride=2, bias=False) between channel-padded NHWC tensors (the full ESPNet's up_l3, up_l2 and
+    classifier): (N, pad4(Cout), 2h, 2w) out, zero pad channels.  `weight` is the (Cin, Cout, 2, 2) parameter.
+      forward: per output-row parity a, one 1x1 GEMM to 2 * pad4(Cout) channels (the two output columns), 3xTF32, written onto the
+               every-other-row sub-grid (ops.conv_transpose2x2_fwd);
+      dgrad:   dx = conv2d(dy, w[ci][a][b][co], 2x2, stride 2) -- a forward wgmma convolution;
+      wgrad:   the weight gradient of that same convolution, with dy as its input and x as its output gradient."""
+
+    @staticmethod
+    def forward(ctx, x, weight):
+        cin, cout = weight.shape[:2]
+        cin_p, cout_p = x.shape[1], ops.pad4(cout)
+        wr = torch.zeros((2, 2, cout_p, cin_p), device=weight.device, dtype=torch.float32)
+        wr[:, :, :cout, :cin] = weight.permute(2, 3, 1, 0)               # [a][b][co][ci]
+        y = ops.conv_transpose2x2_fwd(x, wr.reshape(2, 2 * cout_p, 1, 1, cin_p))
+        ctx.save_for_backward(x, weight)
+        return y
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, dy):
+        x, weight = ctx.saved_tensors
+        cin, cout = weight.shape[:2]
+        cin_p = x.shape[1]
+        dy = ops.to_nhwc(dy)
+        dx = dw = None
+        if ctx.needs_input_grad[0]:
+            wd = torch.zeros((cin_p, 2, 2, dy.shape[1]), device=weight.device, dtype=torch.float32)
+            wd[:cin, :, :, :cout] = weight.permute(0, 2, 3, 1)            # [ci][a][b][co]: OHWI of the 2x2 / stride-2 convolution of dy
+            dx = ops.conv2d_fwd(dy, wd, 2, 0, 1)
+        if ctx.needs_input_grad[1]:
+            dw = ops.conv2d_wgrad(dy, x, (2, 2), 2, 0, 1)[:cin, :, :, :cout].permute(0, 3, 1, 2)
+        return dx, dw
+
+
+class EspConcat(torch.autograd.Function):
+    """torch.cat(pieces, 1) into one channel-padded NHWC buffer (zero pad channels) for the convolution that reads it."""
+
+    @staticmethod
+    def forward(ctx, *pieces):
+        n, _, h, w = pieces[0].shape
+        widths = [p.shape[1] for p in pieces]
+        c = sum(widths)
+        x = torch.zeros((n, h, w, ops.pad4(c)), device=pieces[0].device, dtype=torch.float32).permute(0, 3, 1, 2)
+        off = 0
+        for p, k in zip(pieces, widths):
+            ops.slice_copy(p, 0, x, off, k)
+            off += k
+        ctx.widths = widths
+        return x
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, dx):
+        dx = ops.to_nhwc(dx)
+        n, _, h, w = dx.shape
+        out, off = [], 0
+        for k in ctx.widths:
+            d = ops.empty_nhwc(n, k, h, w, dx.device)
+            ops.slice_copy(dx, off, d, 0, k)
+            out.append(d)
+            off += k
+        return tuple(out)
+
+
+class ResampleBilinear(torch.autograd.Function):
+    """F.interpolate(t, (H, W), mode='bilinear', align_corners=True) with a gradient: the forward is the teacher resample kernel, the
+    backward its adjoint as a fixed-order gather (no float atomics, so two runs of a step stay bit-identical).  The full ESPNet's
+    logits reach the discriminator this way, resized onto the teacher's logit grid."""
+
+    @staticmethod
+    def forward(ctx, t, H, W):
+        ctx.hw = tuple(t.shape[2:])
+        return ops.resample_nhwc(t, H, W)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        return ops.resample_adjoint_nhwc(g, *ctx.hw), None, None
 
 
 class MaxPool3x3s2(torch.autograd.Function):

@@ -1,5 +1,6 @@
 """ESPNet-C (Mehta et al., "ESPNet: Efficient Spatial Pyramid of Dilated Convolutions for Semantic Segmentation", ECCV 2018), the
-encoder-only ESPNet, as a distillation student -- computed by the sm_90a kernels of libskd_b200.
+encoder-only ESPNet, and the full ESPNet (ESPNet-C plus its decoder, logits at the input resolution) as distillation students --
+computed by the sm_90a kernels of libskd_b200.
 
 The modules are parameter containers (attribute names = state-dict keys: `level1.conv.weight`, `level2_0.d16.conv.weight`,
 `level2.0.bn.bn.running_var`, `b2.act.weight`, `classifier.conv.weight`, ...); the computation is the autograd Functions
@@ -136,6 +137,12 @@ class ESPNet_Encoder(nn.Module):
                                    bn.num_batches_tracked, self.training, bn.momentum, bn.eps, *pieces)
 
     def forward(self, x):
+        logits, feat, out2, b2, out1, b1 = self._features(x)
+        c = self.classes
+        return [logits[:, :c], None, feat, out2, b2[:, :131], out1, b1[:, :19]]
+
+    def _features(self, x):
+        """-> the channel-padded (logits, feat, out2, b2, out1, b1) (b2: 132 channels, b1: 20; pad channels zero)."""
         # the (N,3,H,W) image, or the 4-channel NHWC image NetModel.forward builds for the teacher
         x = ops.pad_channels(x, 4) if x.shape[1] == 3 else ops.to_nhwc(x)
         precise = self.precise
@@ -153,9 +160,60 @@ class ESPNet_Encoder(nn.Module):
             out2 = layer(out2, precise)
         feat, _ = self._br(self.b3, [out2_0, out2])
         logits = Fn.EspConv.apply(feat, self.classifier.conv.weight, 1, 0, 1, precise)
-        c = self.classes
-        return [logits[:, :c], None, feat, out2, b2[:, :131], out1, b1[:, :19]]
+        return logits, feat, out2, b2, out1, b1
 
 
 def ESPNet_C(classes=19, p=2, q=8):
     return ESPNet_Encoder(classes, p, q)
+
+
+class ESPNet(nn.Module):
+    """The full ESPNet: ESPNet-C (`encoder.`) plus its decoder, logits at the input resolution.  H and W must be multiples of 8.
+
+        x3 = up_l3(br(enc_logits))                                   1/8 -> 1/4; `br` is BatchNorm2d without PReLU
+        y  = combine_l2_l3(cat([level3_C(b2), x3]))                  1/4: BR(2 classes) -> ESP block (2 classes -> classes, no residual)
+        y  = conv(cat([up_l2(y), b1]))                               1/2: up_l2 = transposed conv + BR; conv = CBR 3x3
+        logits = classifier(y)                                       1/2 -> 1/1
+
+    The up_l3, up_l2 and classifier layers are 2x2 / stride-2 transposed convolutions without bias (`EspConvTranspose`).  forward
+    returns `[logits, None, feat, out2, b2, out1, b1]` like ESPNet-C: feat (1/8) at index -5 for the pair-wise loss."""
+
+    def __init__(self, classes=19, p=2, q=8):
+        super().__init__()
+        self.encoder = ESPNet_Encoder(classes, p, q)
+        self.level3_C = C(128 + 3, classes, 1, 1)
+        self.br = nn.BatchNorm2d(classes, eps=1e-3)
+        self.conv = CBR(19 + classes, classes, 3, 1)
+        self.up_l3 = nn.Sequential(nn.ConvTranspose2d(classes, classes, 2, stride=2, padding=0, output_padding=0, bias=False))
+        self.combine_l2_l3 = nn.Sequential(BR(2 * classes), DilatedParllelResidualBlockB(2 * classes, classes, add=False))
+        self.up_l2 = nn.Sequential(nn.ConvTranspose2d(classes, classes, 2, stride=2, padding=0, output_padding=0, bias=False),
+                                   BR(classes))
+        self.classifier = nn.ConvTranspose2d(classes, classes, 2, stride=2, padding=0, output_padding=0, bias=False)
+        self.classes = classes
+
+    def dropouts(self):
+        return []
+
+    def _bn(self, bn, alpha, pieces):
+        return Fn.EspBnPrelu.apply(None, 0, bn.weight, bn.bias, alpha, bn.running_mean, bn.running_var, bn.num_batches_tracked,
+                                   self.training, bn.momentum, bn.eps, *pieces)[0]
+
+    def forward(self, x):
+        H, W = x.shape[2], x.shape[3]
+        if H % 8 or W % 8:
+            raise ValueError("ESPNet needs H and W divisible by 8 (got %dx%d)" % (H, W))
+        enc = self.encoder
+        logits8, feat, out2, b2, out1, b1 = enc._features(x)
+        c, precise = self.classes, enc.precise
+        x3 = Fn.EspConvTranspose.apply(self._bn(self.br, None, [logits8[:, :c]]), self.up_l3[0].weight)              # 1/4
+        l3 = Fn.EspConv.apply(b2, self.level3_C.conv.weight, 1, 0, 1, precise)
+        br0 = self.combine_l2_l3[0]
+        y = self._bn(br0.bn, br0.act.weight, [l3[:, :c], x3[:, :c]])
+        y = self.combine_l2_l3[1](y, precise)                                                                       # 1/4
+        u = Fn.EspConvTranspose.apply(y, self.up_l2[0].weight)                                                      # 1/2
+        u = self._bn(self.up_l2[1].bn, self.up_l2[1].act.weight, [u[:, :c]])
+        cat = Fn.EspConcat.apply(u[:, :c], b1[:, :19])
+        y = Fn.EspConv.apply(cat, self.conv.conv.weight, 1, 1, 1, precise)
+        y = self._bn(self.conv.bn, self.conv.act.weight, [y[:, :c]])
+        logits = Fn.EspConvTranspose.apply(y, self.classifier.weight)                                               # 1/1
+        return [logits[:, :c], None, feat, out2, b2[:, :131], out1, b1[:, :19]]

@@ -27,7 +27,7 @@ from ..optim import FlatSGD
 from ..utils.criterion import (CriterionAdditionalGP, CriterionAdv, CriterionAdvForG, CriterionCrossEntropy, CriterionDSN,
                                CriterionOhemDSN, CriterionPairWiseforWholeFeatAfterPool, CriterionPixelWise)
 from ..utils.utils import load_D_model, load_S_model, load_T_model
-from .espnet import ESPNet_C
+from .espnet import ESPNet, ESPNet_C
 from .evaluate import evaluate_main
 from .pspnet_combine import BasicBlock, Bottleneck, Res_pspnet
 from .sagan_models import Discriminator
@@ -71,12 +71,13 @@ class NetModel():
         self.student_kind = str(_arg(args, "student", "resnet18"))
         if self.student_kind == "resnet18":
             student = Res_pspnet(BasicBlock, [2, 2, 2, 2], num_classes=args.classes_num)
-        elif self.student_kind == "espnet_c":
+        elif self.student_kind in ("espnet_c", "espnet"):
             if _arg(args, "sync_bn", False):
-                raise ValueError("sync_bn is not available with the ESPNet-C student (its BatchNorm statistics are per rank)")
-            student = ESPNet_C(args.classes_num, _arg(args, "espnet_p", 2), _arg(args, "espnet_q", 8))
+                raise ValueError("sync_bn is not available with the ESPNet students (their BatchNorm statistics are per rank)")
+            student = (ESPNet_C if self.student_kind == "espnet_c" else ESPNet)(args.classes_num, _arg(args, "espnet_p", 2),
+                                                                               _arg(args, "espnet_q", 8))
         else:
-            raise ValueError("student must be 'resnet18' or 'espnet_c' (got %r)" % self.student_kind)
+            raise ValueError("student must be 'resnet18', 'espnet_c' or 'espnet' (got %r)" % self.student_kind)
         load_S_model(args, student, False)                         # ImageNet init or S_resume (utils/utils.py:93-127)
         self.student = student.float().to(device).train()
         if _arg(args, "sync_bn", False):                          # cross-rank batch statistics (the reference's InPlaceABNSync semantics)
@@ -122,7 +123,7 @@ class NetModel():
         if _arg(args, "ohem", False):                             # OHEM task loss (the reference imports CriterionOhemDSN, kd_model.py:18)
             # (ESPNet-C: head 0 only, preds[1] is None)
             self.criterion = CriterionOhemDSN(thresh=_arg(args, "ohem_thres", 0.7), min_kept=_arg(args, "ohem_keep", 100000))
-        elif self.student_kind == "espnet_c":                     # no auxiliary head: single-head cross entropy
+        elif self.student_kind != "resnet18":                     # the ESPNets: no auxiliary head, single-head cross entropy
             self.criterion = CriterionCrossEntropy()
         else:
             self.criterion = CriterionDSN()
@@ -216,16 +217,28 @@ class NetModel():
         self._resample_teacher()
 
     def _resample_teacher(self):
-        """Students on another grid than the teacher (ESPNet-C: 45x60 at 360x480, PSPNet's ceil-mode pool: 46x61): the two teacher
-        tensors the distillation terms read, preds_T[0] and preds_T[-5], are resized onto the student's grid (bilinear,
-        align_corners=True; forward only, the teacher is frozen).  Equal grids (the ResNet18 student): nothing runs."""
-        size = tuple(self.preds_S[0].shape[2:])
-        if tuple(self.preds_T[0].shape[2:]) == size:
-            return
+        """Students on another grid than the teacher (ESPNet-C: 45x60 at 360x480, PSPNet's ceil-mode pool: 46x61; the full ESPNet's
+        logits: 360x480): the two teacher tensors the distillation terms read, preds_T[0] and preds_T[-5], are each resized onto the
+        grid of their own student counterpart, preds_S[0] and preds_S[-5] (bilinear, align_corners=True; forward only, the teacher is
+        frozen).  Equal grids (the ResNet18 student): nothing runs.  The teacher's own logits stay in `logits_T` for the
+        discriminator of a full-resolution student."""
+        self.logits_T = self.preds_T[0]
         preds = list(self.preds_T)
         for i in (0, len(preds) - 5):
-            preds[i] = ops.resample_nhwc(preds[i], *size)
+            size = tuple(self.preds_S[i].shape[2:])
+            if tuple(preds[i].shape[2:]) != size:
+                preds[i] = ops.resample_nhwc(preds[i], *size)
         self.preds_T = preds
+
+    def _d_inputs(self):
+        """-> (student, teacher) logits the discriminator sees.  A student whose logits are at the input resolution (the full ESPNet)
+        meets D on the teacher's logit grid: its logits resized onto that grid (bilinear, align_corners=True, with the gradient of
+        Fn.ResampleBilinear) against the teacher's logits as they came out.  Others: preds_S[0] against preds_T[0]."""
+        s = self.preds_S[0]
+        if tuple(s.shape[2:]) != tuple(self.images.shape[2:]):
+            return s, self.preds_T[0]
+        t = self.logits_T
+        return Fn.ResampleBilinear.apply(s, t.shape[2], t.shape[3]), t
 
     def student_backward(self):
         args = self.args
@@ -241,7 +254,7 @@ class NetModel():
             self.pa_G_loss = _LazyScalar(temp1)
             G_loss = G_loss + args.lambda_pa * temp1
         if args.ho == True:
-            d_out_S = self.parallel_D(self.preds_S[0])
+            d_out_S = self.parallel_D(self._d_inputs()[0])
             G_loss = G_loss + args.lambda_d * self.criterion_adv_for_G(d_out_S, d_out_S)
         # the generator step only needs d D(S) / d logits: the reference's D gradients of this pass are discarded by
         # D_solver.zero_grad() (kd_model.py:154), so they are not computed
@@ -319,11 +332,13 @@ class NetModel():
         D.engine.prepare()                                   # weights are constant within the phase: stage them once
         D.accumulate_into_grad = True                        # the three passes add straight into FlatSGD's gradient buffer
         try:
-            d_out_T = self.parallel_D(self.preds_T[0].detach())
-            d_out_S = self.parallel_D(self.preds_S[0].detach())
+            with torch.no_grad():
+                d_in_S, d_in_T = self._d_inputs()
+            d_out_T = self.parallel_D(d_in_T.detach())
+            d_out_S = self.parallel_D(d_in_S.detach())
             d_loss = args.lambda_d * self.criterion_adv(d_out_S, d_out_T)
             if args.adv_loss_type == 'wgan-gp':
-                d_loss = d_loss + args.lambda_d * self.criterion_AdditionalGP(self.preds_S, self.preds_T)
+                d_loss = d_loss + args.lambda_d * self.criterion_AdditionalGP([d_in_S], [d_in_T])
             d_loss.backward()
         finally:
             D.accumulate_into_grad = False

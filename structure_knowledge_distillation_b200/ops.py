@@ -311,6 +311,32 @@ def conv2d_wgrad(x, dy, kshape, stride, pad, dil, force_direct=False, out=None):
     return dw
 
 
+def conv_transpose2x2_fwd(x, w_rows):
+    """nn.ConvTranspose2d(k=2, stride=2, no bias) forward, fp32-grade (3xTF32).  x: dense NHWC (N, Cin, h, w), Cin a multiple of 4;
+    w_rows: contiguous [2][2 * Coutp][1][1][Cin] -- for output-row parity a, the 1x1 weights of the two output columns 2j, 2j + 1
+    stacked (Coutp each).  Output pixels (2i + a, 2j) and (2i + a, 2j + 1) are 2 * Coutp consecutive floats, so each parity is one
+    1x1 GEMM to 2 * Coutp channels written onto the every-other-row sub-grid.  -> dense NHWC (N, Coutp, 2h, 2w)."""
+    n, cin, h, w, ldx = nhwc_meta(x)
+    if ldx != cin or cin % 4:
+        raise ValueError("Non-contiguous input")
+    cout2 = w_rows.shape[1]
+    coutp = cout2 // 2
+    y = empty_nhwc(n, coutp, 2 * h, 2 * w, x.device)
+    xl, wl = lo_tf32(x), lo_tf32(w_rows)
+    base = y.data_ptr()
+    log = CONV_EVENT_LOG
+    if log is not None:
+        ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        ev0.record()
+    for a in range(2):
+        lib().skd_conv2d_fwd_sm100_strided_3xtf32(n, h, w, cin, cout2, 1, 1, 1, 0, 1, _p(x), _p(xl), ldx, _p(w_rows[a]), _p(wl[a]),
+                                                  base + 4 * a * 2 * w * coutp, cout2, 4 * w * coutp, 4 * h * w * coutp, _st())
+    if log is not None:
+        ev1.record()
+        log.append((ev0, ev1, 2.0 * n * h * w * cin * 4 * coutp, ("convT_fwd", n, cin, h, w, coutp, 2, 2, 1)))
+    return y
+
+
 def im2col_small(x, kh, kw, stride, pad, dil, kp):
     """(N,Cin,H,W) NHWC-stored -> (N, kp, OH, OW) NHWC-stored im2col matrix (k = tap*Cin + ci, zero padded)."""
     n, cin, h, w, ldx = nhwc_meta(x)
@@ -634,7 +660,8 @@ def esp_combine(branches, residual, out, momentum=0.0, running_mean=None, runnin
 
 
 def bnprelu_apply(x, mean, var, weight, bias, alpha, eps, out=None, out_channels=None):
-    """prelu(bn(x)) -> `out` (default: a fresh NHWC tensor with `out_channels` >= C channels, the extra ones zero)."""
+    """prelu(bn(x)) -> `out` (default: a fresh NHWC tensor with `out_channels` >= C channels, the extra ones zero).  alpha=None: bn(x)
+    alone (here and in the two backward passes)."""
     _f32(x)
     n, c, h, w, ldx = nhwc_meta(x)
     cw = out_channels or c
@@ -653,8 +680,8 @@ def bnprelu_bwd_reduce(x, dout, mean, var, weight, bias, alpha, eps):
     red = torch.empty(5, c, device=x.device)             # dweight, dbias, dalpha, mean dz, mean dz*xhat
     ws = torch.empty(L.skd_bnprelu_workspace_doubles(P, c), device=x.device, dtype=torch.float64)
     L.skd_bnprelu_bwd_reduce(P, c, _p(x), ldx, _p(dout), ldd, _p(mean), _p(var), _p(weight), _p(bias), _p(alpha), eps, _p(red[0]),
-                             _p(red[1]), _p(red[2]), _p(red[3]), _p(ws), _st())
-    return red[0], red[1], red[2], red[3:5]
+                             _p(red[1]), _p(red[2]) if alpha is not None else None, _p(red[3]), _p(ws), _st())
+    return red[0], red[1], red[2] if alpha is not None else None, red[3:5]
 
 
 def bnprelu_bwd_dx(x, dout, mean, var, weight, bias, alpha, eps, training, coef, dx_channels=None):
@@ -678,6 +705,18 @@ def esp_bwd_dx(x, dout, mean, var, weight, bias, alpha, eps, training, coef, n1,
     lib().skd_esp_bwd_dx(N * h * w, n1, n, _p(x), ldx, _p(dout), ldd, _p(mean), _p(var), _p(weight), _p(bias), _p(alpha), eps,
                          int(training), _p(coef), _p(dd1), pad4(n1), *[_p(t) for t in dds], pad4(n), _p(dres), c, _st())
     return (dd1, *dds), dres
+
+
+def resample_adjoint_nhwc(dout, h, w, channels=None):
+    """Adjoint of resample_nhwc(t, H, W) for t of size (h, w): (N, C, H, W) gradient -> (N, C, h, w) NHWC gradient, padded to
+    `channels` >= C (pad channels zero).  Fixed-order gather, bit-identical across calls."""
+    _f32(dout)
+    dout = dout.contiguous(memory_format=torch.channels_last)
+    n, c, H, W = dout.shape
+    cw = channels or c
+    dsrc = (torch.zeros if cw != c else torch.empty)((n, h, w, cw), device=dout.device, dtype=torch.float32)
+    lib().skd_resample_bilinear_adjoint_nhwc(n, c, h, w, _p(dout), H, W, _p(dsrc), cw, _st())
+    return dsrc.permute(0, 3, 1, 2)
 
 
 def avgpool3x3s2(src, out):

@@ -61,9 +61,17 @@ def load_T_model(model, ckpt_path):
     return False
 
 
+def _encoder_only(model, state):
+    """True when `model` is the full ESPNet and `state` an ESPNet-C state dict (its keys without the `encoder.` prefix): training the
+    encoder first, then the whole network, is the usual way to train ESPNet."""
+    enc = getattr(model, "encoder", None)
+    return enc is not None and not any(k.startswith("encoder.") for k in state) and set(state) <= set(enc.state_dict())
+
+
 def load_S_model(args, model, with_module=True):
     """utils/utils.py:93-127: ImageNet initialisation (key intersection) when `is_student_load_imgnet`, else resume from
-    `<S_ckpt_path>/model_best.pth.tar` when `S_resume` -- restoring last_step / start_epoch / best_mean_IU into `args`."""
+    `<S_ckpt_path>/model_best.pth.tar` when `S_resume` -- restoring last_step / start_epoch / best_mean_IU into `args`.  The full
+    ESPNet student also takes an ESPNet-C state dict, loaded under `encoder.` (the decoder keeps its initialisation)."""
     ckpt_dir = getattr(args, "S_ckpt_path", "")
     if ckpt_dir and not os.path.exists(ckpt_dir):
         os.makedirs(ckpt_dir, exist_ok=True)
@@ -71,6 +79,8 @@ def load_S_model(args, model, with_module=True):
         path = str(getattr(args, "student_pretrain_model_imgnet", ""))
         if os.path.isfile(path):
             saved = _torch_load(path)
+            if _encoder_only(model, saved):
+                saved = {"encoder." + k: v for k, v in saved.items()}
             new = model.state_dict()
             new.update({k: v for k, v in saved.items() if k in new})
             model.load_state_dict(new)
@@ -85,7 +95,8 @@ def load_S_model(args, model, with_module=True):
             args.last_step = ck.get('step')
             args.start_epoch = ck.get('epoch')
             args.best_mean_IU = ck.get('best_mean_IU')
-            model.load_state_dict(_strip_module(ck['state_dict'], with_module))
+            state = _strip_module(ck['state_dict'], with_module)
+            (model.encoder if _encoder_only(model, state) else model).load_state_dict(state)
             logging.info("=> loaded checkpoint '{}' \n (epoch:{} step:{} best_mean_IU:{} \n )".format(file, args.start_epoch, args.last_step,
                                                                                               args.best_mean_IU))
             return "resume"

@@ -1,5 +1,6 @@
-"""Cost of the ESPNet-C student: the config-4 distillation step (batch 16 at 360x480, Pi+Pa+Ho wgan-gp, CUDA graphs) with the
-ResNet18-PSP and the ESPNet-C students, alternated within one run, and CUDA-event times of the ESPNet-C kernels at that shape.
+"""Cost of the ESPNet students: the config-4 distillation step (batch 16 at 360x480, Pi+Pa+Ho wgan-gp, CUDA graphs) with the
+ResNet18-PSP, ESPNet-C and full ESPNet students, alternated within one run, and CUDA-event times of the ESPNet kernels at that shape
+(the full ESPNet's transposed convolutions and the adjoint of its logits' resize onto the teacher's grid included).
 
     python -m tools.espnet_step_bench --steps 20 --warmup 5 --rounds 2
 
@@ -95,6 +96,22 @@ def kernel_times(batch):
     ft = ops.empty_nhwc(batch, 512, 46, 61, dev); ft.normal_(generator=g)
     out["resample_teacher_logits"] = _time(lambda: ops.resample_nhwc(lt, 45, 60), 50)
     out["resample_teacher_feat"] = _time(lambda: ops.resample_nhwc(ft, 45, 60), 50)
+    # the full ESPNet: up_l3 (1/8 -> 1/4), up_l2 (1/4 -> 1/2) and classifier (1/2 -> 1/1) forward, data and weight gradients
+    from structure_knowledge_distillation_b200 import functions as Fn
+    wt = torch.randn(19, 19, 2, 2, device=dev, generator=g)
+    for name, (h, w) in (("up_l3", (45, 60)), ("up_l2", (90, 120)), ("classifier", (180, 240))):
+        xt = ops.empty_nhwc(batch, 20, h, w, dev); xt.normal_(generator=g)
+        dyt = ops.empty_nhwc(batch, 20, 2 * h, 2 * w, dev); dyt.normal_(generator=g)
+        wd = torch.zeros(20, 2, 2, 20, device=dev); wd[:19, :, :, :19] = wt.permute(0, 2, 3, 1)
+        wr = torch.zeros(2, 2, 20, 20, device=dev); wr[:, :, :19, :19] = wt.permute(2, 3, 1, 0)
+        wr = wr.reshape(2, 40, 1, 1, 20)
+        out["convT_fwd_" + name] = _time(lambda: ops.conv_transpose2x2_fwd(xt, wr), 50)
+        out["convT_dgrad_" + name] = _time(lambda: ops.conv2d_fwd(dyt, wd, 2, 0, 1), 50)
+        out["convT_wgrad_" + name] = _time(lambda: ops.conv2d_wgrad(dyt, xt, (2, 2), 2, 0, 1), 50)
+    ls = ops.empty_nhwc(batch, 19, 360, 480, dev, pitch=20); ls.normal_(generator=g)
+    out["resize_student_logits_to_teacher"] = _time(lambda: Fn.ResampleBilinear.apply(ls, 46, 61), 50)
+    dd = torch.randn(batch, 19, 46, 61, device=dev, generator=g)
+    out["resize_adjoint"] = _time(lambda: ops.resample_adjoint_nhwc(dd, 360, 480), 50)
     return {k: round(v, 4) for k, v in out.items()}
 
 
@@ -106,11 +123,12 @@ def main():
     ap.add_argument("--batch", type=int, default=16)
     a = ap.parse_args()
     torch.cuda.set_device(0)
-    res = dict(card=card(), batch=a.batch, shape="360x480", losses="Pi+Pa+Ho wgan-gp", cuda_graph=True, resnet18=[], espnet_c=[])
+    res = dict(card=card(), batch=a.batch, shape="360x480", losses="Pi+Pa+Ho wgan-gp", cuda_graph=True, resnet18=[], espnet_c=[],
+               espnet=[])
     for _ in range(a.rounds):
-        for student, key in (("resnet18", "resnet18"), ("espnet_c", "espnet_c")):
+        for student in ("resnet18", "espnet_c", "espnet"):
             ips, ms = step_rate(student, a.batch, a.steps, a.warmup)
-            res[key].append(dict(images_per_s=round(ips, 2), ms_per_step=round(ms, 2)))
+            res[student].append(dict(images_per_s=round(ips, 2), ms_per_step=round(ms, 2)))
     res["kernels_ms"] = kernel_times(a.batch)
     res["card_after"] = card()
     print(json.dumps(res))
