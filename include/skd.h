@@ -358,13 +358,20 @@ int skd_cityscapes_id_tables(unsigned char* to_train, unsigned char* to_label);
 typedef struct skd_cs_sample {
   const unsigned char* image; const unsigned char* label;
   int src_h, src_w;
-  double f_scale;               /* 0.7 + randint(0, 14) / 10.0; <= 0: no resize (scale=False) */
+  double f_scale;               /* 0.7 + randint(0, 14) / 10.0 (VOC: 0.5 + randint(0, 11) / 10.0); <= 0: no resize (scale=False) */
   int scaled_h, scaled_w;       /* cvRound(src * f_scale) (ignored without resize) */
   int h_off, w_off;             /* crop origin inside the padded, scaled image */
   int flip;                     /* -1: mirror, +1: keep */
 } skd_cs_sample;
 int skd_cs_augment_batch(int n, const skd_cs_sample* samples, int crop_h, int crop_w, const float* mean_bgr, int ignore_label,
                          float* images, void* labels, int labels_int64, cudaStream_t);
+/* The same kernel for any data set (`VOCDataSet.__getitem__`, dataset/datasets.py:45-81, and the above): label_table is a HOST
+   uint8[256] applied to every raw label (NULL: labels pass through, as VOC's class ids 0..20 and 255 do); mean_bgr is HOST, 3
+   doubles, and the image value is (float)((double)x - mean_bgr[c]), i.e. numpy's `float32 image -= mean` for a float32 mean (pass
+   it rounded to float32) and for a tuple of Python numbers (pass it as is).  skd_cs_augment_batch is this call with the Cityscapes
+   table (ids >= 34 pass through) and its float32 mean. */
+int skd_augment_batch(int n, const skd_cs_sample* samples, int crop_h, int crop_w, const double* mean_bgr,
+                      const unsigned char* label_table, int ignore_label, float* images, void* labels, int labels_int64, cudaStream_t);
 /* `CSDataTestSet.__getitem__` after cv2.imread (dataset/datasets.py:234-250): image (device, uint8 H x W x 3 BGR) -> out (device,
    float32 [3][out_h][out_w]), value (float)((double)x - mean_bgr[c]) -- the reference subtracts a tuple of Python floats, i.e. in
    double -- and zero padding on the bottom / right; out_h = max(H, crop_h), out_w = max(W, crop_w) (no crop).  mean_bgr: HOST, 3. */

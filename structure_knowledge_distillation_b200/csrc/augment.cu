@@ -1,8 +1,12 @@
-// Cityscapes training augmentation on the GPU: ONE kernel per batch does what `CSDataSet.__getitem__` does on the CPU after the two
-// cv2.imread calls (reference dataset/datasets.py:175-206): id -> trainId table, cv2.resize (uint8 INTER_LINEAR for the image,
-// INTER_NEAREST for the label) by the drawn scale factor, float32 mean subtraction, zero / ignore-label padding to the crop size,
-// crop, mirror, HWC -> CHW.  Only the crop's pixels are ever computed: the reference resizes the whole 1024 x 2048 image (up to
-// 2150 x 4301) and then throws away all but 512 x 1024 of it.
+// Training augmentation on the GPU: ONE kernel per batch does what `CSDataSet.__getitem__` / `VOCDataSet.__getitem__` do on the CPU
+// after the two cv2.imread calls (reference dataset/datasets.py:45-81, 175-206): label table (Cityscapes id -> trainId; VOC: none),
+// cv2.resize (uint8 INTER_LINEAR for the image, INTER_NEAREST for the label) by the drawn scale factor, mean subtraction, zero /
+// ignore-label padding to the crop size, crop, mirror, HWC -> CHW.  Only the crop's pixels are ever computed: the reference resizes
+// the whole 1024 x 2048 image (up to 2150 x 4301) and then throws away all but 512 x 1024 of it.
+//
+// Mean subtraction is (float)((double)p - mean[c]) with the mean in double.  numpy's `float32 image -= mean` subtracts in float32 for
+// a float32 mean (then p - m is exact in double, since p is an integer in 0..255, and the one rounding is float32's: bit-identical)
+// and in double for a tuple of Python numbers (VOCDataSet's default (128, 128, 128)); the caller passes the mean with numpy's type.
 //
 // Bit-exact with OpenCV's fixed-point path (modules/imgproc/src/resize.cpp, opencv-python 4.13.0 in this image; restated in
 // oracle/dataset_port.py and pinned there against cv2 and against the unmodified reference loader):
@@ -27,10 +31,7 @@ struct DevSample {
   double inv;                                     // 1 / f_scale
   int src_h, src_w, scaled_h, scaled_w, h_off, w_off, flip, scale_on;
 };
-struct DevBatch { DevSample s[kMaxSamples]; float mean[3]; int ignore_label; };
-
-// datasets.py:143-149 (ids 0..33; everything else passes through)
-__constant__ unsigned char kTrainId[kCityscapesIds] = SKD_CITYSCAPES_TRAINID;
+struct DevBatch { DevSample s[kMaxSamples]; double mean[3]; int ignore_label; unsigned char table[256]; };
 
 __device__ __forceinline__ void linear_coef(int d, double inv, int size, bool reset_at_border, int& s, int& c0, int& c1) {
   float f = __double2float_rn(__dadd_rn(__dmul_rn(__dadd_rn((double)d, 0.5), inv), -0.5));
@@ -81,19 +82,20 @@ cs_augment_kernel(const __grid_constant__ DevBatch b, int crop_h, int crop_w, fl
       p0 = r[0]; p1 = r[1]; p2 = r[2];
       l = sp.label[(size_t)py * sp.src_w + px];
     }
-    v0 = __fsub_rn((float)p0, b.mean[0]); v1 = __fsub_rn((float)p1, b.mean[1]); v2 = __fsub_rn((float)p2, b.mean[2]);
-    lab = l < 34 ? (int)kTrainId[l] : l;
+    v0 = __double2float_rn(__dsub_rn((double)p0, b.mean[0]));
+    v1 = __double2float_rn(__dsub_rn((double)p1, b.mean[1]));
+    v2 = __double2float_rn(__dsub_rn((double)p2, b.mean[2]));
+    lab = b.table[l];
   }
   const size_t plane = (size_t)crop_h * crop_w, o = (size_t)y * crop_w + x;
   float* img = images + (size_t)n * 3 * plane + o;
   img[0] = v0; img[plane] = v1; img[2 * plane] = v2;
   labels[(size_t)n * plane + o] = (LabelT)lab;
 }
-}  // namespace
 
-extern "C" int skd_cs_augment_batch(int n, const skd_cs_sample* samples, int crop_h, int crop_w, const float* mean_bgr, int ignore_label,
-                                    float* images, void* labels, int labels_int64, cudaStream_t st) {
-  const char* who = "skd_cs_augment_batch";
+// `who`: the C entry point whose name errors are reported under
+int augment_batch(const char* who, int n, const skd_cs_sample* samples, int crop_h, int crop_w, const double* mean_bgr,
+                  const unsigned char* label_table, int ignore_label, float* images, void* labels, int labels_int64, cudaStream_t st) {
   if (n <= 0) return 1;
   if (!samples || !mean_bgr || !images || !labels || crop_h <= 0 || crop_w <= 0) { set_error_msg(who, "bad arguments"); return 0; }
   const size_t plane = (size_t)crop_h * crop_w;
@@ -114,6 +116,7 @@ extern "C" int skd_cs_augment_batch(int n, const skd_cs_sample* samples, int cro
     }
     for (int c = 0; c < 3; ++c) b.mean[c] = mean_bgr[c];
     b.ignore_label = ignore_label;
+    for (int i = 0; i < 256; ++i) b.table[i] = label_table ? label_table[i] : (unsigned char)i;
     const dim3 grid((crop_w + 255) / 256, crop_h, cnt);
     float* img = images + (size_t)base * 3 * plane;
     if (labels_int64) cs_augment_kernel<long long><<<grid, 256, 0, st>>>(b, crop_h, crop_w, img, reinterpret_cast<long long*>(labels) + (size_t)base * plane);
@@ -121,4 +124,23 @@ extern "C" int skd_cs_augment_batch(int n, const skd_cs_sample* samples, int cro
     ++kernels;
   }
   return finish(who, kernels);
+}
+}  // namespace
+
+extern "C" int skd_augment_batch(int n, const skd_cs_sample* samples, int crop_h, int crop_w, const double* mean_bgr,
+                                 const unsigned char* label_table, int ignore_label, float* images, void* labels, int labels_int64,
+                                 cudaStream_t st) {
+  return augment_batch("skd_augment_batch", n, samples, crop_h, crop_w, mean_bgr, label_table, ignore_label, images, labels,
+                       labels_int64, st);
+}
+
+// datasets.py:146-151: Cityscapes label ids -> train ids (ids >= 34 pass through), the mean as given in float32
+extern "C" int skd_cs_augment_batch(int n, const skd_cs_sample* samples, int crop_h, int crop_w, const float* mean_bgr, int ignore_label,
+                                    float* images, void* labels, int labels_int64, cudaStream_t st) {
+  if (n <= 0) return 1;
+  if (!mean_bgr) { set_error_msg("skd_cs_augment_batch", "bad arguments"); return 0; }
+  unsigned char to_train[256], to_label[256];
+  skd_cityscapes_id_tables(to_train, to_label);
+  const double mean[3] = {mean_bgr[0], mean_bgr[1], mean_bgr[2]};
+  return augment_batch("skd_cs_augment_batch", n, samples, crop_h, crop_w, mean, to_train, ignore_label, images, labels, labels_int64, st);
 }

@@ -62,6 +62,8 @@ class NetModel():
 
     def __init__(self, args):
         self.args = args
+        if not 1 <= int(args.classes_num) <= 32:              # the loss, OHEM and discriminator kernels hold up to 32 classes
+            raise ValueError("classes_num must be in 1..32 (got %r)" % (args.classes_num,))
         device = torch.device(_arg(args, "device", "cuda"))
         if device.type != "cuda":
             raise RuntimeError("NetModel runs on CUDA (sm_90a) only; there is no CPU path")
