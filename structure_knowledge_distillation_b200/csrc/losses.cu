@@ -315,6 +315,8 @@ dsn_ce_bwd_rows_kernel(const float* __restrict__ L0, const float* __restrict__ L
 }
 
 // Backward, phase 2: dL[n][c][y][x] = g*wh/count * sum_Y wy(y;Y) T1[n][Y][x][c]
+// count 0 (every label ignored): the loss is 0/0 = NaN, as torch's cross entropy over no target, and the gradient is 0, as torch's
+// (g/0 = inf would make it 0 * inf = NaN and carry NaN into every parameter through the SGD step)
 __global__ void __launch_bounds__(256)
 dsn_ce_bwd_cols_kernel(const float* __restrict__ T1, float* __restrict__ d0, float* __restrict__ d1, Strides a0, Strides a1,
                        int N, int C, int h, int w, int H, const float* __restrict__ gout, const float* __restrict__ count,
@@ -322,7 +324,8 @@ dsn_ce_bwd_cols_kernel(const float* __restrict__ T1, float* __restrict__ d0, flo
   const float sy = H > 1 ? (float)(h - 1) / (float)(H - 1) : 0.f;
   const long long per = (long long)N * h * C * w;
   const int heads = d1 ? 2 : 1;
-  const float gc = __ldg(gout) / __ldg(count);
+  const float cnt = __ldg(count);
+  const float gc = cnt > 0.f ? __ldg(gout) / cnt : 0.f;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < per * heads; i += (long long)gridDim.x * blockDim.x) {
     const int head = (int)(i / per); long long r = i - (long long)head * per;
     const int c = (int)(r % C); r /= C; const int x = (int)(r % w); r /= w; const int y = (int)(r % h); const int n = (int)(r / h);
