@@ -210,9 +210,13 @@ conv_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_co
 #pragma unroll
         for (int i = 0; i < R; ++i) acc[i] = tot[i];
       }
-      const float* v = acc;
+      float* v = acc;
 
       // ---- epilogue straight from the fragment ----
+      // the thread's two output rows (fragment rows r_lo and r_lo + 8); in[h] = false past the output
+      bool in[2];
+      float* yrow[2];
+      const float* rrow[2];
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const int row = r_lo + 8 * h;
@@ -220,28 +224,67 @@ conv_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_co
         const int ty = rem / a.tiles_x, tx = rem - ty * a.tiles_x;
         const int dy = row / a.BW, dx = row - dy * a.BW;
         const int oy = ty * a.BH + dy, ox = tx * a.BW + dx;
-        if (oy >= a.OH || ox >= a.OW) continue;
-        float* yrow = a.y + (size_t)sp * a.split_stride + (size_t)img * a.y_img + (size_t)oy * a.y_row + (size_t)ox * a.ldy;
-        const float* rrow = a.residual ? a.residual + (((size_t)img * a.OH + oy) * a.OW + ox) * a.ldr : nullptr;
+        in[h] = oy < a.OH && ox < a.OW;
+        yrow[h] = a.y + (size_t)sp * a.split_stride + (size_t)img * a.y_img + (size_t)oy * a.y_row + (size_t)ox * a.ldy;
+        rrow[h] = in[h] && a.residual ? a.residual + (((size_t)img * a.OH + oy) * a.OW + ox) * a.ldr : nullptr;
+      }
+      // Pass 1: scale, shift and residual, each read in full at the thread's columns and then applied in place, before anything is
+      // stored.  The output may alias what these read, so the compiler keeps every read after the stores that precede it: reads
+      // interleaved with the stores wait one global-memory latency per column pair (a 1x1 convolution with a residual then runs at
+      // a fraction of the DRAM rate), while a pass with no store in it has all its reads in flight at once.  __fmul_rn / __fadd_rn
+      // keep the product and each sum separately rounded (no contraction into an FMA), in the order scale, shift, residual.
+      // Columns past Cout read nothing; their values are never stored.
+      const int c0 = nt * BLOCK_N + cq;
+      float t[BLOCK_N / 4];                                      // one operand at the thread's columns c0 + 8j + {0, 1}
+      auto gather = [&](const float* p) {
+#pragma unroll
+        for (int j = 0; j < BLOCK_N / 8; ++j) {
+          const int c = c0 + 8 * j;
+          t[2 * j] = c < a.Cout ? __ldg(p + c) : 0.f;
+          t[2 * j + 1] = c + 1 < a.Cout ? __ldg(p + c + 1) : 0.f;
+        }
+      };
+      if (a.scale) {
+        gather(a.scale);
+#pragma unroll
+        for (int i = 0; i < R; ++i) v[i] = __fmul_rn(v[i], t[(i >> 2) * 2 + (i & 1)]);
+      }
+      if (a.shift) {
+        gather(a.shift);
+#pragma unroll
+        for (int i = 0; i < R; ++i) v[i] = __fadd_rn(v[i], t[(i >> 2) * 2 + (i & 1)]);
+      }
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        if (!rrow[h]) continue;
+        gather(rrow[h]);
+#pragma unroll
+        for (int j = 0; j < BLOCK_N / 8; ++j) {
+          v[4 * j + 2 * h] = __fadd_rn(v[4 * j + 2 * h], t[2 * j]);
+          v[4 * j + 2 * h + 1] = __fadd_rn(v[4 * j + 2 * h + 1], t[2 * j + 1]);
+        }
+      }
+      // Pass 2: activation, rounding, sum of squares, stores
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        if (!in[h]) continue;
         float part = 0.f;
 #pragma unroll
         for (int j = 0; j < BLOCK_N / 8; ++j) {
-          const int c = nt * BLOCK_N + 8 * j + cq;
+          const int c = c0 + 8 * j;
           if (c >= a.Cout) continue;
           const bool two = c + 1 < a.Cout;
           float v0 = v[4 * j + 2 * h], v1 = v[4 * j + 2 * h + 1];
-          if (a.scale) { v0 *= __ldg(a.scale + c); if (two) v1 *= __ldg(a.scale + c + 1); }
-          if (a.shift) { v0 += __ldg(a.shift + c); if (two) v1 += __ldg(a.shift + c + 1); }
-          if (rrow) { v0 += __ldg(rrow + c); if (two) v1 += __ldg(rrow + c + 1); }
           v0 = epi_act(v0, a.act, a.slope); v1 = epi_act(v1, a.act, a.slope);
           if (a.round_out) { v0 = ptx::round_tf32(v0); v1 = ptx::round_tf32(v1); }
           if (a.sumsq) part = fmaf(v0, v0, two ? fmaf(v1, v1, part) : part);
           if (a.no_store) continue;
-          if (two && !((reinterpret_cast<uintptr_t>(yrow + c)) & 7)) {
-            *reinterpret_cast<float2*>(yrow + c) = make_float2(v0, v1);
+          float* y = yrow[h];
+          if (two && !((reinterpret_cast<uintptr_t>(y + c)) & 7)) {
+            *reinterpret_cast<float2*>(y + c) = make_float2(v0, v1);
           } else {
-            yrow[c] = v0;
-            if (two) yrow[c + 1] = v1;
+            y[c] = v0;
+            if (two) y[c + 1] = v1;
           }
         }
         sq_acc += (double)part;                                 // fp32 within a row of the tile, fp64 across rows and tiles
