@@ -17,6 +17,9 @@
 //                   (x3 for split precision), accumulator in registers, the stage released one stage later (one wgmma batch in
 //                   flight); epilogue straight from the registers: per-channel scale/shift (folded BN or bias), residual add,
 //                   ReLU / leaky-ReLU / ELU, optional TF32 rounding and fused sum of squares, global stores.
+//   TMA_EPI         (short-K flat / im2col launches with a residual) the residual comes in and the output goes out through a
+//                   shared-memory tile: thread 32 of warpgroup 0 loads the tile's residual by TMA while the K loop runs, and each
+//                   consumer warpgroup hands its finished 64 rows to one TMA store and starts the next tile's wgmmas without waiting.
 #include <cuda.h>
 
 #include "common.cuh"
@@ -32,6 +35,8 @@ constexpr int kBlockK = 32;                 // fp32 elements = 128 B = one swizz
 constexpr int kWgmmaK = 8;                  // tf32
 constexpr int kThreads = 384;               // producer warpgroup + 2 consumer warpgroups
 constexpr int kABytes = kBlockM * kBlockK * 4;
+constexpr int kTmaEpiMaxK = 16;             // longest K loop (taps x 32-channel chunks) that takes the TMA epilogue
+constexpr int kEpiBoxBytes = 64 * kBlockK * 4;   // TMA epilogue box: 64 rows x 32 channels
 
 struct ConvArgs {
   int N, OH, OW, Cout, Cin;
@@ -53,15 +58,21 @@ struct ConvArgs {
   long long split_stride;          //   raw fp32 partials go to y + split * split_stride; splitk_epilogue_kernel adds them and applies the epilogue
 };
 
-template <int BLOCK_N, bool SPLIT>
+template <int BLOCK_N, bool SPLIT, bool TMA_EPI>
 struct Cfg {
+  static_assert(!(SPLIT && TMA_EPI), "the TMA epilogue serves single-precision launches only");
   static constexpr int kBBytes = BLOCK_N * kBlockK * 4;
   static constexpr int kStageBytes = (kABytes + kBBytes) * (SPLIT ? 2 : 1);   // split precision: {x_hi, w_hi, x_lo, w_lo}
+  // TMA epilogue: ring of output tiles (128 rows x BLOCK_N fp32, 32-channel x 64-row boxes of 128B-swizzled rows), taken out of the
+  // 227 KB before the operand stages are counted
+  static constexpr int kEpiBufs = TMA_EPI ? 2 : 0;
+  static constexpr int kEpiBytes = kBlockM * BLOCK_N * 4;
   static constexpr int kFixedBytes = 1024 /*align slack*/ + 256 /*barriers*/;
-  static constexpr int kFit = (232448 - kFixedBytes) / kStageBytes;
+  static constexpr int kFit = (232448 - kFixedBytes - kEpiBufs * kEpiBytes) / kStageBytes;
   static constexpr int kStages = kFit > 8 ? 8 : kFit;
-  static constexpr int kSmemBytes = kStages * kStageBytes + kFixedBytes;
+  static constexpr int kSmemBytes = kStages * kStageBytes + kEpiBufs * kEpiBytes + kFixedBytes;
   static_assert(kStages >= 2, "at least two pipeline stages");
+  static_assert(2 * (kStages + kEpiBufs) * 8 <= 256, "barriers");
   static_assert(kSmemBytes <= 232448, "exceeds the 227 KB of shared memory a CTA may use");
 };
 
@@ -72,23 +83,37 @@ __device__ __forceinline__ float epi_act(float v, int act, float slope) {
   return v;
 }
 
-template <int BLOCK_N, bool SPLIT>
+// TMA epilogue (TMA_EPI): tile buffer eb of the ring holds the tile's residual (loaded by TMA; epi_full[eb] completes when it has
+// landed) and then its output (stored by TMA from the same positions; epi_empty[eb] gets one arrival per consumer warpgroup once
+// its store has read the buffer).  The output may be the residual itself (Bottleneck.frozen adds in place).  That stays safe:
+// a tile reads its residual only from the rows and channels it writes, its load has completed (epi_full) before its own store is
+// issued, and no two tiles of a launch write the same element.
+template <int BLOCK_N, bool SPLIT, bool TMA_EPI>
 __global__ void __launch_bounds__(kThreads, 1)
 conv_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_w,
-                     const __grid_constant__ CUtensorMap tmap_x2, const __grid_constant__ CUtensorMap tmap_w2, const ConvArgs a) {
-  using C = Cfg<BLOCK_N, SPLIT>;
+                     const __grid_constant__ CUtensorMap tmap_x2, const __grid_constant__ CUtensorMap tmap_w2,
+                     const __grid_constant__ CUtensorMap tmap_r, const __grid_constant__ CUtensorMap tmap_y, const ConvArgs a) {
+  using C = Cfg<BLOCK_N, SPLIT, TMA_EPI>;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   // keep the pointer in the shared address space (integer round trips make nvcc emit generic LD/ST instead of LDS/STS)
   const uint32_t raw_addr = ptx::smem_u32(smem_raw);
   uint8_t* smem = smem_raw + (((raw_addr + 1023u) & ~1023u) - raw_addr);
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + C::kStages * C::kStageBytes);
+  uint8_t* epi_smem = smem + C::kStages * C::kStageBytes;
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(epi_smem + C::kEpiBufs * C::kEpiBytes);
   uint64_t* empty_bar = full_bar + C::kStages;
+  uint64_t* epi_full = empty_bar + C::kStages;
+  uint64_t* epi_empty = epi_full + C::kEpiBufs;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (threadIdx.x == 0) {
     ptx::prefetch_tmap(&tmap_x);
     ptx::prefetch_tmap(&tmap_w);
     for (int s = 0; s < C::kStages; ++s) { ptx::mbar_init(&full_bar[s], 1); ptx::mbar_init(&empty_bar[s], 8); }   // one arrival per consumer warp
+    if constexpr (TMA_EPI) {
+      ptx::prefetch_tmap(&tmap_y);
+      ptx::prefetch_tmap(&tmap_r);
+      for (int b = 0; b < C::kEpiBufs; ++b) { ptx::mbar_init(&epi_full[b], 1); ptx::mbar_init(&epi_empty[b], 2); }   // one arrival per consumer warpgroup
+    }
     ptx::fence_barrier_init();
   }
   __syncthreads();
@@ -145,6 +170,31 @@ conv_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_co
         }
       }
     }
+    if constexpr (TMA_EPI) {
+      // residual loader, a thread of its own so that waiting for a free tile buffer never holds up the operand loads.  Boxes of 32
+      // channels x 64 rows, one 64-row half per consumer warpgroup; boxes wholly past P or Cout are not loaded (nobody stores them)
+      if (threadIdx.x == 32) {
+        const int P = a.OW;                                          // flat / im2col: one row of P pixels
+        int eb = 0; uint32_t ephase = 0;
+        for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+          const int tu = a.reverse ? total_tiles - 1 - tile : tile;
+          const int mt = tu / a.n_tiles, nt = tu - mt * a.n_tiles;
+          ptx::mbar_wait(&epi_empty[eb], ephase ^ 1);
+          uint32_t bytes = 0;
+          for (int h = 0; h < 2; ++h)
+            for (int j = 0; j < BLOCK_N / kBlockK; ++j)
+              if (mt * kBlockM + 64 * h < P && nt * BLOCK_N + kBlockK * j < a.Cout) bytes += kEpiBoxBytes;
+          ptx::mbar_expect_tx(&epi_full[eb], bytes);
+          uint8_t* buf = epi_smem + eb * C::kEpiBytes;
+          for (int h = 0; h < 2; ++h)
+            for (int j = 0; j < BLOCK_N / kBlockK; ++j)
+              if (mt * kBlockM + 64 * h < P && nt * BLOCK_N + kBlockK * j < a.Cout)
+                ptx::tma_load_2d(buf + (h * (BLOCK_N / kBlockK) + j) * kEpiBoxBytes, &tmap_r, &epi_full[eb], nt * BLOCK_N + kBlockK * j,
+                                 mt * kBlockM + 64 * h);
+          if (++eb == C::kEpiBufs) { eb = 0; ephase ^= 1; }
+        }
+      }
+    }
   } else {
     // ===================== consumers: warpgroup g = rows 64g .. 64g+63 of the tile =====================
     const int g = (warp >> 2) - 1;
@@ -156,6 +206,8 @@ conv_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_co
     float tot[SPLIT ? R : 1];
     double sq_acc = 0.0;
     int stage = 0; uint32_t phase = 0;
+    int eb = 0; uint32_t ephase = 0;                           // TMA epilogue: tile buffer of the current tile
+    const bool epi_leader = (threadIdx.x & 127) == 0;          //   the thread that issues its warpgroup's stores
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
       const int tu = a.reverse ? total_tiles - 1 - tile : tile;
       const int tl = tu / a.splits, sp = tu - tl * a.splits;
@@ -212,7 +264,7 @@ conv_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_co
       }
       float* v = acc;
 
-      // ---- epilogue straight from the fragment ----
+      // ---- epilogue from the fragment ----
       // the thread's two output rows (fragment rows r_lo and r_lo + 8); in[h] = false past the output
       bool in[2];
       float* yrow[2];
@@ -254,41 +306,98 @@ conv_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_co
 #pragma unroll
         for (int i = 0; i < R; ++i) v[i] = __fadd_rn(v[i], t[(i >> 2) * 2 + (i & 1)]);
       }
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        if (!rrow[h]) continue;
-        gather(rrow[h]);
-#pragma unroll
-        for (int j = 0; j < BLOCK_N / 8; ++j) {
-          v[4 * j + 2 * h] = __fadd_rn(v[4 * j + 2 * h], t[2 * j]);
-          v[4 * j + 2 * h + 1] = __fadd_rn(v[4 * j + 2 * h + 1], t[2 * j + 1]);
+      if constexpr (TMA_EPI) {
+        // The residual and the output share the tile buffer: the thread reads the residual at its own fragment positions and writes
+        // the finished values back to the same positions, so the two passes need no barrier between them.  Position of fragment row
+        // rl and column c: box c / 32 of the warpgroup's half, row rl of 128 B, 16-byte chunk (c % 32) / 4 XOR rl % 8 (SWIZZLE_128B,
+        // which also spreads the float2 accesses of a warp over all banks).
+        uint8_t* half = epi_smem + eb * C::kEpiBytes + g * (C::kEpiBytes / 2);
+        const uint32_t frag = (uint32_t)((wq * 16 + (lane >> 2)) * 128 + (cq & 3) * 4);
+        auto at = [&](int h, int j) -> float2* {
+          return reinterpret_cast<float2*>(half + (j >> 2) * kEpiBoxBytes + frag + h * 8 * 128 +
+                                           ((((j & 3) * 2 + (cq >> 2)) ^ (lane >> 2)) << 4));
+        };
+        // the previous tile's stores have had this tile's K loop to read their buffer: hand it to the residual loader
+        if (epi_leader && tile != blockIdx.x) {
+          ptx::bulk_wait_group_read<0>();
+          ptx::mbar_arrive(&epi_empty[eb == 0 ? C::kEpiBufs - 1 : eb - 1]);
         }
-      }
-      // Pass 2: activation, rounding, sum of squares, stores
+        ptx::mbar_wait(&epi_full[eb], ephase);
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        if (!in[h]) continue;
-        float part = 0.f;
+        for (int h = 0; h < 2; ++h) {
 #pragma unroll
-        for (int j = 0; j < BLOCK_N / 8; ++j) {
-          const int c = c0 + 8 * j;
-          if (c >= a.Cout) continue;
-          const bool two = c + 1 < a.Cout;
-          float v0 = v[4 * j + 2 * h], v1 = v[4 * j + 2 * h + 1];
-          v0 = epi_act(v0, a.act, a.slope); v1 = epi_act(v1, a.act, a.slope);
-          if (a.round_out) { v0 = ptx::round_tf32(v0); v1 = ptx::round_tf32(v1); }
-          if (a.sumsq) part = fmaf(v0, v0, two ? fmaf(v1, v1, part) : part);
-          if (a.no_store) continue;
-          float* y = yrow[h];
-          if (two && !((reinterpret_cast<uintptr_t>(y + c)) & 7)) {
-            *reinterpret_cast<float2*>(y + c) = make_float2(v0, v1);
-          } else {
-            y[c] = v0;
-            if (two) y[c + 1] = v1;
+          for (int j = 0; j < BLOCK_N / 8; ++j) {
+            const float2 r = *at(h, j);
+            v[4 * j + 2 * h] = __fadd_rn(v[4 * j + 2 * h], r.x);
+            v[4 * j + 2 * h + 1] = __fadd_rn(v[4 * j + 2 * h + 1], r.y);
           }
         }
-        sq_acc += (double)part;                                 // fp32 within a row of the tile, fp64 across rows and tiles
+        // Pass 2: activation, rounding, sum of squares (from the registers), values into the buffer
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          float part = 0.f;
+#pragma unroll
+          for (int j = 0; j < BLOCK_N / 8; ++j) {
+            const int c = c0 + 8 * j;
+            float v0 = v[4 * j + 2 * h], v1 = v[4 * j + 2 * h + 1];
+            v0 = epi_act(v0, a.act, a.slope); v1 = epi_act(v1, a.act, a.slope);
+            if (a.round_out) { v0 = ptx::round_tf32(v0); v1 = ptx::round_tf32(v1); }
+            if (a.sumsq && c < a.Cout) part = fmaf(v0, v0, c + 1 < a.Cout ? fmaf(v1, v1, part) : part);
+            *at(h, j) = make_float2(v0, v1);
+          }
+          if (in[h]) sq_acc += (double)part;
+        }
+        // one TMA store per 32-channel box of the warpgroup's 64 rows; the tensor map clips rows past P and channels past Cout
+        ptx::fence_proxy_async();
+        ptx::named_bar_sync(1 + g, 128);
+        if (epi_leader) {
+          const int row0 = mt * kBlockM + 64 * g;
+          if (row0 < a.OW)
+            for (int j = 0; j < BLOCK_N / kBlockK; ++j)
+              if (nt * BLOCK_N + kBlockK * j < a.Cout) ptx::tma_store_2d(&tmap_y, half + j * kEpiBoxBytes, nt * BLOCK_N + kBlockK * j, row0);
+          ptx::bulk_commit_group();
+        }
+        if (++eb == C::kEpiBufs) { eb = 0; ephase ^= 1; }
+      } else {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          if (!rrow[h]) continue;
+          gather(rrow[h]);
+#pragma unroll
+          for (int j = 0; j < BLOCK_N / 8; ++j) {
+            v[4 * j + 2 * h] = __fadd_rn(v[4 * j + 2 * h], t[2 * j]);
+            v[4 * j + 2 * h + 1] = __fadd_rn(v[4 * j + 2 * h + 1], t[2 * j + 1]);
+          }
+        }
+        // Pass 2: activation, rounding, sum of squares, stores
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          if (!in[h]) continue;
+          float part = 0.f;
+#pragma unroll
+          for (int j = 0; j < BLOCK_N / 8; ++j) {
+            const int c = c0 + 8 * j;
+            if (c >= a.Cout) continue;
+            const bool two = c + 1 < a.Cout;
+            float v0 = v[4 * j + 2 * h], v1 = v[4 * j + 2 * h + 1];
+            v0 = epi_act(v0, a.act, a.slope); v1 = epi_act(v1, a.act, a.slope);
+            if (a.round_out) { v0 = ptx::round_tf32(v0); v1 = ptx::round_tf32(v1); }
+            if (a.sumsq) part = fmaf(v0, v0, two ? fmaf(v1, v1, part) : part);
+            if (a.no_store) continue;
+            float* y = yrow[h];
+            if (two && !((reinterpret_cast<uintptr_t>(y + c)) & 7)) {
+              *reinterpret_cast<float2*>(y + c) = make_float2(v0, v1);
+            } else {
+              y[c] = v0;
+              if (two) y[c + 1] = v1;
+            }
+          }
+          sq_acc += (double)part;                               // fp32 within a row of the tile, fp64 across rows and tiles
+        }
       }
+    }
+    if constexpr (TMA_EPI) {
+      if (epi_leader) ptx::bulk_wait_group<0>();                // the last stores read shared memory until they complete
     }
     if (a.sumsq) {
       for (int o = 16; o > 0; o >>= 1) sq_acc += __shfl_xor_sync(0xffffffffu, sq_acc, o);
@@ -339,11 +448,15 @@ EncodeTiledFn get_encode_tiled() {
 }
 
 
-bool encode(CUtensorMap* m, int rank, const void* base, const cuuint64_t* dims, const cuuint64_t* strides_bytes,
+// Operand maps round to TF32 on load (CU_TENSOR_MAP_DATA_TYPE_TFLOAT32 under g_tf32_tma_type); epilogue maps (residual, output) are
+// FLOAT32 and move the values unchanged.
+CUtensorMapDataType operand_type() { return g_tf32_tma_type ? CU_TENSOR_MAP_DATA_TYPE_TFLOAT32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32; }
+
+bool encode(CUtensorMap* m, CUtensorMapDataType type, int rank, const void* base, const cuuint64_t* dims, const cuuint64_t* strides_bytes,
             const cuuint32_t* box, const cuuint32_t* estr, const char* who) {
   EncodeTiledFn fn = get_encode_tiled();
   if (!fn) { set_error_msg(who, "cuTensorMapEncodeTiled unavailable (no CUDA driver)"); return false; }
-  CUresult r = fn(m, g_tf32_tma_type ? CU_TENSOR_MAP_DATA_TYPE_TFLOAT32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, (cuuint32_t)rank,
+  CUresult r = fn(m, type, (cuuint32_t)rank,
                   const_cast<void*>(base), dims, strides_bytes, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
@@ -365,21 +478,30 @@ void pick_rect(int OH, int OW, int stride, int* BH, int* BW) {
   }
 }
 
-template <int BLOCK_N, bool SPLIT>
-int launch(const CUtensorMap& tx, const CUtensorMap& tw, const CUtensorMap& tx2, const CUtensorMap& tw2, const ConvArgs& a_in, cudaStream_t st) {
-  using C = Cfg<BLOCK_N, SPLIT>;
+template <int BLOCK_N, bool SPLIT, bool TMA_EPI>
+int launch(const CUtensorMap& tx, const CUtensorMap& tw, const CUtensorMap& tx2, const CUtensorMap& tw2, const CUtensorMap& tr,
+           const CUtensorMap& ty, const ConvArgs& a_in, cudaStream_t st) {
+  using C = Cfg<BLOCK_N, SPLIT, TMA_EPI>;
   ConvArgs a = a_in;
   a.nstages = C::kStages;
   static bool attr = false;
   if (!attr) {
-    cudaError_t e = cudaFuncSetAttribute(conv_fwd_sm90_kernel<BLOCK_N, SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::kSmemBytes);
+    cudaError_t e = cudaFuncSetAttribute(conv_fwd_sm90_kernel<BLOCK_N, SPLIT, TMA_EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::kSmemBytes);
     if (e != cudaSuccess) { set_error("skd_conv2d_fwd_sm100(attr)", e); return 0; }
     attr = true;
   }
   int grid = a.m_tiles * a.n_tiles * a.splits;
   if (grid > kNumSMs) grid = kNumSMs;
-  conv_fwd_sm90_kernel<BLOCK_N, SPLIT><<<grid, kThreads, C::kSmemBytes, st>>>(tx, tw, tx2, tw2, a);
+  conv_fwd_sm90_kernel<BLOCK_N, SPLIT, TMA_EPI><<<grid, kThreads, C::kSmemBytes, st>>>(tx, tw, tx2, tw2, tr, ty, a);
   return finish("skd_conv2d_fwd_sm100");
+}
+
+template <int BLOCK_N>
+int launch_n(bool split3, bool tma_epi, const CUtensorMap& tx, const CUtensorMap& tw, const CUtensorMap& tx2, const CUtensorMap& tw2,
+             const CUtensorMap& tr, const CUtensorMap& ty, const ConvArgs& a, cudaStream_t st) {
+  if (split3) return launch<BLOCK_N, true, false>(tx, tw, tx2, tw2, tr, ty, a, st);
+  if (tma_epi) return launch<BLOCK_N, false, true>(tx, tw, tx2, tw2, tr, ty, a, st);
+  return launch<BLOCK_N, false, false>(tx, tw, tx2, tw2, tr, ty, a, st);
 }
 
 }  // namespace
@@ -493,7 +615,7 @@ static int conv_fwd_impl(int N, int H, int W, int Cin, int Cout, int KH, int KW,
       int lower[2] = {-pad, -pad};                             // (W, H): filter origin of the first output pixel
       int upper[2] = {up_w, up_h};                             // last filter origin = dim-1 + upper
       cuuint32_t estr[4] = {1, (cuuint32_t)stride, (cuuint32_t)stride, 1};
-      CUresult r = get_encode_im2col()(m, g_tf32_tma_type ? CU_TENSOR_MAP_DATA_TYPE_TFLOAT32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4,
+      CUresult r = get_encode_im2col()(m, operand_type(), 4,
                                        const_cast<float*>(ptr), dims, strides, lower, upper, (cuuint32_t)kBlockK, (cuuint32_t)kBlockM, estr,
                                        CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
@@ -504,14 +626,14 @@ static int conv_fwd_impl(int N, int H, int W, int Cin, int Cout, int KH, int KW,
     cuuint64_t strides[3] = {(cuuint64_t)ldx * 4, (cuuint64_t)vW * ldx * 4, (cuuint64_t)vH * vW * ldx * 4};
     cuuint32_t box[4] = {(cuuint32_t)kBlockK, (cuuint32_t)(a.BW * stride), (cuuint32_t)(a.BH * stride), 1};
     cuuint32_t estr[4] = {1, (cuuint32_t)stride, (cuuint32_t)stride, 1};
-    return encode(m, 4, ptr, dims, strides, box, estr, who);
+    return encode(m, operand_type(), 4, ptr, dims, strides, box, estr, who);
   };
   auto encode_w = [&](CUtensorMap* m, const float* ptr) -> bool {
     cuuint64_t dims[3] = {(cuuint64_t)Cin, (cuuint64_t)(KH * KW), (cuuint64_t)Cout};
     cuuint64_t strides[2] = {(cuuint64_t)Cin * 4, (cuuint64_t)KH * KW * Cin * 4};
     cuuint32_t box[3] = {(cuuint32_t)kBlockK, 1, (cuuint32_t)bn};
     cuuint32_t estr[3] = {1, 1, 1};
-    return encode(m, 3, ptr, dims, strides, box, estr, who);
+    return encode(m, operand_type(), 3, ptr, dims, strides, box, estr, who);
   };
   if (!encode_x(&tx, x) || !encode_w(&tw, w)) return 0;
   tx2 = tx; tw2 = tw;
@@ -520,15 +642,34 @@ static int conv_fwd_impl(int N, int H, int W, int Cin, int Cout, int KH, int KW,
     if ((reinterpret_cast<uintptr_t>(x_lo) | reinterpret_cast<uintptr_t>(w_lo)) & 15) { set_error_msg(who, "x_lo / w_lo not 16-byte aligned"); return 0; }
     if (!encode_x(&tx2, x_lo) || !encode_w(&tw2, w_lo)) return 0;
   }
+  // TMA epilogue: short-K launches with a residual (the teacher's bottleneck conv3), whose time goes to reading the residual and
+  // writing the output rather than to the K loop.  Without a residual, or with a longer K loop, the register epilogue and the deeper
+  // operand ring the tile buffers would cost are faster (DESIGN.md §6).  It needs the [P][Cout] pixel rows of the flat / im2col tile
+  // modes (so no strided output), a plain fp32 output (no split-K partials, no reduction-only launch) and pitches and pointers TMA can
+  // address (whole float4s, 16-byte aligned).
+  const bool tma_epi = (flat || a.im2col) && a.splits == 1 && !no_store && !split3 && residual &&
+                       KH * KW * a.k_chunks <= kTmaEpiMaxK && ldy % 4 == 0 && !(reinterpret_cast<uintptr_t>(y) & 15) &&
+                       ldr % 4 == 0 && !(reinterpret_cast<uintptr_t>(residual) & 15);
+  CUtensorMap tr{}, ty{};
+  if (tma_epi) {
+    auto encode_rows = [&](CUtensorMap* m, const float* ptr, int ld) -> bool {
+      cuuint64_t dims[2] = {(cuuint64_t)Cout, (cuuint64_t)P};
+      cuuint64_t strides[1] = {(cuuint64_t)ld * 4};
+      cuuint32_t box[2] = {(cuuint32_t)kBlockK, 64};
+      cuuint32_t estr[2] = {1, 1};
+      return encode(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, ptr, dims, strides, box, estr, who);
+    };
+    if (!encode_rows(&ty, y, ldy) || !encode_rows(&tr, residual, ldr)) return 0;
+  }
   a.kc_outer = kc_outer;
   a.reverse = (g_tile_order == 2) ? (g_tile_flip ^= 1) : g_tile_order;
   a.nstages = 0; a.sumsq = sumsq; a.no_store = no_store;
   if (strided_out && residual) { set_error_msg(who, "strided output takes no residual"); return 0; }
   int ok;
   switch (bn) {
-    case 128: ok = split3 ? launch<128, true>(tx, tw, tx2, tw2, a, st) : launch<128, false>(tx, tw, tx2, tw2, a, st); break;
-    case 64: ok = split3 ? launch<64, true>(tx, tw, tx2, tw2, a, st) : launch<64, false>(tx, tw, tx2, tw2, a, st); break;
-    default: ok = split3 ? launch<32, true>(tx, tw, tx2, tw2, a, st) : launch<32, false>(tx, tw, tx2, tw2, a, st); break;
+    case 128: ok = launch_n<128>(split3, tma_epi, tx, tw, tx2, tw2, tr, ty, a, st); break;
+    case 64: ok = launch_n<64>(split3, tma_epi, tx, tw, tx2, tw2, tr, ty, a, st); break;
+    default: ok = launch_n<32>(split3, tma_epi, tx, tw, tx2, tw2, tr, ty, a, st); break;
   }
   if (!ok || a.splits == 1) return ok;
   const long long tot4 = P * (Cout / 4);
