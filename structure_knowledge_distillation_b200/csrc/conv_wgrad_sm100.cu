@@ -4,12 +4,15 @@
 //   dW[co][tap][ci] = sum_{pixels p} dY[p][co] * X[p shifted by tap][ci]
 //
 // GEMM view: M = Cout (128 per tile), N = Cin (<= 128 per tile, one filter tap per tile), K = pixels.  Both operands lie in HBM with
-// the channels contiguous (NHWC), i.e. MN-major, and wgmma takes tf32 operands only K-major.  So per pipeline stage TMA drops
-// 32-channel x 32-pixel boxes (128B-swizzled, one pixel per 128-byte row) of dY and X into a raw stage, the two consumer warpgroups
-// transpose them into K-major 128B-swizzled tiles (one channel per 128-byte row, double-buffered so the transposition of the next
-// K-block overlaps the wgmmas of this one) and release the raw stage at once; each warpgroup then issues 4 x wgmma.m64nNk8.tf32 for
-// its 64 Cout rows.  Split-K over pixel blocks gives >= 2 waves of work units; fp32 partials go to a workspace and a deterministic
-// reduction adds them in fixed order.
+// the channels contiguous (NHWC), i.e. MN-major, and TF32 wgmma takes a shared-memory operand only K-major.  Per pipeline stage TMA
+// drops 32-channel x 32-pixel boxes (128B-swizzled, one pixel per 128-byte row) of dY and X into a raw stage.
+//  * dY is the A operand and goes to the tensor core from registers: each consumer thread loads its A fragments straight from the raw
+//    box (no transposed copy), so a dY box is never rewritten, however many taps and Cin tiles read it.
+//  * X is the B operand: warps 1-3 of the producer warpgroup transpose it into a ring of K-major 128B-swizzled tiles (one channel per
+//    128-byte row) with its own full / empty barriers, so the transposition of later K-blocks runs while the consumers' wgmmas run.
+//  * The raw stage is released once the three transposer warps have read X and the eight consumer warps have loaded their fragments.
+// Each consumer warpgroup issues 4 x wgmma.m64nNk8.tf32 per K-block for its 64 Cout rows.  Split-K over pixel blocks gives >= 2 waves
+// of work units; fp32 partials go to a workspace and a deterministic reduction adds them in fixed order.
 #include <cuda.h>
 
 #include "common.cuh"
@@ -22,9 +25,11 @@ namespace {
 
 constexpr int kBlockM = 128;               // Cout per tile
 constexpr int kKPix = 32;                  // pixels per pipeline stage (one 128-byte K row of the transposed tiles)
-constexpr int kThreads = 384;              // producer warpgroup + 2 consumer warpgroups
+constexpr int kThreads = 384;              // producer warpgroup (TMA thread + 3 transposer warps) + 2 consumer warpgroups
+constexpr int kTransposeThreads = 96;
 constexpr int kChunkBytes = 32 * kKPix * 4;        // one 32-channel x 32-pixel box
 constexpr int kMaxStages = 4;
+constexpr int kSets = 3;                   // transposed X sets
 
 struct WgArgs {
   int N, OH, OW, Cout, Cin, KH, KW, stride, pad, dil;
@@ -37,18 +42,37 @@ struct WgArgs {
 template <int BLOCK_N>
 struct WCfg {
   static constexpr int kABytes = 4 * kChunkBytes;                    // 128 co
-  static constexpr int kBBytes = (BLOCK_N / 32) * kChunkBytes;
-  static constexpr int kStageBytes = kABytes + kBBytes;              // raw (pixel-major) stage; the transposed set has the same size
-  static constexpr int kFit = (232448 - 2 * kStageBytes - 1024 - 256) / kStageBytes;
+  static constexpr int kBBytes = (BLOCK_N / 32) * kChunkBytes;       // one X box; its transposed tile has the same size
+  static constexpr int kStageBytes = kABytes + kBBytes;              // raw (pixel-major) stage
+  static constexpr int kFit = (232448 - kSets * kBBytes - 1024 - 256) / kStageBytes;
   static constexpr int kStages = kFit > kMaxStages ? kMaxStages : kFit;
-  static constexpr int kSmemBytes = (kStages + 2) * kStageBytes + 1024 + 256;
+  static constexpr int kSmemBytes = kStages * kStageBytes + kSets * kBBytes + 1024 + 256;
   static_assert(kStages >= 2, "at least two pipeline stages");
 };
 
-// raw box (pixel rows of 32 channels, 128B swizzle) -> K-major tile (channel rows of 32 pixels, 128B swizzle); unit = 4 pixels x 4 channels
-__device__ __forceinline__ void transpose_tile(const uint8_t* raw, uint8_t* dst, int rows, int t) {
-  for (int u = t; u < rows * 2; u += 256) {
-    const int pg = u & 7, cg = u >> 3;
+struct Unit { int split, mt, nt, tap; };
+
+__device__ __forceinline__ Unit decode_unit(const WgArgs& a, int u) {
+  const int tiles = a.m_tiles * a.taps * a.n_tiles;
+  Unit w;
+  w.split = u / tiles;
+  const int tile = u - w.split * tiles;
+  w.mt = tile / (a.taps * a.n_tiles);
+  const int r = tile - w.mt * (a.taps * a.n_tiles);
+  w.tap = r / a.n_tiles;
+  w.nt = r - w.tap * a.n_tiles;
+  return w;
+}
+
+// X box (pixel rows of 32 channels, 128B swizzle) -> K-major tile (channel rows of 32 pixels, 128B swizzle); unit = 4 pixels x 4
+// channels, read as 4 float4 (one per pixel row) and written as 4 float4 (one per channel row).  Unit u: q = u & 7, channel group
+// cg = 8 (u >> 6) + q, pixel group pg = q ^ ((u >> 3) & 7).  A quarter-warp (one 128-bit wavefront) holds q = 0..7 with the rest of
+// u fixed, and both its 16-byte slot maps are permutations of 0..7 (enumerated on the host), so neither side has bank conflicts:
+// reads (cg & 7) ^ ((4 pg + i) & 7) = q ^ 4 ((q ^ s) & 1) ^ i, writes pg ^ ((4 cg + e) & 7) = q ^ s ^ 4 (q & 1) ^ e.
+template <int BLOCK_N>
+__device__ __forceinline__ void transpose_x(const uint8_t* raw, uint8_t* dst, int t) {
+  for (int u = t; u < BLOCK_N * 2; u += kTransposeThreads) {
+    const int q = u & 7, pg = q ^ ((u >> 3) & 7), cg = ((u >> 6) << 3) + q;
     const uint8_t* src = raw + (cg >> 3) * kChunkBytes;
     float4 r[4];
 #pragma unroll
@@ -72,111 +96,154 @@ conv_wgrad_sm90_kernel(const __grid_constant__ CUtensorMap tmap_dy, const __grid
   // keep the pointer in the shared address space (integer round trips make nvcc emit generic LD/ST instead of LDS/STS)
   const uint32_t raw_addr = ptx::smem_u32(smem_raw);
   uint8_t* smem = smem_raw + (((raw_addr + 1023u) & ~1023u) - raw_addr);
-  uint8_t* sets = smem + C::kStages * C::kStageBytes;                // 2 transposed {A, B} sets
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(sets + 2 * C::kStageBytes);
+  uint8_t* sets = smem + C::kStages * C::kStageBytes;                // kSets transposed X tiles
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(sets + kSets * C::kBBytes);
   uint64_t* empty_bar = full_bar + kMaxStages;
+  uint64_t* xfull_bar = empty_bar + kMaxStages;
+  uint64_t* xempty_bar = xfull_bar + kSets;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
   if (threadIdx.x == 0) {
     ptx::prefetch_tmap(&tmap_dy); ptx::prefetch_tmap(&tmap_x);
-    for (int s = 0; s < C::kStages; ++s) { ptx::mbar_init(&full_bar[s], 1); ptx::mbar_init(&empty_bar[s], 1); }
+    // one arrival per warp: raw stage <- 3 transposer + 8 consumer warps, X set full <- 3 transposer warps, empty <- 8 consumer warps
+    for (int s = 0; s < C::kStages; ++s) { ptx::mbar_init(&full_bar[s], 1); ptx::mbar_init(&empty_bar[s], 11); }
+    for (int s = 0; s < kSets; ++s) { ptx::mbar_init(&xfull_bar[s], 3); ptx::mbar_init(&xempty_bar[s], 8); }
     ptx::fence_barrier_init();
   }
   __syncthreads();
 
-  const int tiles = a.m_tiles * a.taps * a.n_tiles;
-  const int units = tiles * a.splits;
+  const int units = a.m_tiles * a.taps * a.n_tiles * a.splits;
   const int kb_per_img = a.kb_x * a.kb_y;
 
-  if (warp < 4) {
+  if (warp == 0) {
     // ===================== TMA producer =====================
     // all-out-of-range channel chunks (Cout or Cin < tile) are not issued
     if (threadIdx.x == 0) {
       int stage = 0; uint32_t phase = 0;
       for (int u = blockIdx.x; u < units; u += gridDim.x) {
-        const int split = u / tiles, tile = u - split * tiles;
-        const int mt = tile / (a.taps * a.n_tiles), r = tile - mt * (a.taps * a.n_tiles);
-        const int tap = r / a.n_tiles, nt = r - tap * a.n_tiles;
-        const int kh = tap / a.KW, kw = tap - kh * a.KW;
-        const int kb0 = split * a.kb_per_split;
+        const Unit w = decode_unit(a, u);
+        const int kb0 = w.split * a.kb_per_split;
         const int kb1 = min(a.kb_total, kb0 + a.kb_per_split);
-        const int a_chunks = min(4, (a.Cout - mt * kBlockM + 31) / 32);
-        const int b_chunks = max(0, min(BLOCK_N / 32, (a.Cin - nt * BLOCK_N + 31) / 32));
+        const int a_chunks = min(4, (a.Cout - w.mt * kBlockM + 31) / 32);
+        const int b_chunks = max(0, min(BLOCK_N / 32, (a.Cin - w.nt * BLOCK_N + 31) / 32));
         for (int kb = kb0; kb < kb1; ++kb) {
           ptx::mbar_wait(&empty_bar[stage], phase ^ 1);
           uint8_t* sa = smem + stage * C::kStageBytes;
           uint8_t* sb = sa + C::kABytes;
           ptx::mbar_expect_tx(&full_bar[stage], (uint32_t)((a_chunks + b_chunks) * kChunkBytes));
+          const int kh = w.tap / a.KW, kw = w.tap - kh * a.KW;
           if (a.linear) {
             const int p0 = kb * kKPix;
             const int img = p0 / (a.OH * a.OW), r2 = p0 - img * (a.OH * a.OW);
             const int oy = r2 / a.OW, ox = r2 - oy * a.OW;
             for (int c = 0; c < a_chunks; ++c)
-              ptx::tma_load_4d(sa + c * kChunkBytes, &tmap_dy, &full_bar[stage], mt * kBlockM + c * 32, p0, 0, 0);
+              ptx::tma_load_4d(sa + c * kChunkBytes, &tmap_dy, &full_bar[stage], w.mt * kBlockM + c * 32, p0, 0, 0);
             for (int c = 0; c < b_chunks; ++c)
-              ptx::tma_load_im2col_4d(sb + c * kChunkBytes, &tmap_x, &full_bar[stage], nt * BLOCK_N + c * 32, ox * a.stride - a.pad,
+              ptx::tma_load_im2col_4d(sb + c * kChunkBytes, &tmap_x, &full_bar[stage], w.nt * BLOCK_N + c * 32, ox * a.stride - a.pad,
                                       oy * a.stride - a.pad, img, (uint16_t)(kw * a.dil), (uint16_t)(kh * a.dil));
           } else {
             const int img = kb / kb_per_img, q = kb - img * kb_per_img;
             const int by = q / a.kb_x, bx = q - by * a.kb_x;
             const int oy0 = by * a.BHk, ox0 = bx * a.BWk;
             for (int c = 0; c < a_chunks; ++c)
-              ptx::tma_load_4d(sa + c * kChunkBytes, &tmap_dy, &full_bar[stage], mt * kBlockM + c * 32, ox0, oy0, img);
+              ptx::tma_load_4d(sa + c * kChunkBytes, &tmap_dy, &full_bar[stage], w.mt * kBlockM + c * 32, ox0, oy0, img);
             for (int c = 0; c < b_chunks; ++c)
-              ptx::tma_load_4d(sb + c * kChunkBytes, &tmap_x, &full_bar[stage], nt * BLOCK_N + c * 32,
+              ptx::tma_load_4d(sb + c * kChunkBytes, &tmap_x, &full_bar[stage], w.nt * BLOCK_N + c * 32,
                                ox0 * a.stride - a.pad + kw * a.dil, oy0 * a.stride - a.pad + kh * a.dil, img);
           }
           if (++stage == C::kStages) { stage = 0; phase ^= 1; }
         }
       }
     }
+  } else if (warp < 4) {
+    // ===================== X transposer (warps 1-3) =====================
+    const int t = threadIdx.x - 32;                            // 0..95
+    int stage = 0; uint32_t phase = 0; int xs = 0; uint32_t xphase = 0;
+    for (int u = blockIdx.x; u < units; u += gridDim.x) {
+      const Unit w = decode_unit(a, u);
+      const int kb0 = w.split * a.kb_per_split;
+      const int nkb = min(a.kb_total, kb0 + a.kb_per_split) - kb0;
+      for (int k = 0; k < nkb; ++k) {
+        ptx::mbar_wait(&full_bar[stage], phase);
+        ptx::mbar_wait(&xempty_bar[xs], xphase ^ 1);
+        const uint8_t* raw = smem + stage * C::kStageBytes + C::kABytes;
+        transpose_x<BLOCK_N>(raw, sets + xs * C::kBBytes, t);
+        ptx::fence_proxy_async();                              // generic-proxy writes -> visible to the wgmma (async proxy) reads
+        __syncwarp();
+        if (lane == 0) { ptx::mbar_arrive(&empty_bar[stage]); ptx::mbar_arrive(&xfull_bar[xs]); }
+        if (++stage == C::kStages) { stage = 0; phase ^= 1; }
+        if (++xs == kSets) { xs = 0; xphase ^= 1; }
+      }
+    }
   } else {
     // ===================== consumers =====================
-    const int t = threadIdx.x - 128;                           // 0..255
-    const int g = t >> 7;                                      // warpgroup: Cout rows 64g .. 64g+63 of the tile
-    const int wq = warp & 3;
-    const int r_lo = g * 64 + wq * 16 + (lane >> 2);
-    const int cq = 2 * (lane & 3);
+    const int g = (threadIdx.x - 128) >> 7;                    // warpgroup
+    const int wq = warp & 3, c8 = lane >> 2, j = lane & 3;
+    // MMA row 16 wq + 8 h + c8 of the warpgroup holds Cout 32 (wq >> 1) + 16 (c8 >> 2) + 8 (wq & 1) + 4 h + (c8 & 3) of its 64: with the
+    // fragment's k = j (+4) that puts the 32 lanes of every fragment load on 32 different banks (16-byte slot 4 (c8 >> 2) + 2 (wq & 1)
+    // + h of the 32-channel box, XOR pixel & 7 = j or j + 4: bank bits 4 / 3-2 / 1-0 = c8 >> 2 / j / c8 & 3, enumerated on the host).
+    // Cout = MMA row would put each load's lanes on 16 banks, two per bank.  Each dW element is still the same k8 MMA sequence over
+    // the same operands, only on another row of the tensor core.
+    const int co_base = 64 * g + 32 * (wq >> 1) + 16 * (c8 >> 2) + 8 * (wq & 1) + (c8 & 3);   // + 4 h
+    uint32_t off[4];                                           // byte offsets in the raw stage of (h, pixel & 4) for pixel 4i + j
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int slot = 4 * (c8 >> 2) + 2 * (wq & 1) + h;
+      const int base = (2 * g + (wq >> 1)) * kChunkBytes + j * 128 + 4 * (c8 & 3);
+      off[2 * h] = base + ((slot ^ j) << 4);
+      off[2 * h + 1] = base + ((slot ^ j ^ 4) << 4);
+    }
+    const int cq = 2 * j;
     const size_t kdim = (size_t)a.taps * a.Cin;
     float acc[BLOCK_N / 2];
-    int stage = 0; uint32_t phase = 0; uint32_t it = 0;        // it: K-blocks consumed so far (transposed-set parity)
+    uint32_t fa[16], fb[16];                                   // A fragments of two K-blocks: loads for k + 1 leave k's in-flight operands alone
+    int stage = 0; uint32_t phase = 0; int xs = 0; uint32_t xphase = 0;
+    int prev_xs = -1;                                          // X set of the previous K-block, released once its wgmmas are done
     for (int u = blockIdx.x; u < units; u += gridDim.x) {
-      const int split = u / tiles, tile = u - split * tiles;
-      const int mt = tile / (a.taps * a.n_tiles), r = tile - mt * (a.taps * a.n_tiles);
-      const int tap = r / a.n_tiles, nt = r - tap * a.n_tiles;
-      const int kb0 = split * a.kb_per_split;
+      const Unit w = decode_unit(a, u);
+      const int kb0 = w.split * a.kb_per_split;
       const int nkb = min(a.kb_total, kb0 + a.kb_per_split) - kb0;
-      for (int k = 0; k < nkb; ++k, ++it) {
-        uint8_t* set = sets + (it & 1) * C::kStageBytes;
+      auto kblock = [&](uint32_t (&f)[16], int k) {
         ptx::mbar_wait(&full_bar[stage], phase);
-        ptx::wgmma_wait<1>();                                  // this warpgroup's wgmmas of two K-blocks ago (same set) are done
-        ptx::named_bar_sync(1, 256);                           // ... and the other warpgroup's
         const uint8_t* raw = smem + stage * C::kStageBytes;
-        transpose_tile(raw, set, kBlockM, t);
-        transpose_tile(raw + C::kABytes, set + C::kABytes, BLOCK_N, t);
-        ptx::fence_proxy_async();                              // generic-proxy writes -> visible to the wgmma (async proxy) reads
-        ptx::named_bar_sync(1, 256);
-        if (t == 0) ptx::mbar_arrive(&empty_bar[stage]);       // raw stage consumed
-        const uint32_t sa = ptx::smem_u32(set) + (uint32_t)(g * 64 * 128);
-        const uint32_t sb = ptx::smem_u32(set) + (uint32_t)C::kABytes;
+        // fragment kk: a0 / a1 = rows h 0 / 1 at pixel 8kk + j, a2 / a3 the same at pixel 8kk + j + 4
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) {
+#pragma unroll
+          for (int r = 0; r < 4; ++r)
+            f[4 * kk + r] = *reinterpret_cast<const uint32_t*>(raw + off[2 * (r & 1) + (r >> 1)] + 1024 * kk + 512 * (r >> 1));
+        }
+        __syncwarp();
+        if (lane == 0) ptx::mbar_arrive(&empty_bar[stage]);
+        if (++stage == C::kStages) { stage = 0; phase ^= 1; }
+        ptx::mbar_wait(&xfull_bar[xs], xphase);
+        const uint32_t sb = ptx::smem_u32(sets + xs * C::kBBytes);
         ptx::wgmma_fence();
 #pragma unroll
         for (int kk = 0; kk < kKPix / 8; ++kk)
-          ptx::wgmma_tf32<BLOCK_N>(acc, ptx::make_wgmma_desc_sw128(sa + kk * 32), ptx::make_wgmma_desc_sw128(sb + kk * 32), (k | kk) != 0 ? 1u : 0u);
+          ptx::wgmma_tf32_rs<BLOCK_N>(acc, f[4 * kk], f[4 * kk + 1], f[4 * kk + 2], f[4 * kk + 3], ptx::make_wgmma_desc_sw128(sb + kk * 32),
+                                      (k | kk) != 0 ? 1u : 0u);
         ptx::wgmma_commit();
-        if (++stage == C::kStages) { stage = 0; phase ^= 1; }
-      }
+        ptx::wgmma_wait<1>();                                  // the previous K-block's wgmmas are done: its fragments and X tile are free
+        if (prev_xs >= 0) { __syncwarp(); if (lane == 0) ptx::mbar_arrive(&xempty_bar[prev_xs]); }
+        prev_xs = xs;
+        if (++xs == kSets) { xs = 0; xphase ^= 1; }
+      };
+      int k = 0;
+      for (; k + 1 < nkb; k += 2) { kblock(fa, k); kblock(fb, k + 1); }
+      if (k < nkb) kblock(fa, k);                              // odd count: fa's last wgmmas were retired by fb's wait
       ptx::wgmma_wait<0>();
+      if (prev_xs >= 0) { __syncwarp(); if (lane == 0) ptx::mbar_arrive(&xempty_bar[prev_xs]); prev_xs = -1; }
       ptx::fence_regs(acc);
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
-        const int co = mt * kBlockM + r_lo + 8 * h;
+        const int co = w.mt * kBlockM + co_base + 4 * h;
         if (co >= a.Cout) continue;
-        float* orow = a.ws + ((size_t)split * a.Cout + co) * kdim + (size_t)tap * a.Cin;
+        float* orow = a.ws + ((size_t)w.split * a.Cout + co) * kdim + (size_t)w.tap * a.Cin;
 #pragma unroll
-        for (int j = 0; j < BLOCK_N / 8; ++j) {
-          const int ci = nt * BLOCK_N + 8 * j + cq;            // even; Cin % 4 == 0, so ci + 1 < Cin too
-          if (ci < a.Cin) *reinterpret_cast<float2*>(orow + ci) = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+        for (int jj = 0; jj < BLOCK_N / 8; ++jj) {
+          const int ci = w.nt * BLOCK_N + 8 * jj + cq;         // even; Cin % 4 == 0, so ci + 1 < Cin too
+          if (ci < a.Cin) *reinterpret_cast<float2*>(orow + ci) = make_float2(acc[4 * jj + 2 * h], acc[4 * jj + 2 * h + 1]);
         }
       }
     }

@@ -188,8 +188,9 @@ def _sync_mean(t):
 class WgradOverlap:
     """Weight-gradient kernels on a side stream.  In the backward pass only the data-gradient chain (dgrad -> ABN backward -> dgrad
     ...) is sequential; a layer's weight gradient needs (x, dy) and feeds nothing but the optimizer.  Issued on a second stream the
-    wgmma wgrad kernels (12 K registers, no co-residency conflict) overlap the HBM-bound ABN backward passes of the chain instead
-    of queueing between them.  NetModel opens a window around G_loss.backward(); tensors a side-stream kernel reads are kept alive
+    wgmma wgrad kernels overlap the HBM-bound ABN backward passes of the chain instead of queueing between them.  A wgrad CTA
+    (384 threads, 39-58 K registers, 93-177 KB of shared memory) does not fit on an SM beside a large forward / data-gradient
+    conv CTA (about 200 KB of shared memory), so it overlaps the small ABN kernels, not those convolutions.  NetModel opens a window around G_loss.backward(); tensors a side-stream kernel reads are kept alive
     until the window's join, so the caching allocator cannot hand their memory to a main-stream kernel early (valid in eager
     mode and under CUDA-graph capture alike -- no record_stream)."""
     stream = None
