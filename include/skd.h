@@ -212,6 +212,9 @@ void skd_set_conv_tile_order(int mode); /* 0 (default) front-to-back, 1 back-to-
                                           the tail its producer left in L2) */
 void skd_set_conv_k_order(int mode);   /* K loop of k>1 convolutions: 0 (default) by working set, 1 taps outermost, 2 channel chunks outermost */
 void skd_set_conv_im2col(int on);      /* 1 (default): TMA im2col-mode M tiles for k>1 / strided convs; 0: rectangular tiled-mode tiles */
+void skd_set_conv_tile_m(int mode);    /* wgmma conv M tile: 0 (default) 256 rows for long-K launches with Cout > 128 that fill waves as
+                                          well as 128 rows do; 1 always 128; 2 256 wherever that path can run (flat / im2col, Cout > 64,
+                                          TF32, no split-K, register epilogue, an output tensor) */
 
 /* ---- E. pooling / resampling / optimiser ---- */
 int skd_pool_out_size_ceil(int in, int k, int s, int p);

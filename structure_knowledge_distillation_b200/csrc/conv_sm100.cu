@@ -20,6 +20,9 @@
 //   TMA_EPI         (short-K flat / im2col launches with a residual) the residual comes in and the output goes out through a
 //                   shared-memory tile: thread 32 of warpgroup 0 loads the tile's residual by TMA while the K loop runs, and each
 //                   consumer warpgroup hands its finished 64 rows to one TMA store and starts the next tile's wgmmas without waiting.
+//   BLOCK_M = 256   (long-K flat / im2col launches) 256-pixel tiles: the producer loads A as two 128-row boxes, warpgroup g owns
+//                   rows 128g .. 128g+127 as two m64 sub-tiles sharing each B read, so a stage brings 48 KB for twice the MMA work
+//                   of a 32 KB 128-row stage.  setmaxnreg moves registers from the producer warpgroup to the two accumulators.
 #include <cuda.h>
 
 #include "common.cuh"
@@ -30,12 +33,15 @@ using namespace skd;
 
 namespace {
 
-constexpr int kBlockM = 128;
+constexpr int kBlockM = 128;                // rows of one A box (and of the default tile; a 256-row tile is two boxes)
 constexpr int kBlockK = 32;                 // fp32 elements = 128 B = one swizzle row
 constexpr int kWgmmaK = 8;                  // tf32
 constexpr int kThreads = 384;               // producer warpgroup + 2 consumer warpgroups
-constexpr int kABytes = kBlockM * kBlockK * 4;
+constexpr int kBoxBytes = kBlockM * kBlockK * 4;
+constexpr int kProducerRegs = 40;           // BLOCK_M = 256: per-thread registers of the producer / consumer warpgroups after
+constexpr int kConsumerRegs = 232;          //   setmaxnreg; 128 * 40 + 256 * 232 = 64 512 <= the 65 536 of the SM
 constexpr int kTmaEpiMaxK = 16;             // longest K loop (taps x 32-channel chunks) that takes the TMA epilogue
+constexpr int kTile256MinK = 128;           // shortest K loop that takes 256-row tiles
 constexpr int kEpiBoxBytes = 64 * kBlockK * 4;   // TMA epilogue box: 64 rows x 32 channels
 
 struct ConvArgs {
@@ -58,9 +64,13 @@ struct ConvArgs {
   long long split_stride;          //   raw fp32 partials go to y + split * split_stride; splitk_epilogue_kernel adds them and applies the epilogue
 };
 
-template <int BLOCK_N, bool SPLIT, bool TMA_EPI>
+template <int BLOCK_M, int BLOCK_N, bool SPLIT, bool TMA_EPI>
 struct Cfg {
   static_assert(!(SPLIT && TMA_EPI), "the TMA epilogue serves single-precision launches only");
+  static_assert(BLOCK_M == kBlockM || (BLOCK_M == 2 * kBlockM && BLOCK_N == 128 && !SPLIT && !TMA_EPI),
+                "256-row tiles: BLOCK_N 128, single precision, register epilogue");
+  static constexpr int kMS = BLOCK_M / kBlockM;                // m64 sub-tiles per consumer warpgroup
+  static constexpr int kABytes = BLOCK_M * kBlockK * 4;
   static constexpr int kBBytes = BLOCK_N * kBlockK * 4;
   static constexpr int kStageBytes = (kABytes + kBBytes) * (SPLIT ? 2 : 1);   // split precision: {x_hi, w_hi, x_lo, w_lo}
   // TMA epilogue: ring of output tiles (128 rows x BLOCK_N fp32, 32-channel x 64-row boxes of 128B-swizzled rows), taken out of the
@@ -88,12 +98,12 @@ __device__ __forceinline__ float epi_act(float v, int act, float slope) {
 // its store has read the buffer).  The output may be the residual itself (Bottleneck.frozen adds in place).  That stays safe:
 // a tile reads its residual only from the rows and channels it writes, its load has completed (epi_full) before its own store is
 // issued, and no two tiles of a launch write the same element.
-template <int BLOCK_N, bool SPLIT, bool TMA_EPI>
+template <int BLOCK_M, int BLOCK_N, bool SPLIT, bool TMA_EPI>
 __global__ void __launch_bounds__(kThreads, 1)
 conv_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_w,
                      const __grid_constant__ CUtensorMap tmap_x2, const __grid_constant__ CUtensorMap tmap_w2,
                      const __grid_constant__ CUtensorMap tmap_r, const __grid_constant__ CUtensorMap tmap_y, const ConvArgs a) {
-  using C = Cfg<BLOCK_N, SPLIT, TMA_EPI>;
+  using C = Cfg<BLOCK_M, BLOCK_N, SPLIT, TMA_EPI>;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   // keep the pointer in the shared address space (integer round trips make nvcc emit generic LD/ST instead of LDS/STS)
   const uint32_t raw_addr = ptx::smem_u32(smem_raw);
@@ -125,6 +135,7 @@ conv_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_co
 
   if (warp < 4) {
     // ===================== TMA producer =====================
+    if constexpr (C::kMS > 1) ptx::setmaxnreg_dec<kProducerRegs>();
     if (threadIdx.x == 0) {
       int stage = 0; uint32_t phase = 0;
       for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
@@ -134,15 +145,22 @@ conv_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_co
         const int img = mt / tiles_per_img, rem = mt - img * tiles_per_img;
         const int ty = rem / a.tiles_x, tx = rem - ty * a.tiles_x;
         const int iy0 = ty * a.BH * a.stride - a.pad, ix0 = tx * a.BW * a.stride - a.pad;
-        // im2col: first output pixel of the tile (n, p, q) -> filter-origin input coordinates
-        int in0 = 0, ip0 = 0, iq0 = 0;
+        // im2col: first output pixel of each A box (n, p, q) -> filter-origin input coordinates
+        int in0[C::kMS] = {}, ip0[C::kMS] = {}, iq0[C::kMS] = {};
         if (a.im2col) {
-          const int m0 = mt * kBlockM;
-          in0 = m0 / (a.rOH * a.rOW);
-          const int r2 = m0 - in0 * (a.rOH * a.rOW);
-          ip0 = (r2 / a.rOW) * a.stride - a.pad;
-          iq0 = (r2 % a.rOW) * a.stride - a.pad;
+#pragma unroll
+          for (int b = 0; b < C::kMS; ++b) {
+            const int m0 = mt * BLOCK_M + b * kBlockM;
+            in0[b] = m0 / (a.rOH * a.rOW);
+            const int r2 = m0 - in0[b] * (a.rOH * a.rOW);
+            ip0[b] = (r2 / a.rOW) * a.stride - a.pad;
+            iq0[b] = (r2 % a.rOW) * a.stride - a.pad;
+          }
         }
+        // 256-row tiles (flat / im2col, a.OW = P): a second box that starts past P is not loaded.  Its rows of the stage keep
+        // whatever an earlier stage left there; a GEMM row depends on its own A row only, and rows past P are never stored.
+        const int boxes = (C::kMS > 1 && mt * BLOCK_M + kBlockM >= a.OW) ? 1 : C::kMS;
+        const uint32_t stage_tx = (uint32_t)(C::kStageBytes - (C::kMS - boxes) * kBoxBytes);
         // kc_outer: channel chunk outermost, filter taps innermost -- the taps of one chunk re-read (shifted) the same input lines,
         // L2 hits whatever Cin is; taps outermost streams Cin * 128 pixels per CTA between reuses.
         const int n_inner = a.kc_outer ? taps : a.k_chunks;
@@ -153,17 +171,22 @@ conv_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_co
           const int kh = tap / a.KW, kw = tap - kh * a.KW;
           ptx::mbar_wait(&empty_bar[stage], phase ^ 1);
           uint8_t* sa = smem + stage * C::kStageBytes;
-          ptx::mbar_expect_tx(&full_bar[stage], (uint32_t)C::kStageBytes);
+          ptx::mbar_expect_tx(&full_bar[stage], stage_tx);
 #pragma unroll
           for (int part = 0; part < (SPLIT ? 2 : 1); ++part) {
             const CUtensorMap* mx = part ? &tmap_x2 : &tmap_x;
             const CUtensorMap* mw = part ? &tmap_w2 : &tmap_w;
-            uint8_t* pa = sa + part * (kABytes + C::kBBytes);
-            uint8_t* pb = pa + kABytes;
-            if (a.im2col)
-              ptx::tma_load_im2col_4d(pa, mx, &full_bar[stage], kc * kBlockK, iq0, ip0, in0, (uint16_t)(kw * a.dil), (uint16_t)(kh * a.dil));
-            else
-              ptx::tma_load_4d(pa, mx, &full_bar[stage], kc * kBlockK, ix0 + kw * a.dil, iy0 + kh * a.dil, img);
+            uint8_t* pa = sa + part * (C::kABytes + C::kBBytes);
+            uint8_t* pb = pa + C::kABytes;
+#pragma unroll
+            for (int b = 0; b < C::kMS; ++b) {
+              if (b >= boxes) break;
+              if (a.im2col)
+                ptx::tma_load_im2col_4d(pa + b * kBoxBytes, mx, &full_bar[stage], kc * kBlockK, iq0[b], ip0[b], in0[b], (uint16_t)(kw * a.dil),
+                                        (uint16_t)(kh * a.dil));
+              else
+                ptx::tma_load_4d(pa + b * kBoxBytes, mx, &full_bar[stage], kc * kBlockK, ix0 + b * kBlockM + kw * a.dil, iy0 + kh * a.dil, img);
+            }
             ptx::tma_load_3d(pb, mw, &full_bar[stage], kc * kBlockK, tap, nt * BLOCK_N);
           }
           if (++stage == a.nstages) { stage = 0; phase ^= 1; }
@@ -196,13 +219,15 @@ conv_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_co
       }
     }
   } else {
-    // ===================== consumers: warpgroup g = rows 64g .. 64g+63 of the tile =====================
+    // ===================== consumers: warpgroup g = rows 64g .. 64g+63 of the tile (128g .. 128g+127 at BLOCK_M 256) =====================
+    if constexpr (C::kMS > 1) ptx::setmaxnreg_inc<kConsumerRegs>();
+    constexpr int MS = C::kMS;
     const int g = (warp >> 2) - 1;
     const int wq = warp & 3;
-    const int r_lo = g * 64 + wq * 16 + (lane >> 2);          // tile rows of this thread's fragment: r_lo and r_lo + 8
+    const int r_lo = g * 64 * MS + wq * 16 + (lane >> 2);     // tile rows of this thread's fragment of sub-tile s: r_lo + 64s + {0, 8}
     const int cq = 2 * (lane & 3);                             // first of the thread's two columns in every 8-column group
     constexpr int R = BLOCK_N / 2;
-    float acc[R];
+    float acc[MS][R];
     float tot[SPLIT ? R : 1];
     double sq_acc = 0.0;
     int stage = 0; uint32_t phase = 0;
@@ -220,31 +245,35 @@ conv_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_co
       int prev_stage = -1;
       for (int k = 0; k < nk; ++k) {
         ptx::mbar_wait(&full_bar[stage], phase);
-        const uint32_t sa = ptx::smem_u32(smem + stage * C::kStageBytes) + (uint32_t)(g * 64 * 128);
-        const uint32_t sb = ptx::smem_u32(smem + stage * C::kStageBytes) + (uint32_t)kABytes;
+        const uint32_t sa = ptx::smem_u32(smem + stage * C::kStageBytes) + (uint32_t)(g * MS * 64 * 128);
+        const uint32_t sb = ptx::smem_u32(smem + stage * C::kStageBytes) + (uint32_t)C::kABytes;
         ptx::wgmma_fence();
 #pragma unroll
         for (int kk = 0; kk < kBlockK / kWgmmaK; ++kk) {
-          const uint64_t da = ptx::make_wgmma_desc_sw128(sa + kk * kWgmmaK * 4);
+          // sub-tile s: the warpgroup's rows 64s .. 64s+63, each its own accumulator through the same k8 sequence, one B read for all
+          uint64_t da[MS];
+#pragma unroll
+          for (int s = 0; s < MS; ++s) da[s] = ptx::make_wgmma_desc_sw128(sa + s * 64 * 128 + kk * kWgmmaK * 4);
           const uint64_t db = ptx::make_wgmma_desc_sw128(sb + kk * kWgmmaK * 4);
           if constexpr (SPLIT) {
             // split precision: this stage's x_hi*w_hi + x_lo*w_hi + x_hi*w_lo in a fresh accumulator, added to the running total with
             // round-to-nearest fp32 adds below (the tensor core truncates on every accumulate: over hundreds of K steps that, not the
             // operand split, would limit the "fp32-grade" layers)
-            constexpr uint32_t kLo = kABytes + C::kBBytes;
-            ptx::wgmma_tf32<BLOCK_N>(acc, da, db, kk != 0 ? 1u : 0u);
-            ptx::wgmma_tf32<BLOCK_N>(acc, ptx::make_wgmma_desc_sw128(sa + kLo + kk * kWgmmaK * 4), db, 1u);
-            ptx::wgmma_tf32<BLOCK_N>(acc, da, ptx::make_wgmma_desc_sw128(sb + kLo + kk * kWgmmaK * 4), 1u);
+            constexpr uint32_t kLo = C::kABytes + C::kBBytes;
+            ptx::wgmma_tf32<BLOCK_N>(acc[0], da[0], db, kk != 0 ? 1u : 0u);
+            ptx::wgmma_tf32<BLOCK_N>(acc[0], ptx::make_wgmma_desc_sw128(sa + kLo + kk * kWgmmaK * 4), db, 1u);
+            ptx::wgmma_tf32<BLOCK_N>(acc[0], da[0], ptx::make_wgmma_desc_sw128(sb + kLo + kk * kWgmmaK * 4), 1u);
           } else {
-            ptx::wgmma_tf32<BLOCK_N>(acc, da, db, (k | kk) != 0 ? 1u : 0u);
+#pragma unroll
+            for (int s = 0; s < MS; ++s) ptx::wgmma_tf32<BLOCK_N>(acc[s], da[s], db, (k | kk) != 0 ? 1u : 0u);
           }
         }
         ptx::wgmma_commit();
         if constexpr (SPLIT) {
           ptx::wgmma_wait<0>();
-          ptx::fence_regs(acc);
+          ptx::fence_regs(acc[0]);
 #pragma unroll
-          for (int i = 0; i < R; ++i) tot[i] += acc[i];
+          for (int i = 0; i < R; ++i) tot[i] += acc[0][i];
           if (lane == 0) ptx::mbar_arrive(&empty_bar[stage]);
         } else {
           ptx::wgmma_wait<1>();                                  // the previous stage's wgmmas are done: release its buffers
@@ -255,37 +284,40 @@ conv_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_co
       }
       if constexpr (!SPLIT) {
         ptx::wgmma_wait<0>();
-        ptx::fence_regs(acc);
+#pragma unroll
+        for (int s = 0; s < MS; ++s) ptx::fence_regs(acc[s]);
         if (prev_stage >= 0 && lane == 0) ptx::mbar_arrive(&empty_bar[prev_stage]);
       }
       if constexpr (SPLIT) {
 #pragma unroll
-        for (int i = 0; i < R; ++i) acc[i] = tot[i];
+        for (int i = 0; i < R; ++i) acc[0][i] = tot[i];
       }
-      float* v = acc;
 
       // ---- epilogue from the fragment ----
-      // the thread's two output rows (fragment rows r_lo and r_lo + 8); in[h] = false past the output
-      bool in[2];
-      float* yrow[2];
-      const float* rrow[2];
+      // the thread's two output rows of sub-tile s (fragment rows r_lo + 64s and r_lo + 64s + 8); in[s][h] = false past the output
+      bool in[MS][2];
+      float* yrow[MS][2];
+      const float* rrow[MS][2];
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int row = r_lo + 8 * h;
-        const int img = mt / tiles_per_img, rem = mt - img * tiles_per_img;
-        const int ty = rem / a.tiles_x, tx = rem - ty * a.tiles_x;
-        const int dy = row / a.BW, dx = row - dy * a.BW;
-        const int oy = ty * a.BH + dy, ox = tx * a.BW + dx;
-        in[h] = oy < a.OH && ox < a.OW;
-        yrow[h] = a.y + (size_t)sp * a.split_stride + (size_t)img * a.y_img + (size_t)oy * a.y_row + (size_t)ox * a.ldy;
-        rrow[h] = in[h] && a.residual ? a.residual + (((size_t)img * a.OH + oy) * a.OW + ox) * a.ldr : nullptr;
+      for (int s = 0; s < MS; ++s) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int row = r_lo + 64 * s + 8 * h;
+          const int img = mt / tiles_per_img, rem = mt - img * tiles_per_img;
+          const int ty = rem / a.tiles_x, tx = rem - ty * a.tiles_x;
+          const int dy = row / a.BW, dx = row - dy * a.BW;
+          const int oy = ty * a.BH + dy, ox = tx * a.BW + dx;
+          in[s][h] = oy < a.OH && ox < a.OW;
+          yrow[s][h] = a.y + (size_t)sp * a.split_stride + (size_t)img * a.y_img + (size_t)oy * a.y_row + (size_t)ox * a.ldy;
+          rrow[s][h] = in[s][h] && a.residual ? a.residual + (((size_t)img * a.OH + oy) * a.OW + ox) * a.ldr : nullptr;
+        }
       }
       // Pass 1: scale, shift and residual, each read in full at the thread's columns and then applied in place, before anything is
       // stored.  The output may alias what these read, so the compiler keeps every read after the stores that precede it: reads
       // interleaved with the stores wait one global-memory latency per column pair (a 1x1 convolution with a residual then runs at
       // a fraction of the DRAM rate), while a pass with no store in it has all its reads in flight at once.  __fmul_rn / __fadd_rn
       // keep the product and each sum separately rounded (no contraction into an FMA), in the order scale, shift, residual.
-      // Columns past Cout read nothing; their values are never stored.
+      // Columns past Cout read nothing; their values are never stored.  A per-channel operand is read once for both sub-tiles.
       const int c0 = nt * BLOCK_N + cq;
       float t[BLOCK_N / 4];                                      // one operand at the thread's columns c0 + 8j + {0, 1}
       auto gather = [&](const float* p) {
@@ -299,14 +331,19 @@ conv_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_co
       if (a.scale) {
         gather(a.scale);
 #pragma unroll
-        for (int i = 0; i < R; ++i) v[i] = __fmul_rn(v[i], t[(i >> 2) * 2 + (i & 1)]);
+        for (int s = 0; s < MS; ++s)
+#pragma unroll
+          for (int i = 0; i < R; ++i) acc[s][i] = __fmul_rn(acc[s][i], t[(i >> 2) * 2 + (i & 1)]);
       }
       if (a.shift) {
         gather(a.shift);
 #pragma unroll
-        for (int i = 0; i < R; ++i) v[i] = __fadd_rn(v[i], t[(i >> 2) * 2 + (i & 1)]);
+        for (int s = 0; s < MS; ++s)
+#pragma unroll
+          for (int i = 0; i < R; ++i) acc[s][i] = __fadd_rn(acc[s][i], t[(i >> 2) * 2 + (i & 1)]);
       }
       if constexpr (TMA_EPI) {
+        float* v = acc[0];
         // The residual and the output share the tile buffer: the thread reads the residual at its own fragment positions and writes
         // the finished values back to the same positions, so the two passes need no barrier between them.  Position of fragment row
         // rl and column c: box c / 32 of the warpgroup's half, row rl of 128 B, 16-byte chunk (c % 32) / 4 XOR rl % 8 (SWIZZLE_128B,
@@ -345,7 +382,7 @@ conv_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_co
             if (a.sumsq && c < a.Cout) part = fmaf(v0, v0, c + 1 < a.Cout ? fmaf(v1, v1, part) : part);
             *at(h, j) = make_float2(v0, v1);
           }
-          if (in[h]) sq_acc += (double)part;
+          if (in[0][h]) sq_acc += (double)part;
         }
         // one TMA store per 32-channel box of the warpgroup's 64 rows; the tensor map clips rows past P and channels past Cout
         ptx::fence_proxy_async();
@@ -360,39 +397,45 @@ conv_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_co
         if (++eb == C::kEpiBufs) { eb = 0; ephase ^= 1; }
       } else {
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          if (!rrow[h]) continue;
-          gather(rrow[h]);
+        for (int s = 0; s < MS; ++s) {
 #pragma unroll
-          for (int j = 0; j < BLOCK_N / 8; ++j) {
-            v[4 * j + 2 * h] = __fadd_rn(v[4 * j + 2 * h], t[2 * j]);
-            v[4 * j + 2 * h + 1] = __fadd_rn(v[4 * j + 2 * h + 1], t[2 * j + 1]);
+          for (int h = 0; h < 2; ++h) {
+            if (!rrow[s][h]) continue;
+            gather(rrow[s][h]);
+#pragma unroll
+            for (int j = 0; j < BLOCK_N / 8; ++j) {
+              acc[s][4 * j + 2 * h] = __fadd_rn(acc[s][4 * j + 2 * h], t[2 * j]);
+              acc[s][4 * j + 2 * h + 1] = __fadd_rn(acc[s][4 * j + 2 * h + 1], t[2 * j + 1]);
+            }
           }
         }
         // Pass 2: activation, rounding, sum of squares, stores
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          if (!in[h]) continue;
-          float part = 0.f;
+        for (int s = 0; s < MS; ++s) {
 #pragma unroll
-          for (int j = 0; j < BLOCK_N / 8; ++j) {
-            const int c = c0 + 8 * j;
-            if (c >= a.Cout) continue;
-            const bool two = c + 1 < a.Cout;
-            float v0 = v[4 * j + 2 * h], v1 = v[4 * j + 2 * h + 1];
-            v0 = epi_act(v0, a.act, a.slope); v1 = epi_act(v1, a.act, a.slope);
-            if (a.round_out) { v0 = ptx::round_tf32(v0); v1 = ptx::round_tf32(v1); }
-            if (a.sumsq) part = fmaf(v0, v0, two ? fmaf(v1, v1, part) : part);
-            if (a.no_store) continue;
-            float* y = yrow[h];
-            if (two && !((reinterpret_cast<uintptr_t>(y + c)) & 7)) {
-              *reinterpret_cast<float2*>(y + c) = make_float2(v0, v1);
-            } else {
-              y[c] = v0;
-              if (two) y[c + 1] = v1;
+          for (int h = 0; h < 2; ++h) {
+            if (!in[s][h]) continue;
+            float part = 0.f;
+#pragma unroll
+            for (int j = 0; j < BLOCK_N / 8; ++j) {
+              const int c = c0 + 8 * j;
+              if (c >= a.Cout) continue;
+              const bool two = c + 1 < a.Cout;
+              float v0 = acc[s][4 * j + 2 * h], v1 = acc[s][4 * j + 2 * h + 1];
+              v0 = epi_act(v0, a.act, a.slope); v1 = epi_act(v1, a.act, a.slope);
+              if (a.round_out) { v0 = ptx::round_tf32(v0); v1 = ptx::round_tf32(v1); }
+              if (a.sumsq) part = fmaf(v0, v0, two ? fmaf(v1, v1, part) : part);
+              if (a.no_store) continue;
+              float* y = yrow[s][h];
+              if (two && !((reinterpret_cast<uintptr_t>(y + c)) & 7)) {
+                *reinterpret_cast<float2*>(y + c) = make_float2(v0, v1);
+              } else {
+                y[c] = v0;
+                if (two) y[c + 1] = v1;
+              }
             }
+            sq_acc += (double)part;                             // fp32 within a row of the tile, fp64 across rows and tiles
           }
-          sq_acc += (double)part;                               // fp32 within a row of the tile, fp64 across rows and tiles
         }
       }
     }
@@ -432,6 +475,7 @@ int g_conv_im2col = 1;
 int g_tile_order = 0;             // 0 front-to-back, 1 back-to-front, 2 alternate per launch
 int g_tile_flip = 0;
 int g_k_order = 0;                // 0: by working set (channel chunks outermost when Cin >= 2048); 1: taps outermost; 2: chunks outermost
+int g_tile_m = 0;                 // 0: 256-row tiles by the launch's shape; 1: always 128; 2: 256 wherever the 256-row path can run
 
 EncodeTiledFn get_encode_tiled() {
   static EncodeTiledFn fn = nullptr;
@@ -478,30 +522,31 @@ void pick_rect(int OH, int OW, int stride, int* BH, int* BW) {
   }
 }
 
-template <int BLOCK_N, bool SPLIT, bool TMA_EPI>
+template <int BLOCK_M, int BLOCK_N, bool SPLIT, bool TMA_EPI>
 int launch(const CUtensorMap& tx, const CUtensorMap& tw, const CUtensorMap& tx2, const CUtensorMap& tw2, const CUtensorMap& tr,
            const CUtensorMap& ty, const ConvArgs& a_in, cudaStream_t st) {
-  using C = Cfg<BLOCK_N, SPLIT, TMA_EPI>;
+  using C = Cfg<BLOCK_M, BLOCK_N, SPLIT, TMA_EPI>;
   ConvArgs a = a_in;
   a.nstages = C::kStages;
   static bool attr = false;
   if (!attr) {
-    cudaError_t e = cudaFuncSetAttribute(conv_fwd_sm90_kernel<BLOCK_N, SPLIT, TMA_EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::kSmemBytes);
+    cudaError_t e = cudaFuncSetAttribute(conv_fwd_sm90_kernel<BLOCK_M, BLOCK_N, SPLIT, TMA_EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         C::kSmemBytes);
     if (e != cudaSuccess) { set_error("skd_conv2d_fwd_sm100(attr)", e); return 0; }
     attr = true;
   }
   int grid = a.m_tiles * a.n_tiles * a.splits;
   if (grid > kNumSMs) grid = kNumSMs;
-  conv_fwd_sm90_kernel<BLOCK_N, SPLIT, TMA_EPI><<<grid, kThreads, C::kSmemBytes, st>>>(tx, tw, tx2, tw2, tr, ty, a);
+  conv_fwd_sm90_kernel<BLOCK_M, BLOCK_N, SPLIT, TMA_EPI><<<grid, kThreads, C::kSmemBytes, st>>>(tx, tw, tx2, tw2, tr, ty, a);
   return finish("skd_conv2d_fwd_sm100");
 }
 
 template <int BLOCK_N>
 int launch_n(bool split3, bool tma_epi, const CUtensorMap& tx, const CUtensorMap& tw, const CUtensorMap& tx2, const CUtensorMap& tw2,
              const CUtensorMap& tr, const CUtensorMap& ty, const ConvArgs& a, cudaStream_t st) {
-  if (split3) return launch<BLOCK_N, true, false>(tx, tw, tx2, tw2, tr, ty, a, st);
-  if (tma_epi) return launch<BLOCK_N, false, true>(tx, tw, tx2, tw2, tr, ty, a, st);
-  return launch<BLOCK_N, false, false>(tx, tw, tx2, tw2, tr, ty, a, st);
+  if (split3) return launch<kBlockM, BLOCK_N, true, false>(tx, tw, tx2, tw2, tr, ty, a, st);
+  if (tma_epi) return launch<kBlockM, BLOCK_N, false, true>(tx, tw, tx2, tw2, tr, ty, a, st);
+  return launch<kBlockM, BLOCK_N, false, false>(tx, tw, tx2, tw2, tr, ty, a, st);
 }
 
 }  // namespace
@@ -509,6 +554,7 @@ int launch_n(bool split3, bool tma_epi, const CUtensorMap& tx, const CUtensorMap
 extern "C" void skd_set_conv_im2col(int on) { g_conv_im2col = on ? 1 : 0; }
 extern "C" void skd_set_conv_tile_order(int mode) { g_tile_order = mode; g_tile_flip = 0; }
 extern "C" void skd_set_conv_k_order(int mode) { g_k_order = mode; }
+extern "C" void skd_set_conv_tile_m(int mode) { g_tile_m = mode; }
 
 // ---- split-K for convolutions with few output tiles and a long K loop (the discriminator: 256 .. 4096 output pixels, K up to 4096) ----
 // Without it a 4x8-pixel map at batch 8 is 2 x 2 tiles: 4 of 132 SMs walk 128 K steps each.  Units = tiles x K ranges fill the
@@ -661,13 +707,26 @@ static int conv_fwd_impl(int N, int H, int W, int Cin, int Cout, int KH, int KW,
     };
     if (!encode_rows(&ty, y, ldy) || !encode_rows(&tr, residual, ldr)) return 0;
   }
+  // 256-row tiles (two 128-row A boxes per stage, same maps) for the long-K launches, where a 128x128 tile is bound by the operand
+  // bytes per FLOP rather than by the tensor cores: K loops of at least kTile256MinK steps and more than one N tile (DESIGN.md §6:
+  // the 1x1 convolutions, K = 32 / 64, and the 3x3 256-channel ones, K = 72, lose with half the stages and twice the epilogue per
+  // tile; a lone N tile lost as well).  And only where halving the work-unit count adds no ragged wave of 132 CTAs: a 256-row unit
+  // takes two 128-row unit times.
+  const bool tile256_legal = (flat || a.im2col) && bn == 128 && !split3 && a.splits == 1 && !tma_epi && !sumsq && !no_store;
+  const long long units128 = (long long)a.m_tiles * a.n_tiles, units256 = (P + 2 * kBlockM - 1) / (2 * kBlockM) * a.n_tiles;
+  const bool tile256 = tile256_legal && g_tile_m != 1 &&
+                       (g_tile_m == 2 || (KH * KW * a.k_chunks >= kTile256MinK && a.n_tiles > 1 &&
+                                          2 * ((units256 + kNumSMs - 1) / kNumSMs) <= (units128 + kNumSMs - 1) / kNumSMs));
+  if (tile256) { a.BW = 2 * kBlockM; a.tiles_x = (a.OW + a.BW - 1) / a.BW; a.m_tiles = a.tiles_x; }
   a.kc_outer = kc_outer;
   a.reverse = (g_tile_order == 2) ? (g_tile_flip ^= 1) : g_tile_order;
   a.nstages = 0; a.sumsq = sumsq; a.no_store = no_store;
   if (strided_out && residual) { set_error_msg(who, "strided output takes no residual"); return 0; }
   int ok;
   switch (bn) {
-    case 128: ok = launch_n<128>(split3, tma_epi, tx, tw, tx2, tw2, tr, ty, a, st); break;
+    case 128:
+      ok = tile256 ? launch<2 * kBlockM, 128, false, false>(tx, tw, tx2, tw2, tr, ty, a, st) : launch_n<128>(split3, tma_epi, tx, tw, tx2, tw2, tr, ty, a, st);
+      break;
     case 64: ok = launch_n<64>(split3, tma_epi, tx, tw, tx2, tw2, tr, ty, a, st); break;
     default: ok = launch_n<32>(split3, tma_epi, tx, tw, tx2, tw2, tr, ty, a, st); break;
   }

@@ -86,6 +86,14 @@ __device__ __forceinline__ void bulk_wait_group() { asm volatile("cp.async.bulk.
 
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory"); }
 
+// ---- per-warpgroup register budget ----------------------------------------------------------------
+// Every thread of the warpgroup executes it.  dec hands registers above N back to the CTA's pool; inc waits until the pool holds
+// enough to raise every thread of the warpgroup to N.  N is a multiple of 8 in [24, 256].
+template <uint32_t N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+template <uint32_t N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+
 // ---- wgmma (warpgroup MMA, accumulator in registers) --------------------------------------------------
 // Shared-memory matrix descriptor (sm_90 GMMA): start>>4 [0,14) | LBO>>4 [16,30) | SBO>>4 [32,46) | layout [62,64) (1 = SWIZZLE_128B).
 // K-major operands only for tf32: rows of 128 B (32 fp32 of K), 8-row groups SBO = 1024 B apart; the K step of one wgmma (8 tf32 =
