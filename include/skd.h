@@ -429,6 +429,35 @@ int skd_resample_bilinear_nhwc(int N, int C, int h, int w, const float* src, lon
    discriminator input is its logits resized onto the teacher's grid; this is the gradient of that resize. */
 int skd_resample_bilinear_adjoint_nhwc(int N, int C, int h, int w, const float* dout, int H, int W, float* dsrc, int lds, cudaStream_t);
 
+/* ---- I. MobileNetV2 student (networks/mobilenet.py, csrc/mobilenet.cu).  fp32 NHWC, C a multiple of 4, rows 16-byte aligned.
+        Fixed-order reductions (double partials, no atomics): two runs give bit-identical results. ---- */
+/* workspace of the reductions below over P rows (the depthwise forward statistics and weight gradient: P = N * OH * OW) of C channels */
+long long skd_mbv2_workspace_doubles(long long P, int C);
+/* replaces nn.Conv2d(C, C, 3, stride, padding=dilation, dilation, groups=C, bias=False) forward: x dense [N][H][W][C], weight the
+   (C, 1, 3, 3) parameter, y dense [N][OH][OW][C] with OH = (H - 1) / stride + 1.  stride 1 or 2.  When mean != NULL, the following
+   BatchNorm2d's training statistics of y are formed in the same pass (as skd_bnprelu_stats: running statistics and counter may be NULL) */
+int skd_dwconv3x3_fwd(int N, int H, int W, int C, int stride, int dilation, const float* x, const float* weight, float* y, float momentum,
+                      float* running_mean, float* running_var, long long* num_batches_tracked, float* mean, float* var, double* workspace,
+                      cudaStream_t);
+/* its data gradient dx [N][H][W][C] from dy [N][OH][OW][C]: a gather, one thread per input element group, no atomics */
+int skd_dwconv3x3_dgrad(int N, int H, int W, int C, int stride, int dilation, const float* dy, const float* weight, float* dx, cudaStream_t);
+/* its weight gradient dweight (C, 1, 3, 3) = sum over output pixels of dy * x at each tap: per-block partials in the workspace, then
+   one fixed-order reduction */
+int skd_dwconv3x3_wgrad(int N, int H, int W, int C, int stride, int dilation, const float* x, const float* dy, float* dweight,
+                        double* workspace, cudaStream_t);
+/* BatchNorm2d (mean / var as skd_bnprelu_stats gives them, or the running statistics) followed by ReLU6 (relu6 = 1: clamp to [0, 6]) or
+   by nothing (relu6 = 0), plus residual (may be NULL; linear mode only): out = z + residual, the projection of an inverted residual */
+int skd_bnact_apply(long long P, int C, int relu6, const float* x, int ldx, const float* mean, const float* var, const float* weight,
+                    const float* bias, float eps, const float* residual, int ldr, float* out, int ldo, cudaStream_t);
+/* backward reduce pass: dweight = sum dz * xhat, dbias = sum dz (each may be NULL), dz = dout where 0 < z < 6 (ReLU6; z recomputed from
+   x) or dout (linear); coef[2C] = (mean dz, mean dz * xhat) for the dx pass.  The residual's gradient is dout itself. */
+int skd_bnact_bwd_reduce(long long P, int C, int relu6, const float* x, int ldx, const float* dout, int ldd, const float* mean,
+                         const float* var, const float* weight, const float* bias, float eps, float* dweight, float* dbias, float* coef,
+                         double* workspace, cudaStream_t);
+/* dx pass: w * rsqrt(var + eps) * (dz - coef[c] - xhat * coef[C + c]) (training) or w * rsqrt(var + eps) * dz (running statistics) */
+int skd_bnact_bwd_dx(long long P, int C, int relu6, const float* x, int ldx, const float* dout, int ldd, const float* mean, const float* var,
+                     const float* weight, const float* bias, float eps, int training, const float* coef, float* dx, int lddx, cudaStream_t);
+
 #ifdef __cplusplus
 }
 #endif

@@ -577,6 +577,63 @@ class EspConcat(torch.autograd.Function):
         return tuple(out)
 
 
+# ------------------------------------------------------------------------------------------------ MobileNetV2 (networks/mobilenet.py)
+# Activations are dense NHWC tensors (every MobileNetV2 width is a multiple of 8).  The 1x1 expand / project convolutions and the stem
+# are Conv2d above; these two Functions are the rest of an inverted residual.  Saved for backward: each BatchNorm's input (z is
+# recomputed from it for the ReLU6 mask, never stored) and each convolution's input, i.e. the activated expansion is stored, not
+# recomputed (DESIGN.md "MobileNetV2 student" has the memory this takes).
+class MbBnAct(torch.autograd.Function):
+    """nn.BatchNorm2d followed by nn.ReLU6 (`relu6`: the stem and the 1x1 expansions), or the linear BatchNorm of an inverted
+    residual's projection plus, when the block has one, its input (`residual`: x + bn(conv(x)))."""
+
+    @staticmethod
+    def forward(ctx, x, weight, bias, running_mean, running_var, nbt, training, momentum, eps, relu6, residual):
+        st = _bn_stats(x, training, momentum, running_mean, running_var, nbt)
+        y = ops.bnact_apply(x, st[0], st[1], weight, bias, eps, relu6, residual)
+        ctx.save_for_backward(x, st, weight, bias)
+        ctx.cfg = (training, eps, relu6, residual is not None)
+        return y
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, dy):
+        x, st, weight, bias = ctx.saved_tensors
+        training, eps, relu6, has_res = ctx.cfg
+        dy = ops.dense_nhwc(dy)
+        dw, db, coef = ops.bnact_bwd_reduce(x, dy, st[0], st[1], weight, bias, eps, relu6)
+        dx = ops.bnact_bwd_dx(x, dy, st[0], st[1], weight, bias, eps, relu6, training, coef)
+        dres = dy if has_res and ctx.needs_input_grad[10] else None
+        return dx, dw, db, None, None, None, None, None, None, None, dres
+
+
+class MbDwBnRelu6(torch.autograd.Function):
+    """Depthwise 3x3 convolution (stride 1 or 2, padding = dilation) -> BatchNorm2d -> ReLU6 of an inverted residual.  In training
+    the convolution's pass also forms the BatchNorm's batch statistics, so its output is not read a second time for them."""
+
+    @staticmethod
+    def forward(ctx, x, w_dw, weight, bias, running_mean, running_var, nbt, stride, dilation, training, momentum, eps):
+        x = ops.dense_nhwc(x)
+        t, st = ops.dwconv3x3_fwd(x, w_dw, stride, dilation, training, momentum, running_mean, running_var, nbt)
+        if not training:
+            st = torch.stack([running_mean, running_var])
+        y = ops.bnact_apply(t, st[0], st[1], weight, bias, eps, True)
+        ctx.save_for_backward(x, t, st, w_dw, weight, bias)
+        ctx.cfg = (stride, dilation, training, eps)
+        return y
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, dy):
+        x, t, st, w_dw, weight, bias = ctx.saved_tensors
+        stride, dilation, training, eps = ctx.cfg
+        dy = ops.dense_nhwc(dy)
+        dbw, dbb, coef = ops.bnact_bwd_reduce(t, dy, st[0], st[1], weight, bias, eps, True)
+        dt = ops.bnact_bwd_dx(t, dy, st[0], st[1], weight, bias, eps, True, training, coef)
+        dx = ops.dwconv3x3_dgrad(dt, w_dw, tuple(x.shape), stride, dilation) if ctx.needs_input_grad[0] else None
+        dwd = ops.dwconv3x3_wgrad(x, dt, stride, dilation) if ctx.needs_input_grad[1] else None
+        return (dx, dwd, dbw, dbb) + (None,) * 8
+
+
 class ResampleBilinear(torch.autograd.Function):
     """F.interpolate(t, (H, W), mode='bilinear', align_corners=True) with a gradient: the forward is the teacher resample kernel, the
     backward its adjoint as a fixed-order gather (no float atomics, so two runs of a step stay bit-identical).  The full ESPNet's

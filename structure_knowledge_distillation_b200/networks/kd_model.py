@@ -29,6 +29,7 @@ from ..utils.criterion import (CriterionAdditionalGP, CriterionAdv, CriterionAdv
 from ..utils.utils import load_D_model, load_S_model, load_T_model
 from .espnet import ESPNet, ESPNet_C
 from .evaluate import evaluate_main
+from .mobilenet import MobileNetV2
 from .pspnet_combine import BasicBlock, Bottleneck, Res_pspnet
 from .sagan_models import Discriminator
 
@@ -78,8 +79,12 @@ class NetModel():
                 raise ValueError("sync_bn is not available with the ESPNet students (their BatchNorm statistics are per rank)")
             student = (ESPNet_C if self.student_kind == "espnet_c" else ESPNet)(args.classes_num, _arg(args, "espnet_p", 2),
                                                                                _arg(args, "espnet_q", 8))
+        elif self.student_kind == "mobilenetv2":
+            if _arg(args, "sync_bn", False):
+                raise ValueError("sync_bn is not available with the MobileNetV2 student (its BatchNorm statistics are per rank)")
+            student = MobileNetV2(args.classes_num)
         else:
-            raise ValueError("student must be 'resnet18', 'espnet_c' or 'espnet' (got %r)" % self.student_kind)
+            raise ValueError("student must be 'resnet18', 'espnet_c', 'espnet' or 'mobilenetv2' (got %r)" % self.student_kind)
         load_S_model(args, student, False)                         # ImageNet init or S_resume (utils/utils.py:93-127)
         self.student = student.float().to(device).train()
         if _arg(args, "sync_bn", False):                          # cross-rank batch statistics (the reference's InPlaceABNSync semantics)
@@ -125,7 +130,7 @@ class NetModel():
         if _arg(args, "ohem", False):                             # OHEM task loss (the reference imports CriterionOhemDSN, kd_model.py:18)
             # (ESPNet-C: head 0 only, preds[1] is None)
             self.criterion = CriterionOhemDSN(thresh=_arg(args, "ohem_thres", 0.7), min_kept=_arg(args, "ohem_keep", 100000))
-        elif self.student_kind != "resnet18":                     # the ESPNets: no auxiliary head, single-head cross entropy
+        elif self.student_kind in ("espnet_c", "espnet"):         # the ESPNets: no auxiliary head, single-head cross entropy
             self.criterion = CriterionCrossEntropy()
         else:
             self.criterion = CriterionDSN()
@@ -266,7 +271,7 @@ class NetModel():
             # the ONE collective of the path (teacher frozen): bucketed NCCL all-reduce of the flat student gradient, issued from
             # inside the backward pass as each range of parameters completes (utils/parallel.py:54-63,155 semantics: mean over ranks)
             self.G_solver.begin_overlapped_reduce(self.world)
-        if self.overlap_streams and self.student_kind == "resnet18":
+        if self.overlap_streams and self.student_kind in ("resnet18", "mobilenetv2"):
             # (ESPNet-C issues its weight gradients on the main stream: no side-stream window, so no join on an idle stream, which
             # a CUDA-graph capture would reject)
             Fn.WgradOverlap.begin()

@@ -736,6 +736,98 @@ def resample_nhwc(t, h, w):
     return out.permute(0, 3, 1, 2)
 
 
+# ------------------------------------------------------------------------------------------------ MobileNetV2 (csrc/mobilenet.cu)
+def dwconv_check(channels, weight_shape, stride, dilation):
+    """ValueError unless the depthwise shape is one the kernels run: a (C, 1, 3, 3) weight, C a multiple of 4, stride 1 or 2,
+    dilation >= 1 (padding = dilation)."""
+    if tuple(weight_shape) != (channels, 1, 3, 3):
+        raise ValueError("depthwise conv: weight must be (C, 1, 3, 3) = (%d, 1, 3, 3), got %s" % (channels, tuple(weight_shape)))
+    if channels % 4:
+        raise ValueError("depthwise conv: C must be a multiple of 4 (got %d)" % channels)
+    if stride not in (1, 2) or int(dilation) < 1:
+        raise ValueError("depthwise conv: stride must be 1 or 2 and dilation >= 1 (got stride %r, dilation %r)" % (stride, dilation))
+
+
+def dense_nhwc(t):
+    t = to_nhwc(t)
+    if nhwc_meta(t)[4] != t.shape[1]:
+        t = t.contiguous(memory_format=torch.channels_last)
+    return t
+
+
+def _mbv2_ws(P, c, device):
+    return torch.empty(max(int(lib().skd_mbv2_workspace_doubles(P, c)), 1), device=device, dtype=torch.float64)
+
+
+def dwconv3x3_fwd(x, weight, stride, dilation, stats=False, momentum=0.0, running_mean=None, running_var=None, num_batches_tracked=None):
+    """Depthwise 3x3 convolution (padding = dilation) of an (N, C, H, W) tensor -> (dense NHWC output, its (2, C) batch statistics or
+    None).  With `stats` the BatchNorm that follows gets its mean / biased variance (and its running statistics) from the same pass."""
+    n, c, h, w = x.shape
+    dwconv_check(c, weight.shape, stride, dilation)
+    _f32(x, weight)
+    x = dense_nhwc(x)
+    oh, ow = (h - 1) // stride + 1, (w - 1) // stride + 1
+    y = empty_nhwc(n, c, oh, ow, x.device)
+    st = torch.empty(2, c, device=x.device) if stats else None
+    ws = _mbv2_ws(n * oh * ow, c, x.device) if stats else None
+    lib().skd_dwconv3x3_fwd(n, h, w, c, stride, int(dilation), _p(x), _p(weight.contiguous()), _p(y), momentum, _p(running_mean),
+                            _p(running_var), _p(num_batches_tracked), _p(st[0]) if stats else None, _p(st[1]) if stats else None,
+                            _p(ws), _st())
+    return y, st
+
+
+def dwconv3x3_dgrad(dy, weight, x_shape, stride, dilation):
+    n, c, h, w = x_shape
+    dwconv_check(c, weight.shape, stride, dilation)
+    _f32(dy, weight)
+    dy = dense_nhwc(dy)
+    dx = empty_nhwc(n, c, h, w, dy.device)
+    lib().skd_dwconv3x3_dgrad(n, h, w, c, stride, int(dilation), _p(dy), _p(weight.contiguous()), _p(dx), _st())
+    return dx
+
+
+def dwconv3x3_wgrad(x, dy, stride, dilation):
+    """-> the (C, 1, 3, 3) weight gradient (fixed-order reduction over every output pixel)."""
+    n, c, h, w = x.shape
+    dwconv_check(c, (c, 1, 3, 3), stride, dilation)
+    _f32(x, dy)
+    x, dy = dense_nhwc(x), dense_nhwc(dy)
+    dw = torch.empty((c, 1, 3, 3), device=x.device, dtype=torch.float32)
+    ws = _mbv2_ws(n * dy.shape[2] * dy.shape[3], c, x.device)
+    lib().skd_dwconv3x3_wgrad(n, h, w, c, stride, int(dilation), _p(x), _p(dy), _p(dw), _p(ws), _st())
+    return dw
+
+
+def bnact_apply(x, mean, var, weight, bias, eps, relu6, residual=None):
+    """relu6(bn(x)) (relu6=True) or bn(x) + residual (relu6=False; residual may be None) -> fresh dense NHWC tensor."""
+    _f32(x, residual)
+    P, c, ldx = _rows(x)
+    out = empty_nhwc(x.shape[0], c, x.shape[2], x.shape[3], x.device)
+    ldr = _rows(residual)[2] if residual is not None else 0
+    lib().skd_bnact_apply(P, c, int(relu6), _p(x), ldx, _p(mean), _p(var), _p(weight), _p(bias), eps, _p(residual), ldr, _p(out), c,
+                          _st())
+    return out
+
+
+def bnact_bwd_reduce(x, dout, mean, var, weight, bias, eps, relu6):
+    """-> (dweight, dbias) and the (2, C) coefficients of the dx pass."""
+    P, c, ldx = _rows(x)
+    ldd = _rows(dout)[2]
+    red = torch.empty(4, c, device=x.device)             # dweight, dbias, mean dz, mean dz*xhat
+    lib().skd_bnact_bwd_reduce(P, c, int(relu6), _p(x), ldx, _p(dout), ldd, _p(mean), _p(var), _p(weight), _p(bias), eps, _p(red[0]),
+                               _p(red[1]), _p(red[2]), _p(_mbv2_ws(P, c, x.device)), _st())
+    return red[0], red[1], red[2:4]
+
+
+def bnact_bwd_dx(x, dout, mean, var, weight, bias, eps, relu6, training, coef):
+    P, c, ldx = _rows(x)
+    ldd = _rows(dout)[2]
+    dx = empty_nhwc(x.shape[0], c, x.shape[2], x.shape[3], x.device)
+    lib().skd_bnact_bwd_dx(P, c, int(relu6), _p(x), ldx, _p(dout), ldd, _p(mean), _p(var), _p(weight), _p(bias), eps, int(training),
+                           _p(coef), _p(dx), c, _st())
+    return dx
+
+
 def sgd_step_nvls(lo, hi, param_mc, grad_mc, param_local, buf, lr_dev, momentum, weight_decay, grad_scale):
     """data-parallel SGD over NVSwitch multicast on the owned range [lo, hi): see include/skd.h skd_sgd_step_nvls"""
     lib().skd_sgd_step_nvls(int(lo), int(hi), int(param_mc), int(grad_mc), _p(param_local), _p(buf), _p(lr_dev), momentum, weight_decay,
