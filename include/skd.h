@@ -295,8 +295,10 @@ int skd_bn2d_jacobian(int N, int C, int HW, const float* x, long long sn, long l
 int skd_bn2d_param_grad(int C, long long P, const float* rstd, const float* sums_g, const float* sums_t, const float* sums_v, float* dgamma,
                         float* dbeta, int accumulate, cudaStream_t);
 /* Self_Attn core (sagan_models.py:31-40): A = softmax(Q K^T) (no 1/sqrt(d)), O = A V, y = gamma O + x.
-   qkv [B*n][ldq] = [q(d) | k(d) | v(C)] (the three 1x1 convolutions as one GEMM), x / o / y [B*n][C], attn [B][n][n]; n <= 128, d <= 64 */
+   qkv [B*n][ldq] = [q(d) | k(d) | v(C)] (the three 1x1 convolutions as one GEMM), x / o / y [B*n][C], attn [B][n][n]; n <= 1024, d <= 64.
+   n <= 128 runs whole n x n tiles per CTA; n > 128 runs stripes of query rows with keys / values streamed in tiles. */
 void skd_set_attn_tensor_cores(int on);   /* 1 (default): the attention products on mma.sync TF32 in split precision; 0: SIMT fp32 (cross-check) */
+void skd_set_attn_tiled(int force);       /* 1: the row-stripe kernels for every n (cross-checks and timing at n <= 128); 0 (default): only for n > 128 */
 int skd_attn_fwd(int B, int n, int C, int d, const float* qkv, int ldq, const float* x, const float* gamma, float* attn, float* o, float* y,
                  float* y_lo, cudaStream_t);
 /* forward-mode tangent along (tqkv, tx): dattn = Adot, to = Odot, ty = gamma Odot + tx */

@@ -81,7 +81,7 @@ __device__ __forceinline__ void block_gemm(int M, int N, int K, FA a, FB b, FS s
 
 // The same product on the tensor cores: mma.sync m16n8k8 TF32 in split precision (a_lo*b_hi + a_hi*b_lo + a_hi*b_hi, fp32-grade like
 // the 3xTF32 convolutions), operands through the same shared-memory accessors.  Warp tiles of 16 x 8*NT, eight warps round-robin.
-// The attention products are 32..128 positions wide (n x n x d scores, n x C x n values): far below one wgmma tile pipeline's
+// The attention products are 32..1024 positions wide (n x n x d scores, n x C x n values): far below one wgmma tile pipeline's
 // start-up cost, so the warp-level MMA is the tensor-core path that fits them.
 __device__ __forceinline__ void mma_m16n8k8_tf32(float (&c)[4], const uint32_t (&a)[4], const uint32_t (&b)[2]) {
   asm volatile("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
@@ -977,21 +977,406 @@ attn_bwd2_kernel(int B, int n, int d, int nsl, const float* __restrict__ qkv, co
   }
 }
 
+// --------------------------------------------------------------------------------------------------------------------
+// Row-stripe attention for n > 128 (and for every n under skd_set_attn_tiled(1)).  The kernels above hold whole n x n tiles
+// in shared memory; these hold stripes of R query rows ([R][n+1] each, R = 16 or 8) and stream K / Kdot / V / Vdot through
+// 64-row tiles, so shared memory grows with n, not n^2.  Products accumulate tile by tile into shared memory (each output
+// element is owned by one thread of one attn_gemm call, and every call is fenced by __syncthreads), in a fixed order.
+// --------------------------------------------------------------------------------------------------------------------
+constexpr int kAttnTiledMaxN = 1024, kAttnKeyTile = 64, kAttnKeyRows = 32;
+
+// softmax over each of `rows` rows of s[rows][ld], `cols` entries each (warp per row)
+__device__ __forceinline__ void softmax_stripe(float* s, int rows, int cols, int ld) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
+  for (int i = warp; i < rows; i += nw) {
+    float* row = s + i * ld;
+    float m = -INFINITY;
+    for (int j = lane; j < cols; j += 32) m = fmaxf(m, row[j]);
+    m = warp_max(m);
+    float sum = 0.f;
+    for (int j = lane; j < cols; j += 32) { const float e = __expf(row[j] - m); row[j] = e; sum += e; }
+    sum = warp_sum(sum);
+    const float inv = 1.f / sum;
+    for (int j = lane; j < cols; j += 32) row[j] *= inv;
+  }
+}
+
+__device__ __forceinline__ void zero_smem(float* p, int len) {
+  for (int i = threadIdx.x; i < len; i += blockDim.x) p[i] = 0.f;
+}
+
+// grid (B, n / R, C / 64): S stripe = Q_rows K^T (K in 64-row tiles), row softmax, A stripe out, O = A V (V in 64-row tiles)
+__global__ void __launch_bounds__(256)
+attn_fwd_tiled_kernel(int n, int C, int d, int R, const float* __restrict__ qkv, int ldq, const float* __restrict__ x,
+                      const float* __restrict__ gamma, float* __restrict__ attn, float* __restrict__ o, float* __restrict__ y,
+                      float* __restrict__ y_lo, int tc) {
+  extern __shared__ float smem[];
+  const int b = blockIdx.x, i0 = blockIdx.y * R, sl = blockIdx.z;
+  const int rr = min(R, n - i0), ldS = n + 1, ldD = d + 1, ldV = kAttnFwdSlice + 1, KT = kAttnKeyTile;
+  float* sS = smem;                       // [R][n+1]  scores, then A
+  float* sQ = sS + R * ldS;               // [R][d+1]
+  float* sO = sQ + R * ldD;               // [R][65]   O accumulator
+  float* sT = sO + R * ldV;               // [64][65]  a K tile, later a V tile
+  const float* base = qkv + (size_t)b * n * ldq;
+  load_rows(sQ, ldD, base + (size_t)i0 * ldq, ldq, rr, d);
+  zero_smem(sO, R * ldV);
+  for (int j0 = 0; j0 < n; j0 += KT) {
+    const int jw = min(KT, n - j0);
+    __syncthreads();
+    load_rows(sT, ldD, base + (size_t)j0 * ldq + d, ldq, jw, d);
+    __syncthreads();
+    attn_gemm<1, 4>(tc, rr, jw, d, [&](int i, int k) { return sQ[i * ldD + k]; }, [&](int k, int j) { return sT[j * ldD + k]; },
+                     [&](int i, int j, float v) { sS[i * ldS + j0 + j] = v; });
+  }
+  __syncthreads();
+  softmax_stripe(sS, rr, n, ldS);
+  __syncthreads();
+  if (sl == 0 && attn)
+    for (int t = threadIdx.x; t < rr * n; t += 256) attn[((size_t)b * n + i0) * n + t] = sS[(t / n) * ldS + t % n];
+  const int c0 = sl * kAttnFwdSlice, cw = min(kAttnFwdSlice, C - c0);
+  for (int j0 = 0; j0 < n; j0 += KT) {
+    const int jw = min(KT, n - j0);
+    __syncthreads();
+    load_rows(sT, ldV, base + (size_t)j0 * ldq + 2 * d + c0, ldq, jw, cw);
+    __syncthreads();
+    attn_gemm<1, 4>(tc, rr, cw, jw, [&](int i, int k) { return sS[i * ldS + j0 + k]; }, [&](int k, int c) { return sT[k * ldV + c]; },
+                     [&](int i, int c, float v) { sO[i * ldV + c] += v; });
+  }
+  __syncthreads();
+  const float gm = gamma[0];
+  for (int t = threadIdx.x; t < rr * cw; t += 256) {
+    const int i = t / cw, c = t - i * cw;
+    const size_t idx = ((size_t)b * n + i0 + i) * C + c0 + c;
+    const float v = sO[i * ldV + c];
+    if (o) o[idx] = v;
+    const float yy = fmaf(gm, v, __ldg(x + idx));
+    y[idx] = yy;
+    if (y_lo) y_lo[idx] = lo_part(yy);
+  }
+}
+
+// grid (B, n / R, C / 64): Sdot stripe = Qdot K^T + Q Kdot^T, Adot = A (Sdot - rowsum(A Sdot)), Odot = Adot V + A Vdot
+__global__ void __launch_bounds__(256)
+attn_tangent_tiled_kernel(int n, int C, int d, int R, const float* __restrict__ qkv, const float* __restrict__ tqkv, int ldq,
+                          const float* __restrict__ attn, const float* __restrict__ tx, const float* __restrict__ gamma,
+                          float* __restrict__ dattn, float* __restrict__ to, float* __restrict__ ty, float* __restrict__ ty_lo, int tc) {
+  extern __shared__ float smem[];
+  const int b = blockIdx.x, i0 = blockIdx.y * R, sl = blockIdx.z;
+  const int rr = min(R, n - i0), ldS = n + 1, ldD = d + 1, ldV = kAttnFwdSlice + 1, KT = kAttnKeyTile;
+  float* sA = smem;                       // [R][n+1]
+  float* sdA = sA + R * ldS;              // [R][n+1]  Sdot, then Adot
+  float* sQ = sdA + R * ldS;              // [R][d+1]
+  float* sTQ = sQ + R * ldD;              // [R][d+1]
+  float* sO = sTQ + R * ldD;              // [R][65]   Odot accumulator
+  float* sT = sO + R * ldV;               // 2 x [64][65]: K | Kdot tiles, later V | Vdot tiles
+  float* sT2 = sT + KT * ldV;
+  const float* base = qkv + (size_t)b * n * ldq;
+  const float* tbase = tqkv + (size_t)b * n * ldq;
+  load_rows(sA, ldS, attn + ((size_t)b * n + i0) * n, n, rr, n);
+  load_rows(sQ, ldD, base + (size_t)i0 * ldq, ldq, rr, d);
+  load_rows(sTQ, ldD, tbase + (size_t)i0 * ldq, ldq, rr, d);
+  zero_smem(sO, R * ldV);
+  for (int j0 = 0; j0 < n; j0 += KT) {
+    const int jw = min(KT, n - j0);
+    __syncthreads();
+    load_rows(sT, ldD, base + (size_t)j0 * ldq + d, ldq, jw, d);
+    load_rows(sT2, ldD, tbase + (size_t)j0 * ldq + d, ldq, jw, d);
+    __syncthreads();
+    attn_gemm<1, 4>(tc, rr, jw, 2 * d,
+                     [&](int i, int k) { return k < d ? sTQ[i * ldD + k] : sQ[i * ldD + k - d]; },
+                     [&](int k, int j) { return k < d ? sT[j * ldD + k] : sT2[j * ldD + k - d]; },
+                     [&](int i, int j, float v) { sdA[i * ldS + j0 + j] = v; });
+  }
+  __syncthreads();
+  {
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    for (int i = warp; i < rr; i += 8) {
+      float r = 0.f;
+      for (int j = lane; j < n; j += 32) r = fmaf(sA[i * ldS + j], sdA[i * ldS + j], r);
+      r = warp_sum(r);
+      for (int j = lane; j < n; j += 32) sdA[i * ldS + j] = sA[i * ldS + j] * (sdA[i * ldS + j] - r);
+    }
+  }
+  __syncthreads();
+  if (sl == 0 && dattn)
+    for (int t = threadIdx.x; t < rr * n; t += 256) dattn[((size_t)b * n + i0) * n + t] = sdA[(t / n) * ldS + t % n];
+  const int c0 = sl * kAttnFwdSlice, cw = min(kAttnFwdSlice, C - c0);
+  for (int j0 = 0; j0 < n; j0 += KT) {
+    const int jw = min(KT, n - j0);
+    __syncthreads();
+    load_rows(sT, ldV, base + (size_t)j0 * ldq + 2 * d + c0, ldq, jw, cw);
+    load_rows(sT2, ldV, tbase + (size_t)j0 * ldq + 2 * d + c0, ldq, jw, cw);
+    __syncthreads();
+    attn_gemm<1, 4>(tc, rr, cw, 2 * jw,
+                     [&](int i, int k) { return k < jw ? sdA[i * ldS + j0 + k] : sA[i * ldS + j0 + k - jw]; },
+                     [&](int k, int c) { return k < jw ? sT[k * ldV + c] : sT2[(k - jw) * ldV + c]; },
+                     [&](int i, int c, float v) { sO[i * ldV + c] += v; });
+  }
+  __syncthreads();
+  const float gm = gamma[0];
+  for (int t = threadIdx.x; t < rr * cw; t += 256) {
+    const int i = t / cw, c = t - i * cw;
+    const size_t idx = ((size_t)b * n + i0 + i) * C + c0 + c;
+    const float v = sO[i * ldV + c];
+    to[idx] = v;
+    const float yy = fmaf(gm, v, __ldg(tx + idx));
+    ty[idx] = yy;
+    if (ty_lo) ty_lo[idx] = lo_part(yy);
+  }
+}
+
+// Backward stage 1, grid (B, n / R): everything indexed by query row i.
+//   Abar = Go V^T + Gto Vdot^T + G (Sdot - r) - g Sdot,  G = Gto V^T,  r = rowsum(A Sdot),  g = rowsum(A G)   (Go = gamma gy, ...)
+//   Sbar = A (Abar - rowsum(A Abar)),  St^ = A (G - g)                                          -> sbar / stbar [B][n][n]
+//   gQ = Sbar K + St^ Kdot,  gQdot^ = St^ K                                                     -> gqkv / gtqkv, query columns
+//   per-row ggamma partials <gy, O> + <gty, Odot>                                               -> gpart [B][n]
+// V / Vdot and Go / Gto are streamed in 64 x 64 tiles; K / Kdot in 64-row tiles.  DUAL = false: first-order backward.
+template <bool DUAL>
+__global__ void __launch_bounds__(256)
+attn_bwd_rows_kernel(int n, int C, int d, int R, const float* __restrict__ qkv, const float* __restrict__ tqkv, int ldq,
+                     const float* __restrict__ attn, const float* __restrict__ o, const float* __restrict__ to, const float* __restrict__ gamma,
+                     const float* __restrict__ gy, const float* __restrict__ gty, float* __restrict__ gqkv, float* __restrict__ gtqkv,
+                     float* __restrict__ sbar, float* __restrict__ stbar, float* __restrict__ gpart, int tc) {
+  extern __shared__ float smem[];
+  const int b = blockIdx.x, i0 = blockIdx.y * R;
+  const int rr = min(R, n - i0), ldS = n + 1, ldD = d + 1, CS = kAttnFwdSlice, ldV = CS + 1, KT = kAttnKeyTile;
+  float* p = smem;
+  float* sA = p;   p += R * ldS;          // [R][n+1]
+  float* sAb = p;  p += R * ldS;          // Abar, then Sbar
+  float* sG = p;                          // G, then St^   (DUAL)
+  float* sSd = p + R * ldS;               // Sdot          (DUAL)
+  if (DUAL) p += 2 * R * ldS;
+  float* sGO = p;  p += R * ldV;          // [R][65] gamma gy, one 64-channel chunk
+  float* sGTO = p; if (DUAL) p += R * ldV;
+  float* sQ = p;                          // q / qdot rows (DUAL: for Sdot)
+  float* sTQ = p + R * ldD;
+  if (DUAL) p += 2 * R * ldD;
+  float* sAcc = p; p += R * ldD;          // gQ
+  float* sAccT = p; if (DUAL) p += R * ldD;   // gQdot^
+  float* sT = p;                          // 2 x [64][65] tiles
+  float* sT2 = sT + KT * ldV;
+  const float* base = qkv + (size_t)b * n * ldq;
+  const float* tbase = DUAL ? tqkv + (size_t)b * n * ldq : nullptr;
+  const size_t grow0 = (size_t)b * n + i0;
+  const float gm = gamma[0];
+  load_rows(sA, ldS, attn + grow0 * n, n, rr, n);
+  zero_smem(sAb, (DUAL ? 2 : 1) * R * ldS);
+  zero_smem(sAcc, (DUAL ? 2 : 1) * R * ldD);
+  if (DUAL) {
+    load_rows(sQ, ldD, base + (size_t)i0 * ldq, ldq, rr, d);
+    load_rows(sTQ, ldD, tbase + (size_t)i0 * ldq, ldq, rr, d);
+    for (int j0 = 0; j0 < n; j0 += KT) {
+      const int jw = min(KT, n - j0);
+      __syncthreads();
+      load_rows(sT, ldD, base + (size_t)j0 * ldq + d, ldq, jw, d);
+      load_rows(sT2, ldD, tbase + (size_t)j0 * ldq + d, ldq, jw, d);
+      __syncthreads();
+      attn_gemm<1, 4>(tc, rr, jw, 2 * d,
+                       [&](int i, int k) { return k < d ? sTQ[i * ldD + k] : sQ[i * ldD + k - d]; },
+                       [&](int k, int j) { return k < d ? sT[j * ldD + k] : sT2[j * ldD + k - d]; },
+                       [&](int i, int j, float v) { sSd[i * ldS + j0 + j] = v; });
+    }
+  }
+  // Abar1[i][j] = sum_c Go[i][c] V[j][c] (+ Gto[i][c] Vdot[j][c]),  G[i][j] = sum_c Gto[i][c] V[j][c]
+  for (int c0 = 0; c0 < C; c0 += CS) {
+    const int cw = min(CS, C - c0);
+    __syncthreads();
+    load_rows(sGO, ldV, gy ? gy + grow0 * C + c0 : nullptr, C, rr, cw, gm);
+    if (DUAL) load_rows(sGTO, ldV, gty + grow0 * C + c0, C, rr, cw, gm);
+    for (int j0 = 0; j0 < n; j0 += KT) {
+      const int jw = min(KT, n - j0);
+      __syncthreads();
+      load_rows(sT, ldV, base + (size_t)j0 * ldq + 2 * d + c0, ldq, jw, cw);
+      if (DUAL) load_rows(sT2, ldV, tbase + (size_t)j0 * ldq + 2 * d + c0, ldq, jw, cw);
+      __syncthreads();
+      attn_gemm<1, 4>(tc, rr, jw, DUAL ? 2 * cw : cw,
+                       [&](int i, int k) { return (!DUAL || k < cw) ? sGO[i * ldV + k] : sGTO[i * ldV + k - cw]; },
+                       [&](int k, int j) { return (!DUAL || k < cw) ? sT[j * ldV + k] : sT2[j * ldV + k - cw]; },
+                       [&](int i, int j, float v) { sAb[i * ldS + j0 + j] += v; });
+      if (DUAL)
+        attn_gemm<1, 4>(tc, rr, jw, cw, [&](int i, int k) { return sGTO[i * ldV + k]; }, [&](int k, int j) { return sT[j * ldV + k]; },
+                         [&](int i, int j, float v) { sG[i * ldS + j0 + j] += v; });
+    }
+  }
+  __syncthreads();
+  {
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    for (int i = warp; i < rr; i += 8) {
+      float* a = sA + i * ldS;
+      float* ab = sAb + i * ldS;
+      float r = 0.f, g = 0.f;
+      if (DUAL) {
+        for (int j = lane; j < n; j += 32) { r = fmaf(a[j], sSd[i * ldS + j], r); g = fmaf(a[j], sG[i * ldS + j], g); }
+        r = warp_sum(r); g = warp_sum(g);
+      }
+      float aa = 0.f;
+      for (int j = lane; j < n; j += 32) {
+        if (DUAL) { const float sd = sSd[i * ldS + j]; ab[j] += sG[i * ldS + j] * (sd - r) - g * sd; }
+        aa = fmaf(a[j], ab[j], aa);
+      }
+      aa = warp_sum(aa);
+      float* gsb = sbar + (grow0 + i) * n;
+      for (int j = lane; j < n; j += 32) {
+        const float s = a[j] * (ab[j] - aa);
+        ab[j] = s;
+        gsb[j] = s;
+        if (DUAL) {
+          const float st = a[j] * (sG[i * ldS + j] - g);
+          sG[i * ldS + j] = st;
+          stbar[(grow0 + i) * n + j] = st;
+        }
+      }
+      float gp = 0.f;
+      for (int c = lane; c < C; c += 32) {
+        const size_t idx = (grow0 + i) * C + c;
+        if (gy) gp = fmaf(__ldg(gy + idx), __ldg(o + idx), gp);
+        if (DUAL) gp = fmaf(__ldg(gty + idx), __ldg(to + idx), gp);
+      }
+      gp = warp_sum(gp);
+      if (lane == 0) gpart[grow0 + i] = gp;
+    }
+  }
+  // gQ[i] = sum_j Sbar[i][j] K[j] (+ St^[i][j] Kdot[j]),  gQdot^[i] = sum_j St^[i][j] K[j]
+  for (int j0 = 0; j0 < n; j0 += KT) {
+    const int jw = min(KT, n - j0);
+    __syncthreads();
+    load_rows(sT, ldD, base + (size_t)j0 * ldq + d, ldq, jw, d);
+    if (DUAL) load_rows(sT2, ldD, tbase + (size_t)j0 * ldq + d, ldq, jw, d);
+    __syncthreads();
+    attn_gemm<1, 4>(tc, rr, d, DUAL ? 2 * jw : jw,
+                     [&](int i, int k) { return (!DUAL || k < jw) ? sAb[i * ldS + j0 + k] : sG[i * ldS + j0 + k - jw]; },
+                     [&](int k, int c) { return (!DUAL || k < jw) ? sT[k * ldD + c] : sT2[(k - jw) * ldD + c]; },
+                     [&](int i, int c, float v) { sAcc[i * ldD + c] += v; });
+    if (DUAL)
+      attn_gemm<1, 4>(tc, rr, d, jw, [&](int i, int k) { return sG[i * ldS + j0 + k]; }, [&](int k, int c) { return sT[k * ldD + c]; },
+                       [&](int i, int c, float v) { sAccT[i * ldD + c] += v; });
+  }
+  __syncthreads();
+  for (int t = threadIdx.x; t < rr * d; t += 256) {
+    const int i = t / d, c = t - i * d;
+    gqkv[(grow0 + i) * ldq + c] = sAcc[i * ldD + c];
+    if (DUAL) gtqkv[(grow0 + i) * ldq + c] = sAccT[i * ldD + c];
+  }
+}
+
+// Backward stage 2, grid (B, n / 32, 1 + C / 64): everything indexed by key row j, as X^T P (+ Y^T PT) and X^T PT over query
+// tiles i of 32 rows:
+//   z = 0:      gK = St^^T Qdot + Sbar^T Q,  gKdot^ = St^^T Q      (X, Y = stbar, sbar; P, PT = qdot, q.  First order: Sbar^T Q)
+//   z = 1 + s:  gV = A^T Go + Adot^T Gto,    gVdot^ = A^T Gto      (X, Y = attn, dattn; P, PT = gamma gy, gamma gty; slice s)
+// Block (0, 0, 0) also sums the per-row ggamma partials (fixed order).
+template <bool DUAL>
+__global__ void __launch_bounds__(256)
+attn_bwd_keys_kernel(int B, int n, int C, int d, const float* __restrict__ qkv, const float* __restrict__ tqkv, int ldq,
+                     const float* __restrict__ attn, const float* __restrict__ dattn, const float* __restrict__ gamma,
+                     const float* __restrict__ gy, const float* __restrict__ gty, const float* __restrict__ sbar,
+                     const float* __restrict__ stbar, const float* __restrict__ gpart, float* __restrict__ gqkv, float* __restrict__ gtqkv,
+                     float* ggamma, int accumulate, int tc) {
+  extern __shared__ float smem[];
+  __shared__ float red[64];
+  constexpr int RJ = kAttnKeyRows, IT = kAttnKeyRows, ldX = RJ + 1, ldP = kAttnFwdSlice + 1;
+  const int b = blockIdx.x, j0 = blockIdx.y * RJ, z = blockIdx.z;
+  const int rw = min(RJ, n - j0);
+  float* sX = smem;                       // [IT][33]  X[i][j]
+  float* sY = sX + IT * ldX;              // [IT][33]  Y[i][j]   (DUAL)
+  float* sP = sY + IT * ldX;              // [IT][65]  P[i][c]
+  float* sPT = sP + IT * ldP;             // [IT][65]  PT[i][c]  (DUAL)
+  float* sAcc = sPT + IT * ldP;           // [32][65]
+  float* sAccT = sAcc + RJ * ldP;         // [32][65]  (DUAL)
+  const float gm = gamma[0];
+  const size_t nn = (size_t)b * n * n;
+  const float *X, *Y = nullptr, *P, *PT = nullptr;
+  int cw, pcol, ocol;
+  long long ldp;
+  float mul;
+  if (z == 0) {
+    cw = d; pcol = 0; ocol = d; ldp = ldq; mul = 1.f;
+    const float* q = qkv + (size_t)b * n * ldq;
+    if (DUAL) { X = stbar + nn; Y = sbar + nn; P = tqkv + (size_t)b * n * ldq; PT = q; }
+    else { X = sbar + nn; P = q; }
+  } else {
+    X = attn + nn;
+    if (DUAL) Y = dattn + nn;
+    const int c0 = (z - 1) * kAttnFwdSlice;
+    cw = min(kAttnFwdSlice, C - c0); pcol = c0; ocol = 2 * d + c0; ldp = C; mul = gm;
+    P = gy ? gy + (size_t)b * n * C : nullptr; PT = DUAL ? gty + (size_t)b * n * C : nullptr;
+  }
+  zero_smem(sAcc, 2 * RJ * ldP);
+  for (int i0 = 0; i0 < n; i0 += IT) {
+    const int iw = min(IT, n - i0);
+    __syncthreads();
+    load_rows(sX, ldX, X + (size_t)i0 * n + j0, n, iw, rw);
+    load_rows(sP, ldP, P ? P + (size_t)i0 * ldp + pcol : nullptr, ldp, iw, cw, mul);
+    if (DUAL) {
+      load_rows(sY, ldX, Y + (size_t)i0 * n + j0, n, iw, rw);
+      load_rows(sPT, ldP, PT + (size_t)i0 * ldp + pcol, ldp, iw, cw, mul);
+    }
+    __syncthreads();
+    attn_gemm<1, 4>(tc, rw, cw, DUAL ? 2 * iw : iw,
+                     [&](int j, int k) { return (!DUAL || k < iw) ? sX[k * ldX + j] : sY[(k - iw) * ldX + j]; },
+                     [&](int k, int c) { return (!DUAL || k < iw) ? sP[k * ldP + c] : sPT[(k - iw) * ldP + c]; },
+                     [&](int j, int c, float v) { sAcc[j * ldP + c] += v; });
+    if (DUAL)
+      attn_gemm<1, 4>(tc, rw, cw, iw, [&](int j, int k) { return sX[k * ldX + j]; }, [&](int k, int c) { return sPT[k * ldP + c]; },
+                       [&](int j, int c, float v) { sAccT[j * ldP + c] += v; });
+  }
+  __syncthreads();
+  for (int t = threadIdx.x; t < rw * cw; t += 256) {
+    const int j = t / cw, c = t - j * cw;
+    const size_t row = (size_t)b * n + j0 + j;
+    gqkv[row * ldq + ocol + c] = sAcc[j * ldP + c];
+    if (DUAL) gtqkv[row * ldq + ocol + c] = sAccT[j * ldP + c];
+  }
+  if (ggamma && b == 0 && blockIdx.y == 0 && z == 0) {
+    float t = 0.f;
+    for (int i = threadIdx.x; i < B * n; i += 256) t += gpart[i];
+    t = block_sum(t, red);
+    if (threadIdx.x == 0) ggamma[0] = accumulate ? ggamma[0] + t : t;
+  }
+}
+
 template <typename Kernel>
 bool set_smem(Kernel k, size_t bytes, const char* who) {
-  if (bytes > 232448) { set_error_msg(who, "attention tile exceeds the 227 KB of shared memory (n <= 128, d <= 64)"); return false; }
+  if (bytes > 232448) { set_error_msg(who, "attention tile exceeds the 227 KB of shared memory (n <= 1024, d <= 64)"); return false; }
   cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
   if (e != cudaSuccess) { set_error(who, e); return false; }
   return true;
 }
 
 bool attn_shape_ok(int B, int n, int C, int d, int ldq, const char* who) {
-  if (B <= 0 || n <= 0 || n > kAttnMaxN || d <= 0 || d > 64 || C <= 0 || ldq < 2 * d + C) {
-    set_error_msg(who, "unsupported attention shape (1 <= n <= 128 positions, d <= 64, ldq >= 2d + C)");
+  if (B <= 0 || n <= 0 || n > kAttnTiledMaxN || d <= 0 || d > 64 || C <= 0 || ldq < 2 * d + C) {
+    set_error_msg(who, "unsupported attention shape (1 <= n <= 1024 positions, d <= 64, ldq >= 2d + C)");
     return false;
   }
   return true;
 }
+
+int g_attn_tiled = 0;
+
+constexpr size_t kAttnSmemMax = 232448;
+
+// The whole-tile kernels for n <= 128 where their tiles fit shared memory (whole_tile_bytes; at n = 128 the tangent and the joint
+// backward of d = 64 do not); the row-stripe kernels for everything else, and for every n under skd_set_attn_tiled(1).
+bool attn_use_tiled(int n, size_t whole_tile_bytes) { return n > kAttnMaxN || whole_tile_bytes > kAttnSmemMax || g_attn_tiled; }
+
+// rows per stripe: 16, or 8 where 16 would not fit (floats(R) = the kernel's shared-memory floats).  8 always fits: the
+// static_asserts below check the largest kernels at n = kAttnTiledMaxN, d = 64, so raising the bound fails to compile first.
+template <class F>
+int attn_stripe_rows(F floats) { return floats(16) * 4 <= kAttnSmemMax ? 16 : 8; }
+
+constexpr size_t attn_fwd_tiled_floats(int R, int n, int d, bool tangent) {
+  const size_t ldS = n + 1, ldD = d + 1, ldV = kAttnFwdSlice + 1;
+  return (tangent ? 2 : 1) * R * ldS + (tangent ? 2 : 1) * R * ldD + R * ldV + (tangent ? 2 : 1) * kAttnKeyTile * ldV;
+}
+
+constexpr size_t attn_bwd_rows_floats(int R, int n, int d, bool dual) {
+  const size_t ldS = n + 1, ldD = d + 1, ldV = kAttnFwdSlice + 1;
+  return (dual ? 4 : 2) * R * ldS + (dual ? 2 : 1) * R * ldV + (dual ? 4 : 1) * R * ldD + 2 * kAttnKeyTile * ldV;
+}
+
+static_assert(attn_fwd_tiled_floats(8, kAttnTiledMaxN, 64, true) * 4 <= kAttnSmemMax, "tangent stripe of 8 rows must fit at the bound");
+static_assert(attn_bwd_rows_floats(8, kAttnTiledMaxN, 64, true) * 4 <= kAttnSmemMax, "joint backward stripe of 8 rows must fit at the bound");
+
+constexpr size_t kAttnKeysBytes = (2 * kAttnKeyRows * (kAttnKeyRows + 1) + 4 * kAttnKeyRows * (kAttnFwdSlice + 1)) * 4;
 
 }  // namespace
 
@@ -1170,11 +1555,21 @@ extern "C" int skd_gp_direction(int B, long long len, const float* g, const floa
 
 extern "C" void skd_set_attn_tensor_cores(int on) { g_attn_tc = on ? 1 : 0; }
 
+extern "C" void skd_set_attn_tiled(int force) { g_attn_tiled = force ? 1 : 0; }
+
 extern "C" int skd_attn_fwd(int B, int n, int C, int d, const float* qkv, int ldq, const float* x, const float* gamma, float* attn, float* o,
                             float* y, float* y_lo, cudaStream_t st) {
   const char* who = "skd_attn_fwd";
   if (!attn_shape_ok(B, n, C, d, ldq, who)) return 0;
   const size_t bytes = ((size_t)n * (n + 1) + 2 * (size_t)n * (d + 1) + (size_t)n * (kAttnFwdSlice + 1)) * 4;
+  if (attn_use_tiled(n, bytes)) {
+    const int R = attn_stripe_rows([&](int r) { return attn_fwd_tiled_floats(r, n, d, false); });
+    const size_t tb = attn_fwd_tiled_floats(R, n, d, false) * 4;
+    if (!set_smem(attn_fwd_tiled_kernel, tb, who)) return 0;
+    attn_fwd_tiled_kernel<<<dim3(B, (n + R - 1) / R, (C + kAttnFwdSlice - 1) / kAttnFwdSlice), 256, tb, st>>>(
+        n, C, d, R, qkv, ldq, x, gamma, attn, o, y, y_lo, g_attn_tc);
+    return finish(who);
+  }
   if (!set_smem(attn_fwd_kernel, bytes, who)) return 0;
   attn_fwd_kernel<<<dim3(B, (C + kAttnFwdSlice - 1) / kAttnFwdSlice), 256, bytes, st>>>(n, C, d, qkv, ldq, x, gamma, attn, o, y, y_lo, g_attn_tc);
   return finish(who);
@@ -1187,14 +1582,27 @@ extern "C" int skd_attn_tangent_fwd(int B, int n, int C, int d, const float* qkv
   size_t region = 4 * (size_t)n * (d + 1), need = 2 * (size_t)n * (kAttnFwdSlice + 1);
   if (region < need) region = need;
   const size_t bytes = (2 * (size_t)n * (n + 1) + region) * 4;
+  if (attn_use_tiled(n, bytes)) {
+    const int R = attn_stripe_rows([&](int r) { return attn_fwd_tiled_floats(r, n, d, true); });
+    const size_t tb = attn_fwd_tiled_floats(R, n, d, true) * 4;
+    if (!set_smem(attn_tangent_tiled_kernel, tb, who)) return 0;
+    attn_tangent_tiled_kernel<<<dim3(B, (n + R - 1) / R, (C + kAttnFwdSlice - 1) / kAttnFwdSlice), 256, tb, st>>>(
+        n, C, d, R, qkv, tqkv, ldq, attn, tx, gamma, dattn, to, ty, ty_lo, g_attn_tc);
+    return finish(who);
+  }
   if (!set_smem(attn_tangent_kernel, bytes, who)) return 0;
   attn_tangent_kernel<<<dim3(B, (C + kAttnFwdSlice - 1) / kAttnFwdSlice), 256, bytes, st>>>(n, C, d, qkv, tqkv, ldq, attn, tx, gamma, dattn, to, ty, ty_lo, g_attn_tc);
   return finish(who);
 }
 
+// The row-stripe backward: Sbar, St^ [B][n][n] and per-row ggamma partials.  For n <= 128 the larger of both paths' sizes: which
+// path runs there also depends on d, the mode (first order / joint) and skd_set_attn_tiled.
 extern "C" long long skd_attn_bwd_workspace_floats(int B, int n, int C) {
+  const long long tiled = 2LL * B * n * n + (long long)B * n;
+  if (n > kAttnMaxN) return tiled;
   const long long nsl = (C + kAttnBwdSlice - 1) / kAttnBwdSlice;
-  return (long long)B * nsl * 2 * n * n + (long long)B * nsl;
+  const long long whole = (long long)B * nsl * 2 * n * n + (long long)B * nsl;
+  return whole > tiled ? whole : tiled;
 }
 
 extern "C" int skd_attn_bwd(int B, int n, int C, int d, const float* qkv, int ldq, const float* attn, const float* o, const float* gamma,
@@ -1204,11 +1612,30 @@ extern "C" int skd_attn_bwd(int B, int n, int C, int d, const float* qkv, int ld
   if (!attn_shape_ok(B, n, C, d, ldq, who)) return 0;
   const bool dual = gty != nullptr;
   if (dual && !(tqkv && dattn && to && gtqkv)) { set_error_msg(who, "the joint backward needs tqkv, dattn, to and gtqkv"); return 0; }
+  const size_t b1 = ((dual ? 2 : 1) * (size_t)n * (n + 1) + (dual ? 4 : 2) * (size_t)n * (kAttnBwdSlice + 1)) * 4;
+  const size_t b2 = ((dual ? 2 : 1) * (size_t)n * (n + 1) + (dual ? 4 : 2) * (size_t)n * (d + 1)) * 4;
+  if (attn_use_tiled(n, b1 > b2 ? b1 : b2)) {
+    const size_t nn = (size_t)B * n * n;
+    float *sbar = workspace, *stbar = workspace + nn, *gpart = workspace + 2 * nn;
+    const int R = attn_stripe_rows([&](int r) { return attn_bwd_rows_floats(r, n, d, dual); });
+    const size_t rb = attn_bwd_rows_floats(R, n, d, dual) * 4;
+    const dim3 g1(B, (n + R - 1) / R), g2(B, (n + kAttnKeyRows - 1) / kAttnKeyRows, 1 + (C + kAttnFwdSlice - 1) / kAttnFwdSlice);
+    if (dual) {
+      if (!set_smem(attn_bwd_rows_kernel<true>, rb, who) || !set_smem(attn_bwd_keys_kernel<true>, kAttnKeysBytes, who)) return 0;
+      attn_bwd_rows_kernel<true><<<g1, 256, rb, st>>>(n, C, d, R, qkv, tqkv, ldq, attn, o, to, gamma, gy, gty, gqkv, gtqkv, sbar, stbar, gpart, g_attn_tc);
+      attn_bwd_keys_kernel<true><<<g2, 256, kAttnKeysBytes, st>>>(B, n, C, d, qkv, tqkv, ldq, attn, dattn, gamma, gy, gty, sbar, stbar, gpart, gqkv,
+                                                                  gtqkv, ggamma, accumulate, g_attn_tc);
+    } else {
+      if (!set_smem(attn_bwd_rows_kernel<false>, rb, who) || !set_smem(attn_bwd_keys_kernel<false>, kAttnKeysBytes, who)) return 0;
+      attn_bwd_rows_kernel<false><<<g1, 256, rb, st>>>(n, C, d, R, qkv, nullptr, ldq, attn, o, nullptr, gamma, gy, nullptr, gqkv, nullptr, sbar, nullptr,
+                                                       gpart, g_attn_tc);
+      attn_bwd_keys_kernel<false><<<g2, 256, kAttnKeysBytes, st>>>(B, n, C, d, qkv, nullptr, ldq, attn, nullptr, gamma, gy, nullptr, sbar, nullptr, gpart,
+                                                                   gqkv, nullptr, ggamma, accumulate, g_attn_tc);
+    }
+    return finish(who, 2);
+  }
   const int nsl = (C + kAttnBwdSlice - 1) / kAttnBwdSlice;
   float* gpart = workspace + (size_t)B * nsl * 2 * n * n;
-  const size_t ldV = kAttnBwdSlice + 1;
-  const size_t b1 = ((dual ? 2 : 1) * (size_t)n * (n + 1) + (dual ? 4 : 2) * (size_t)n * ldV) * 4;
-  const size_t b2 = ((dual ? 2 : 1) * (size_t)n * (n + 1) + (dual ? 4 : 2) * (size_t)n * (d + 1)) * 4;
   if (dual) {
     if (!set_smem(attn_bwd1_kernel<true>, b1, who) || !set_smem(attn_bwd2_kernel<true>, b2, who)) return 0;
     attn_bwd1_kernel<true><<<dim3(B, nsl), 256, b1, st>>>(n, C, d, qkv, tqkv, ldq, attn, dattn, o, to, gamma, gy, gty, gqkv, gtqkv, workspace, gpart, g_attn_tc);
