@@ -294,6 +294,15 @@ int skd_bn2d_jacobian(int N, int C, int HW, const float* x, long long sn, long l
 /* dgamma (+)= sum gh xhat [+ sum gth t0], dbeta (+)= sum gh; sums_t / sums_v NULL for the first-order backward */
 int skd_bn2d_param_grad(int C, long long P, const float* rstd, const float* sums_g, const float* sums_t, const float* sums_v, float* dgamma,
                         float* dbeta, int accumulate, cudaStream_t);
+/* preprocess_GAN_mode 2 / 3 (sagan_models.py:149-152), no parameters: mode 2 out = tanhf(x); mode 3 out = 2 * (x / 255 - 0.5) in the
+   reference's fp32 operation order (IEEE division).  Same addressing and output as skd_bn2d_apply: x by (sn, sc, sp) strides, out
+   [N*HW][Cp] with channels >= C zero, out_lo (may be NULL) its TF32 lo part */
+int skd_disc_pointwise_prep(int mode, int N, int C, int HW, const float* x, long long sn, long long sc, long long sp, float* out, float* out_lo,
+                            int Cp, cudaStream_t);
+/* out = J a with the diagonal Jacobian of that map at x: mode 2 a * (1 - tanhf(x)^2), mode 3 (a * 2) / 255.  a dense [N*HW][ld]; out by
+   (on, oc, op) strides over Cq channels (channels >= C zero), out_lo may be NULL -- as skd_bn2d_jacobian */
+int skd_disc_pointwise_prep_jacobian(int mode, int N, int C, int HW, const float* x, long long sn, long long sc, long long sp, const float* a,
+                                     int ld, float* out, long long on, long long oc, long long op, int Cq, float* out_lo, cudaStream_t);
 /* Self_Attn core (sagan_models.py:31-40): A = softmax(Q K^T) (no 1/sqrt(d)), O = A V, y = gamma O + x.
    qkv [B*n][ldq] = [q(d) | k(d) | v(C)] (the three 1x1 convolutions as one GEMM), x / o / y [B*n][C], attn [B][n][n]; n <= 1024, d <= 64.
    n <= 128 runs whole n x n tiles per CTA; n > 128 runs stripes of query rows with keys / values streamed in tiles. */

@@ -548,6 +548,58 @@ __global__ void bn2d_param_grad_kernel(int C, long long P, const float* __restri
 }
 
 // ====================================================================================================================
+// pointwise preprocessing of preprocess_GAN_mode 2 (nn.Tanh) and 3 (lambda x: 2 * (x / 255 - 0.5)), sagan_models.py:149-152
+// ====================================================================================================================
+// Mode 3 keeps the reference's operation order in fp32 with IEEE division (torch's CPU `x / 255` is a true division, not a
+// multiply by the reciprocal); the explicit _rn intrinsics keep the compiler from contracting the steps into one FMA.
+__device__ __forceinline__ float pointwise_prep(int mode, float x) {
+  return mode == 2 ? tanhf(x) : __fmul_rn(2.f, __fsub_rn(__fdiv_rn(x, 255.f), 0.5f));
+}
+
+// out[p][c] = f(x) for c < C; channels C..Cp-1 zero (the same output contract as bn2d_apply_kernel)
+__global__ void __launch_bounds__(256)
+pointwise_prep_kernel(int mode, int N, int C, int HW, const float* __restrict__ x, long long sn, long long sc, long long sp,
+                      float* __restrict__ out, float* __restrict__ out_lo, int Cp) {
+  const long long total = (long long)N * HW * Cp;
+  for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < total; i += (long long)gridDim.x * 256) {
+    const int c = (int)(i % Cp); const long long p = i / Cp;
+    float val = 0.f;
+    if (c < C) {
+      const long long n = p / HW, q = p - n * HW;
+      val = pointwise_prep(mode, __ldg(x + n * sn + c * sc + q * sp));
+    }
+    out[i] = val;
+    if (out_lo) out_lo[i] = lo_part(val);
+  }
+}
+
+// out = f'(x) * a.  Mode 2: torch's tanh_backward a * (1 - y^2) with y = tanhf(x) in full fp32 (exactly 0 where tanhf saturates
+// to +-1).  Mode 3: autograd's order for 2 * (x / 255 - 0.5): (a * 2) / 255.  The Jacobian is diagonal, hence its own transpose:
+// the same kernel gives the input gradient and the forward-mode tangent.  a dense [N*HW][ld], out strided; channels C..Cq-1 zero.
+__global__ void __launch_bounds__(256)
+pointwise_prep_jacobian_kernel(int mode, int N, int C, int HW, const float* __restrict__ x, long long sn, long long sc, long long sp,
+                               const float* __restrict__ a, int ld, float* __restrict__ out, long long on, long long oc, long long op,
+                               int Cq, float* __restrict__ out_lo) {
+  const long long total = (long long)N * HW * Cq;
+  for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < total; i += (long long)gridDim.x * 256) {
+    const int c = (int)(i % Cq); const long long p = i / Cq;
+    const long long n = p / HW, q = p - n * HW;
+    float val = 0.f;
+    if (c < C) {
+      const float g = __ldg(a + p * ld + c);
+      if (mode == 2) {
+        const float y = tanhf(__ldg(x + n * sn + c * sc + q * sp));
+        val = __fmul_rn(g, __fsub_rn(1.f, __fmul_rn(y, y)));
+      } else {
+        val = __fdiv_rn(__fmul_rn(g, 2.f), 255.f);
+      }
+    }
+    out[n * on + c * oc + q * op] = val;
+    if (out_lo) out_lo[n * on + c * oc + q * op] = lo_part(val);
+  }
+}
+
+// ====================================================================================================================
 // element-wise glue around the convolutions
 // ====================================================================================================================
 // out = in * leaky'(ref)   (the mask is recovered from the sign of the post-activation output; ref repeats every `period` elements:
@@ -1491,6 +1543,24 @@ extern "C" int skd_bn2d_param_grad(int C, long long P, const float* rstd, const 
                                    float* dgamma, float* dbeta, int accumulate, cudaStream_t st) {
   bn2d_param_grad_kernel<<<1, 32, 0, st>>>(C, P, rstd, sums_g, sums_t, sums_v, dgamma, dbeta, accumulate);
   return finish("skd_bn2d_param_grad");
+}
+
+extern "C" int skd_disc_pointwise_prep(int mode, int N, int C, int HW, const float* x, long long sn, long long sc, long long sp, float* out,
+                                       float* out_lo, int Cp, cudaStream_t st) {
+  if (mode != 2 && mode != 3) { set_error_msg("skd_disc_pointwise_prep", "mode must be 2 (tanh) or 3 (rescale)"); return 0; }
+  if (C <= 0 || Cp < C) { set_error_msg("skd_disc_pointwise_prep", "need 0 < C <= Cp"); return 0; }
+  pointwise_prep_kernel<<<blocks_for((long long)N * HW * Cp), 256, 0, st>>>(mode, N, C, HW, x, sn, sc, sp, out, out_lo, Cp);
+  return finish("skd_disc_pointwise_prep");
+}
+
+extern "C" int skd_disc_pointwise_prep_jacobian(int mode, int N, int C, int HW, const float* x, long long sn, long long sc, long long sp,
+                                                const float* a, int ld, float* out, long long on, long long oc, long long op, int Cq,
+                                                float* out_lo, cudaStream_t st) {
+  if (mode != 2 && mode != 3) { set_error_msg("skd_disc_pointwise_prep_jacobian", "mode must be 2 (tanh) or 3 (rescale)"); return 0; }
+  if (C <= 0 || Cq < C || ld < C) { set_error_msg("skd_disc_pointwise_prep_jacobian", "need 0 < C <= Cq and C <= ld"); return 0; }
+  pointwise_prep_jacobian_kernel<<<blocks_for((long long)N * HW * Cq), 256, 0, st>>>(mode, N, C, HW, x, sn, sc, sp, a, ld, out, on, oc, op, Cq,
+                                                                                    out_lo);
+  return finish("skd_disc_pointwise_prep_jacobian");
 }
 
 extern "C" int skd_disc_mask_mul(long long n, long long period, const float* ref, const float* in, float* out, float* out_lo, float slope,

@@ -2,13 +2,15 @@
 
 Three passes over the same parameters, none of them through torch operators or autograd:
 
-  forward(x)            networks/sagan_models.py:156-168 (+ spectral.py:23-35 power iteration per SN layer, BN2d batch stats)
+  forward(x)            networks/sagan_models.py:156-168 (+ spectral.py:23-35 power iteration per SN layer, then the input
+                        preprocessing: BN2d batch stats (preprocess_GAN_mode 1), tanh (2) or 2 (x / 255 - 0.5) (3))
   backward(tape, gout)  first-order reverse pass: parameter gradients and, on request, d out / d x
   gp_forward / gp_backward   CriterionAdditionalGP (utils/criterion.py:98-120) WITHOUT double backward: the first-order chain to
                         the input gives g = d(sum D(x))/dx and the penalty value; the parameter gradient is "reverse over
                         forward" -- a tangent pass along v = c_n g_n, then one reverse pass over the joint (primal, tangent)
                         graph, which for the bilinear layers is the ordinary backward over a [primal | tangent] batch of 2B.
-                        oracle/gp_dual.py states the same operation sequence in torch and is pinned against autograd.
+                        oracle/gp_dual.py (mode 1) and oracle/gp_dual_preprocess.py (modes 2 / 3) state the same operation
+                        sequence in torch and are pinned against autograd.
 
 Activations are NHWC rows.  The 4x4/s2 spectral-norm convolutions and the q/k/v projections run on the wgmma implicit-GEMM
 kernel in split precision (3xTF32); weight gradients on the wgmma wgrad kernel (TF32); 1/sigma rides in the convolution
@@ -176,12 +178,15 @@ class DiscEngine:
         # all four layers in one call: each phase of the iteration is a grid over every layer (csrc/disc.cu, sn_phase*_kernel)
         sn_ws = _f(L.skd_sn_power_iter_batched_workspace_floats(len(descs), ctypes.cast(descs, ctypes.c_void_p)), dev=dev)
         L.skd_sn_power_iter_batched(len(descs), ctypes.cast(descs, ctypes.c_void_p), _p(sn_ws), st)
-        # ---- preprocess (sagan_models.py:147,157): BatchNorm2d with batch statistics in train mode
+        # ---- preprocess (sagan_models.py:147-152,158): BatchNorm2d with batch statistics in train mode (mode 1), or the
+        # parameter-free tanh (mode 2) / rescale 2 (x / 255 - 0.5) (mode 3), the same in train() and eval()
         bn = D.preprocess_additional
         Cp = ops.pad4(C)
         t.Cp = Cp
         t.h0, t.h0_lo = _f(cap, H, W, Cp, dev=dev), _f(cap, H, W, Cp, dev=dev)
-        if D.preprocess_mode == 1:
+        if D.preprocess_mode in (2, 3):
+            L.skd_disc_pointwise_prep(D.preprocess_mode, B, C, H * W, _p(x), *t.xs, _p(t.h0), _p(t.h0_lo) if self.precise else None, Cp, st)
+        elif D.preprocess_mode == 1:
             t.mean, t.rstd = _f(32, dev=dev), _f(32, dev=dev)
             if bn.training:
                 L.skd_bn2d_stats(B, C, H * W, _p(x), *t.xs, bn.eps, bn.momentum, _p(bn.running_mean), _p(bn.running_var),
@@ -192,7 +197,7 @@ class DiscEngine:
             L.skd_bn2d_apply(B, C, H * W, _p(x), *t.xs, _p(t.mean), _p(t.rstd), _p(bn.weight), _p(bn.bias), _p(t.h0),
                              _p(t.h0_lo) if self.precise else None, Cp, st)
         else:
-            raise NotImplementedError("preprocess_GAN_mode 2 / 3 (tanh / rescale) are not on the distillation path (run_train_val.sh uses 1)")
+            raise ValueError("preprocess_GAN_mode should be 1:bn or 2:tanh or 3:-1 - 1")
         # ---- SN conv -> LeakyReLU(0.1) stacks, attention after l3 and l4 (sagan_models.py:158-165)
         t.h, t.h_lo, t.dims, t.att = [], [], [(H, W)], {}
         hin, hin_lo, hc, wc = t.h0, t.h0_lo, H, W
@@ -244,7 +249,7 @@ class DiscEngine:
     def _reverse_layers(self, t, g_top, joint, sink, param_grads, need_input_adj):
         """Reverse pass through the conv / attention stack from the adjoint of the last conv's input.  joint: rows are
         [primal | tangent] (2B images); masks and attention maps come from the primal half.  Returns the adjoint of the
-        BatchNorm output [nb][H][W][Cp] (None when not needed)."""
+        preprocessing's output [nb][H][W][Cp] (None when not needed)."""
         L, st = lib(), _st()
         D = self.D
         dev = g_top.device
@@ -371,6 +376,27 @@ class DiscEngine:
                             C, None, st)
         return dx
 
+    def _prep_jacobian(self, t, a, dense, out=None, out_lo=None):
+        """Modes 2 / 3: out = J a with the diagonal Jacobian of the pointwise preprocessing at t.x; a dense [B][H][W][Cp].
+        dense: out is [B][H][W][Cp] rows with zero pad channels (`out` / `out_lo` given, or new); else a new tensor in x's layout."""
+        B, C, H, W, Cp = t.B, t.C, t.H, t.W, t.Cp
+        if dense:
+            out = _f(B, H, W, Cp, dev=a.device) if out is None else out
+            strides, cq = (H * W * Cp, 1, Cp), Cp
+        else:
+            out = torch.empty_strided(t.x.shape, t.x.stride(), device=a.device, dtype=torch.float32)
+            strides, cq = ops.pixel_strides(out), C
+        lib().skd_disc_pointwise_prep_jacobian(self.D.preprocess_mode, B, C, H * W, _p(t.x), *t.xs, _p(a), Cp, _p(out), *strides, cq,
+                                               _p(out_lo) if self.precise else None, _st())
+        return out
+
+    def _reverse_prep(self, t, g, joint, sink, param_grads, want_dx, sums_v=None, vdir=None, dense=False):
+        """Reverse pass through the preprocessing from g, the adjoint of its output: BatchNorm2d (mode 1, parameter gradients
+        included) or the parameter-free pointwise maps of modes 2 / 3, whose only contribution is d / d x on request."""
+        if self.D.preprocess_mode == 1:
+            return self._reverse_bn(t, g, joint, sink, param_grads, want_dx, sums_v=sums_v, vdir=vdir, dense=dense)
+        return self._prep_jacobian(t, g, dense) if want_dx else None
+
     def _emit(self, sink, name, param, value):
         buf, acc = self._grad_buf(sink, name, param)
         if acc:
@@ -395,10 +421,12 @@ class DiscEngine:
             if not acc and (t.kh < 4 or t.kw < 4):
                 gw.zero_()
             L.skd_disc_last_wgrad(B, hc, wc, t.ctop, t.kh, t.kw, _p(t.top), _p(gout), _p(gw), 4 * t.ctop, _p(gb), acc, st)
-        gh0 = self._reverse_layers(t, g, False, sink, param_grads, need_input_adj=want_dx or param_grads)
+        # layer 1's data gradient feeds d / d x and, in mode 1, BatchNorm's weight / bias gradients; modes 2 / 3 have no parameters there
+        need = want_dx or (param_grads and D.preprocess_mode == 1)
+        gh0 = self._reverse_layers(t, g, False, sink, param_grads, need_input_adj=need)
         if gh0 is None:
             return None
-        return self._reverse_bn(t, gh0, False, sink, param_grads, want_dx)
+        return self._reverse_prep(t, gh0, False, sink, param_grads, want_dx)
 
     # ------------------------------------------------------------------------------------------------ WGAN-GP
     def gp_forward(self, x, lambda_gp):
@@ -411,9 +439,9 @@ class DiscEngine:
         last = self.D.last[0]
         g = _f(B, hc, wc, t.ctop, dev=dev)
         L.skd_disc_last_dgrad(B, hc, wc, t.ctop, t.kh, t.kw, None, _p(last.weight), 4 * t.ctop, _p(g), None, st)   # grad_outputs = ones
-        # first-order chain to the input, no parameter gradients; BN's input gradient in the dense [B][H][W][Cp] layout
+        # first-order chain to the input, no parameter gradients; the preprocessing's input gradient in the dense [B][H][W][Cp] layout
         gh0 = self._reverse_layers(t, g, False, None, False, need_input_adj=True)
-        gx = self._reverse_bn(t, gh0, False, None, False, True, dense=True)
+        gx = self._reverse_prep(t, gh0, False, None, False, True, dense=True)
         t.g = gx
         t.norms, t.gp = _f(B, dev=dev), torch.empty((), device=dev, dtype=torch.float32)
         L.skd_gp_norms(B, t.H * t.W * t.Cp, _p(gx), float(lambda_gp), _p(t.norms), _p(t.gp), st)
@@ -427,14 +455,20 @@ class DiscEngine:
         dev = t.g.device
         B, C, H, W, Cp = t.B, t.C, t.H, t.W, t.Cp
         ws = self._workspaces(dev)
-        bn = D.preprocess_additional
+        mode = D.preprocess_mode
         vdir = _f(B, H, W, Cp, dev=dev)
         L.skd_gp_direction(B, H * W * Cp, _p(t.g), _p(t.norms), t.lambda_gp, _p(upstream), _p(vdir), st)
-        # ---- tangent forward along v: BN's Jacobian is symmetric -> same kernel as its input gradient
-        sums_v = _f(96, dev=dev)
-        L.skd_bn2d_reduce(B, C, H * W, _p(t.x), *t.xs, _p(t.mean), _p(t.rstd), _p(vdir), None, Cp, _p(sums_v), _p(ws["bn"]), st)
-        L.skd_bn2d_jacobian(B, C, H * W, _p(t.x), *t.xs, _p(t.mean), _p(t.rstd), _p(bn.weight), _p(vdir), Cp, _p(sums_v), _p(t.h0[B:]),
-                            H * W * Cp, 1, Cp, Cp, _p(t.h0_lo[B:]) if self.precise else None, st)
+        # ---- tangent forward along v: the preprocessing's Jacobian is symmetric (BN) or diagonal (tanh / rescale) -> same kernel as
+        # its input gradient
+        sums_v = None
+        if mode == 1:
+            bn = D.preprocess_additional
+            sums_v = _f(96, dev=dev)
+            L.skd_bn2d_reduce(B, C, H * W, _p(t.x), *t.xs, _p(t.mean), _p(t.rstd), _p(vdir), None, Cp, _p(sums_v), _p(ws["bn"]), st)
+            L.skd_bn2d_jacobian(B, C, H * W, _p(t.x), *t.xs, _p(t.mean), _p(t.rstd), _p(bn.weight), _p(vdir), Cp, _p(sums_v), _p(t.h0[B:]),
+                                H * W * Cp, 1, Cp, Cp, _p(t.h0_lo[B:]) if self.precise else None, st)
+        else:
+            self._prep_jacobian(t, vdir, True, out=t.h0[B:], out_lo=t.h0_lo[B:])
         hin, hin_lo, (hc, wc) = t.h0[B:], t.h0_lo[B:], t.dims[0]
         for li, (lay, s) in enumerate(zip(t.prep["layers"], t.sn)):
             oh, ow = t.dims[li + 1]
@@ -468,8 +502,10 @@ class DiscEngine:
         top_li = len(t.prep["layers"]) - 1
         if top_li in t.att:
             t.att[top_li]["primal_adj_zero"] = True
-        gh0 = self._reverse_layers(t, g, True, sink, True, need_input_adj=True)
-        self._reverse_bn(t, gh0, True, sink, True, False, sums_v=sums_v, vdir=vdir)
+        # modes 2 / 3: x is detached (CriterionAdditionalGP), so the pointwise map adds no parameter and no second-order term and the
+        # joint pass stops at layer 1's weight gradient
+        gh0 = self._reverse_layers(t, g, True, sink, True, need_input_adj=mode == 1)
+        self._reverse_prep(t, gh0, True, sink, True, False, sums_v=sums_v, vdir=vdir)
         if top_li in t.att:
             t.att[top_li].pop("primal_adj_zero", None)
 

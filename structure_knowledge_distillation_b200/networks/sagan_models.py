@@ -9,6 +9,11 @@ The modules below are parameter containers with the reference's names; `Discrimi
     forward() then fails): l4 is always built, and the 4x4 "last" conv uses the top-left window of its kernel when the map it
     sees is smaller than 4x4 (360x480 crops -> 46x61 logits -> 2x3 map; SURVEY.md §8-f2).  With 65-pixel logits the
     behaviour is the reference's.
+
+All three input modes of the reference (`preprocess_GAN_mode`, sagan_models.py:147-154) train, WGAN-GP included: 1 =
+BatchNorm2d with batch statistics (default), 2 = tanh, 3 = 2 * (x / 255 - 0.5).  Modes 2 and 3 hold no parameters or buffers, so
+their state dict and parameter list are the reference's (no `preprocess_additional.*` entries) and train() / eval() do not
+change them; mode 3 keeps the reference's lambda as the module attribute.
 """
 import torch
 import torch.nn as nn
