@@ -215,6 +215,15 @@ void skd_set_conv_im2col(int on);      /* 1 (default): TMA im2col-mode M tiles f
 void skd_set_conv_tile_m(int mode);    /* wgmma conv M tile: 0 (default) 256 rows for long-K launches with Cout > 128 that fill waves as
                                           well as 128 rows do; 1 always 128; 2 256 wherever that path can run (flat / im2col, Cout > 64,
                                           TF32, no split-K, register epilogue, an output tensor) */
+/* two frozen bottleneck 1x1 convolutions in one launch, over P pixel rows:
+     y3 = relu(conv1x1(x3, w3) * scale3 + shift3 + residual)   w3 [Cout3][Cin3], y3 may be the residual itself
+     y1 = relu(conv1x1(y3, w1) * scale1 + shift1)              w1 [Cout1][Cout3]
+   both bit for bit what two skd_conv2d_fwd_sm100 launches compute.  Cout3 % 64 == 0, Cout1 in {64, 128, 256} */
+int skd_conv1x1_chain_sm100(int P, int Cin3, int Cout3, int Cout1, const float* x3, int ldx3, const float* w3, const float* scale3,
+                            const float* shift3, const float* residual, int ldr, float* y3, int ldy3, const float* w1,
+                            const float* scale1, const float* shift1, float* y1, int ldy1, cudaStream_t);
+void skd_set_conv_chain(int mode);     /* frozen bottlenecks: 0 (default) chain conv3 with the next block's conv1 where the shapes allow; 1 never */
+int skd_conv_chain_mode(void);
 
 /* ---- E. pooling / resampling / optimiser ---- */
 int skd_pool_out_size_ceil(int in, int k, int s, int p);

@@ -549,12 +549,293 @@ int launch_n(bool split3, bool tma_epi, const CUtensorMap& tx, const CUtensorMap
   return launch<kBlockM, BLOCK_N, false, false>(tx, tw, tx2, tw2, tr, ty, a, st);
 }
 
+// ---------------------------------------------------------------------------------------------------
+// Chained bottleneck 1x1 pair (frozen teacher): block i's conv3 and block i+1's conv1 in one launch.
+//   y3 = relu(conv1x1(x3, w3) * scale3 + shift3 + residual)       (Cin3 -> Cout3; y3 may be the residual itself)
+//   y1 = relu(conv1x1(y3, w1) * scale1 + shift1)                   (Cout3 -> Cout1 <= 256)
+// Per flat 128-pixel tile the consumers walk conv3's output channels in chunks of kChainBN3: the conv3 K loop, the TMA epilogue of
+// conv_fwd_sm90_kernel (residual loaded into a tile buffer by thread 32, the same float operations, a TMA store of the 64 rows of the
+// warpgroup), and the finished values -- rounded as the TFLOAT32 tensor map of the unfused conv1 would round them -- into a K-major
+// SWIZZLE_128B staging buffer that is conv1's A operand for the chunk's 64 channels of K.  conv1's weights stream through the
+// operand ring after the chunk's conv3 stages.  conv1's accumulators stay in registers across the chunks; its register epilogue
+// runs after the last one.  Both outputs equal the two unfused launches bit for bit: the same k8 wgmma sequences per element
+// (conv1's K in ascending 32-channel chunks, m64n128 per 128 output channels as the unfused BLOCK_N 128 tiles), and the same
+// epilogue arithmetic.  What it saves is reading y3 back from HBM and one launch per bottleneck.
+// ---------------------------------------------------------------------------------------------------
+constexpr int kChainBN3 = 64;                    // conv3 output channels per chunk = conv1 K per chunk
+
+struct ChainArgs {
+  int P, Cin3, Cout3;
+  const float* scale3; const float* shift3;
+  const float* scale1; const float* shift1;
+  float* y1; int ldy1;
+  int round_stage;                               // 1: conv1 operand rounded to nearest TF32 (the TFLOAT32 operand maps); 0: raw fp32
+  int nstages;
+};
+
+template <int COUT1>
+struct ChainCfg {
+  static_assert(COUT1 == 64 || COUT1 == 128 || COUT1 == 256, "conv1 output channels: 64, 128 or 256");
+  static constexpr int kN1 = COUT1 > 128 ? 128 : COUT1;        // conv1 wgmma width: the unfused launch's BLOCK_N
+  static constexpr int kNT1 = COUT1 / kN1;                     // conv1 accumulators per consumer thread
+  static constexpr int kA3Bytes = kBlockM * kBlockK * 4;
+  static constexpr int kB3Bytes = kChainBN3 * kBlockK * 4;
+  static constexpr int kB1Bytes = COUT1 * kBlockK * 4;
+  static constexpr int kStageBytes = kA3Bytes + kB3Bytes > kB1Bytes ? kA3Bytes + kB3Bytes : kB1Bytes;
+  static constexpr int kTileBytes = kBlockM * kChainBN3 * 4;   // one residual / output tile buffer, and the staging buffer
+  static constexpr int kEpiBufs = 2;
+  static constexpr int kFixedBytes = 1024 /*align slack*/ + 256 /*barriers*/;
+  static constexpr int kFit = (232448 - kFixedBytes - (kEpiBufs + 1) * kTileBytes) / kStageBytes;
+  static constexpr int kStages = kFit > 8 ? 8 : kFit;
+  static constexpr int kSmemBytes = kStages * kStageBytes + (kEpiBufs + 1) * kTileBytes + kFixedBytes;
+  static_assert(kStages >= 3, "operand ring");
+  static_assert(2 * (kStages + kEpiBufs) * 8 <= 256, "barriers");
+  static_assert(kSmemBytes <= 232448, "exceeds the 227 KB of shared memory a CTA may use");
+};
+
+template <int COUT1>
+__global__ void __launch_bounds__(kThreads, 1)
+conv1x1_chain_sm90_kernel(const __grid_constant__ CUtensorMap tmap_x3, const __grid_constant__ CUtensorMap tmap_w3,
+                          const __grid_constant__ CUtensorMap tmap_w1, const __grid_constant__ CUtensorMap tmap_r,
+                          const __grid_constant__ CUtensorMap tmap_y3, const ChainArgs a) {
+  using C = ChainCfg<COUT1>;
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  const uint32_t raw_addr = ptx::smem_u32(smem_raw);
+  uint8_t* smem = smem_raw + (((raw_addr + 1023u) & ~1023u) - raw_addr);
+  uint8_t* epi_smem = smem + C::kStages * C::kStageBytes;
+  uint8_t* stg_smem = epi_smem + C::kEpiBufs * C::kTileBytes;
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(stg_smem + C::kTileBytes);
+  uint64_t* empty_bar = full_bar + C::kStages;
+  uint64_t* epi_full = empty_bar + C::kStages;
+  uint64_t* epi_empty = epi_full + C::kEpiBufs;
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (threadIdx.x == 0) {
+    ptx::prefetch_tmap(&tmap_x3);
+    ptx::prefetch_tmap(&tmap_w3);
+    ptx::prefetch_tmap(&tmap_w1);
+    ptx::prefetch_tmap(&tmap_r);
+    ptx::prefetch_tmap(&tmap_y3);
+    for (int s = 0; s < C::kStages; ++s) { ptx::mbar_init(&full_bar[s], 1); ptx::mbar_init(&empty_bar[s], 8); }
+    for (int b = 0; b < C::kEpiBufs; ++b) { ptx::mbar_init(&epi_full[b], 1); ptx::mbar_init(&epi_empty[b], 2); }
+    ptx::fence_barrier_init();
+  }
+  __syncthreads();
+
+  const int m_tiles = (a.P + kBlockM - 1) / kBlockM;
+  const int chunks = a.Cout3 / kChainBN3;
+  const int k3 = (a.Cin3 + kBlockK - 1) / kBlockK;
+  constexpr int k1 = kChainBN3 / kBlockK;
+
+  if (warp < 4) {
+    ptx::setmaxnreg_dec<kProducerRegs>();
+    if (threadIdx.x == 0) {
+      // operand producer: per chunk, k3 stages of {x3 box, w3 box}, then k1 stages of one w1 box (all conv1 output channels)
+      int stage = 0; uint32_t phase = 0;
+      for (int mt = blockIdx.x; mt < m_tiles; mt += gridDim.x) {
+        for (int c = 0; c < chunks; ++c) {
+          for (int k = 0; k < k3; ++k) {
+            ptx::mbar_wait(&empty_bar[stage], phase ^ 1);
+            uint8_t* sa = smem + stage * C::kStageBytes;
+            ptx::mbar_expect_tx(&full_bar[stage], C::kA3Bytes + C::kB3Bytes);
+            ptx::tma_load_2d(sa, &tmap_x3, &full_bar[stage], k * kBlockK, mt * kBlockM);
+            ptx::tma_load_2d(sa + C::kA3Bytes, &tmap_w3, &full_bar[stage], k * kBlockK, c * kChainBN3);
+            if (++stage == a.nstages) { stage = 0; phase ^= 1; }
+          }
+          for (int k = 0; k < k1; ++k) {
+            ptx::mbar_wait(&empty_bar[stage], phase ^ 1);
+            ptx::mbar_expect_tx(&full_bar[stage], C::kB1Bytes);
+            ptx::tma_load_2d(smem + stage * C::kStageBytes, &tmap_w1, &full_bar[stage], (c * k1 + k) * kBlockK, 0);
+            if (++stage == a.nstages) { stage = 0; phase ^= 1; }
+          }
+        }
+      }
+    }
+    if (threadIdx.x == 32) {
+      // residual loader: one tile buffer per chunk, 32-channel x 64-row boxes; a 64-row half wholly past P is not loaded
+      int eb = 0; uint32_t ephase = 0;
+      for (int mt = blockIdx.x; mt < m_tiles; mt += gridDim.x) {
+        const uint32_t bytes = (mt * kBlockM + 64 < a.P ? 2 : 1) * k1 * kEpiBoxBytes;
+        for (int c = 0; c < chunks; ++c) {
+          ptx::mbar_wait(&epi_empty[eb], ephase ^ 1);
+          ptx::mbar_expect_tx(&epi_full[eb], bytes);
+          uint8_t* buf = epi_smem + eb * C::kTileBytes;
+          for (int h = 0; h < 2; ++h)
+            for (int j = 0; j < k1; ++j)
+              if (mt * kBlockM + 64 * h < a.P)
+                ptx::tma_load_2d(buf + (h * k1 + j) * kEpiBoxBytes, &tmap_r, &epi_full[eb], c * kChainBN3 + kBlockK * j, mt * kBlockM + 64 * h);
+          if (++eb == C::kEpiBufs) { eb = 0; ephase ^= 1; }
+        }
+      }
+    }
+  } else {
+    ptx::setmaxnreg_inc<kConsumerRegs>();
+    constexpr int N1 = C::kN1, NT1 = C::kNT1;
+    const int g = (warp >> 2) - 1;
+    const int wq = warp & 3;
+    const int r_lo = g * 64 + wq * 16 + (lane >> 2);
+    const int cq = 2 * (lane & 3);
+    float acc1[NT1][N1 / 2];
+    float acc3[kChainBN3 / 2];
+    int stage = 0; uint32_t phase = 0;
+    int eb = 0; uint32_t ephase = 0;
+    bool first_chunk = true;
+    const bool epi_leader = (threadIdx.x & 127) == 0;
+    // the warpgroup's 64 rows of the staging buffer: conv1's A operand, boxes of 32 channels as in the tile buffers
+    uint8_t* stg = stg_smem + g * (C::kTileBytes / 2);
+    const uint32_t stg_addr = ptx::smem_u32(stg);
+    const uint32_t frag = (uint32_t)((wq * 16 + (lane >> 2)) * 128 + (cq & 3) * 4);
+    auto at = [&](uint8_t* half, int h, int j) -> float2* {     // fragment position (row half h, column group j), SWIZZLE_128B
+      return reinterpret_cast<float2*>(half + (j >> 2) * kEpiBoxBytes + frag + h * 8 * 128 + ((((j & 3) * 2 + (cq >> 2)) ^ (lane >> 2)) << 4));
+    };
+    float t[N1 / 4];
+    auto gather = [&](const float* p, int c0, int n) {
+#pragma unroll
+      for (int j = 0; j < n / 8; ++j) { t[2 * j] = __ldg(p + c0 + 8 * j); t[2 * j + 1] = __ldg(p + c0 + 8 * j + 1); }
+    };
+    for (int mt = blockIdx.x; mt < m_tiles; mt += gridDim.x) {
+      int prev_stage = -1;
+      auto release_prev = [&]() {
+        if (prev_stage >= 0 && lane == 0) ptx::mbar_arrive(&empty_bar[prev_stage]);
+      };
+      for (int c = 0; c < chunks; ++c) {
+        // ---- conv3, output channels c*64 .. c*64+63 ----
+        for (int k = 0; k < k3; ++k) {
+          ptx::mbar_wait(&full_bar[stage], phase);
+          const uint32_t base = ptx::smem_u32(smem + stage * C::kStageBytes);
+          const uint32_t sa = base + (uint32_t)(g * 64 * 128), sb = base + (uint32_t)C::kA3Bytes;
+          ptx::wgmma_fence();
+#pragma unroll
+          for (int kk = 0; kk < kBlockK / kWgmmaK; ++kk)
+            ptx::wgmma_tf32<kChainBN3>(acc3, ptx::make_wgmma_desc_sw128(sa + kk * kWgmmaK * 4), ptx::make_wgmma_desc_sw128(sb + kk * kWgmmaK * 4),
+                                      (k | kk) != 0 ? 1u : 0u);
+          ptx::wgmma_commit();
+          ptx::wgmma_wait<1>();
+          release_prev();
+          prev_stage = stage;
+          if (++stage == a.nstages) { stage = 0; phase ^= 1; }
+        }
+        ptx::wgmma_wait<0>();
+        ptx::fence_regs(acc3);
+#pragma unroll
+        for (int n = 0; n < NT1; ++n) ptx::fence_regs(acc1[n]);
+        release_prev();
+        prev_stage = -1;
+
+        // ---- conv3 epilogue: scale, shift, residual, ReLU (conv_fwd_sm90_kernel's TMA epilogue, BLOCK_N 64) ----
+        const int c0 = c * kChainBN3 + cq;
+        gather(a.scale3, c0, kChainBN3);
+#pragma unroll
+        for (int i = 0; i < kChainBN3 / 2; ++i) acc3[i] = __fmul_rn(acc3[i], t[(i >> 2) * 2 + (i & 1)]);
+        gather(a.shift3, c0, kChainBN3);
+#pragma unroll
+        for (int i = 0; i < kChainBN3 / 2; ++i) acc3[i] = __fadd_rn(acc3[i], t[(i >> 2) * 2 + (i & 1)]);
+        uint8_t* half = epi_smem + eb * C::kTileBytes + g * (C::kTileBytes / 2);
+        if (epi_leader && !first_chunk) {                       // the previous chunk's stores have read their buffer
+          ptx::bulk_wait_group_read<0>();
+          ptx::mbar_arrive(&epi_empty[eb == 0 ? C::kEpiBufs - 1 : eb - 1]);
+        }
+        first_chunk = false;
+        ptx::mbar_wait(&epi_full[eb], ephase);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+#pragma unroll
+          for (int j = 0; j < kChainBN3 / 8; ++j) {
+            const float2 r = *at(half, h, j);
+            float v0 = __fadd_rn(acc3[4 * j + 2 * h], r.x), v1 = __fadd_rn(acc3[4 * j + 2 * h + 1], r.y);
+            v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f);
+            *at(half, h, j) = make_float2(v0, v1);
+            if (a.round_stage) { v0 = ptx::round_tf32(v0); v1 = ptx::round_tf32(v1); }
+            *at(stg, h, j) = make_float2(v0, v1);
+          }
+        }
+        // the tile buffer goes to the TMA store and the staging buffer to the tensor core: both read through the async proxy
+        ptx::fence_proxy_async();
+        ptx::named_bar_sync(1 + g, 128);
+        if (epi_leader) {
+          const int row0 = mt * kBlockM + 64 * g;
+          if (row0 < a.P)
+            for (int j = 0; j < k1; ++j) ptx::tma_store_2d(&tmap_y3, half + j * kEpiBoxBytes, c * kChainBN3 + kBlockK * j, row0);
+          ptx::bulk_commit_group();
+        }
+        if (++eb == C::kEpiBufs) { eb = 0; ephase ^= 1; }
+
+        // ---- conv1, K = channels c*64 .. c*64+63 of y3, from the staging buffer ----
+        for (int kb = 0; kb < k1; ++kb) {
+          ptx::mbar_wait(&full_bar[stage], phase);
+          const uint32_t sb = ptx::smem_u32(smem + stage * C::kStageBytes);
+          ptx::wgmma_fence();
+#pragma unroll
+          for (int kk = 0; kk < kBlockK / kWgmmaK; ++kk) {
+            const uint64_t da = ptx::make_wgmma_desc_sw128(stg_addr + kb * kEpiBoxBytes + kk * kWgmmaK * 4);
+#pragma unroll
+            for (int n = 0; n < NT1; ++n)
+              ptx::wgmma_tf32<N1>(acc1[n], da, ptx::make_wgmma_desc_sw128(sb + n * N1 * 128 + kk * kWgmmaK * 4), (c | kb | kk) != 0 ? 1u : 0u);
+          }
+          ptx::wgmma_commit();
+          ptx::wgmma_wait<1>();
+          release_prev();
+          prev_stage = stage;
+          if (++stage == a.nstages) { stage = 0; phase ^= 1; }
+        }
+      }
+      ptx::wgmma_wait<0>();
+#pragma unroll
+      for (int n = 0; n < NT1; ++n) ptx::fence_regs(acc1[n]);
+      release_prev();
+
+      // ---- conv1 epilogue: scale, shift, ReLU, stores (conv_fwd_sm90_kernel's register epilogue) ----
+#pragma unroll
+      for (int n = 0; n < NT1; ++n) {
+        const int c0 = n * N1 + cq;
+        gather(a.scale1, c0, N1);
+#pragma unroll
+        for (int i = 0; i < N1 / 2; ++i) acc1[n][i] = __fmul_rn(acc1[n][i], t[(i >> 2) * 2 + (i & 1)]);
+        gather(a.shift1, c0, N1);
+#pragma unroll
+        for (int i = 0; i < N1 / 2; ++i) acc1[n][i] = __fadd_rn(acc1[n][i], t[(i >> 2) * 2 + (i & 1)]);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int row = mt * kBlockM + r_lo + 8 * h;
+          if (row >= a.P) continue;
+          float* y = a.y1 + (size_t)row * a.ldy1 + c0;
+#pragma unroll
+          for (int j = 0; j < N1 / 8; ++j)
+            *reinterpret_cast<float2*>(y + 8 * j) = make_float2(fmaxf(acc1[n][4 * j + 2 * h], 0.f), fmaxf(acc1[n][4 * j + 2 * h + 1], 0.f));
+        }
+      }
+    }
+    if (epi_leader) ptx::bulk_wait_group<0>();
+  }
+}
+
+template <int COUT1>
+int launch_chain(const CUtensorMap& tx3, const CUtensorMap& tw3, const CUtensorMap& tw1, const CUtensorMap& tr, const CUtensorMap& ty3,
+                 const ChainArgs& a_in, cudaStream_t st) {
+  using C = ChainCfg<COUT1>;
+  ChainArgs a = a_in;
+  a.nstages = C::kStages;
+  static bool attr = false;
+  if (!attr) {
+    cudaError_t e = cudaFuncSetAttribute(conv1x1_chain_sm90_kernel<COUT1>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::kSmemBytes);
+    if (e != cudaSuccess) { set_error("skd_conv1x1_chain_sm100(attr)", e); return 0; }
+    attr = true;
+  }
+  const int m_tiles = (a.P + kBlockM - 1) / kBlockM;
+  conv1x1_chain_sm90_kernel<COUT1><<<m_tiles < kNumSMs ? m_tiles : kNumSMs, kThreads, C::kSmemBytes, st>>>(tx3, tw3, tw1, tr, ty3, a);
+  return finish("skd_conv1x1_chain_sm100");
+}
+
+int g_conv_chain = 0;              // 0: frozen bottlenecks chain conv3 into the next block's conv1; 1: never
+
 }  // namespace
 
 extern "C" void skd_set_conv_im2col(int on) { g_conv_im2col = on ? 1 : 0; }
 extern "C" void skd_set_conv_tile_order(int mode) { g_tile_order = mode; g_tile_flip = 0; }
 extern "C" void skd_set_conv_k_order(int mode) { g_k_order = mode; }
 extern "C" void skd_set_conv_tile_m(int mode) { g_tile_m = mode; }
+extern "C" void skd_set_conv_chain(int mode) { g_conv_chain = mode; }
+extern "C" int skd_conv_chain_mode(void) { return g_conv_chain; }
 
 // ---- split-K for convolutions with few output tiles and a long K loop (the discriminator: 256 .. 4096 output pixels, K up to 4096) ----
 // Without it a 4x8-pixel map at batch 8 is 2 x 2 tiles: 4 of 132 SMs walk 128 K steps each.  Units = tiles x K ranges fill the
@@ -821,4 +1102,45 @@ extern "C" int skd_conv2d_fwd_sm100_splitk(int N, int H, int W, int Cin, int Cou
   if (workspace && (reinterpret_cast<uintptr_t>(workspace) & 15)) { set_error_msg("skd_conv2d_fwd_sm100_splitk", "workspace not 16-byte aligned"); return 0; }
   return conv_fwd_impl(N, H, W, Cin, Cout, KH, KW, stride, pad, dil, x, x_lo, ldx, w, w_lo, y, ldy, (long long)OW * ldy, (long long)OH * OW * ldy,
                        out_h, out_w, nullptr, 0, scale, shift, residual, ldr, act, slope, 0, st, workspace, workspace_floats);
+}
+
+// Chained frozen-bottleneck pair (conv1x1_chain_sm90_kernel): y3 = relu(x3 * w3 * scale3 + shift3 + residual) over P pixel rows
+// (y3 may be the residual), then y1 = relu(y3 * w1 * scale1 + shift1) in the same launch.
+extern "C" int skd_conv1x1_chain_sm100(int P, int Cin3, int Cout3, int Cout1, const float* x3, int ldx3, const float* w3, const float* scale3,
+                                       const float* shift3, const float* residual, int ldr, float* y3, int ldy3, const float* w1,
+                                       const float* scale1, const float* shift1, float* y1, int ldy1, cudaStream_t st) {
+  const char* who = "skd_conv1x1_chain_sm100";
+  if (P <= 0) return 1;
+  if (Cin3 % 4 || Cout3 % kChainBN3 || !(Cout1 == 64 || Cout1 == 128 || Cout1 == 256) || ldx3 % 4 || ldr % 4 || ldy3 % 4 || ldy1 % 2) {
+    set_error_msg(who, "Cin3 and the pitches must be multiples of 4 floats, Cout3 a multiple of 64, Cout1 64, 128 or 256");
+    return 0;
+  }
+  if ((reinterpret_cast<uintptr_t>(x3) | reinterpret_cast<uintptr_t>(w3) | reinterpret_cast<uintptr_t>(residual) | reinterpret_cast<uintptr_t>(y3) |
+       reinterpret_cast<uintptr_t>(w1)) & 15 || (reinterpret_cast<uintptr_t>(y1) & 7) || !scale3 || !shift3 || !scale1 || !shift1) {
+    set_error_msg(who, "operands 16-byte aligned (y1 8-byte), scale and shift of both convolutions required");
+    return 0;
+  }
+  auto rows = [&](CUtensorMap* m, CUtensorMapDataType type, const float* ptr, int cols, int nrows, int ld, int box_rows) -> bool {
+    cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)nrows};
+    cuuint64_t strides[1] = {(cuuint64_t)ld * 4};
+    cuuint32_t box[2] = {(cuuint32_t)kBlockK, (cuuint32_t)box_rows};
+    cuuint32_t estr[2] = {1, 1};
+    return encode(m, type, 2, ptr, dims, strides, box, estr, who);
+  };
+  CUtensorMap tx3, tw3, tw1, tr, ty3;
+  if (!rows(&tx3, operand_type(), x3, Cin3, P, ldx3, kBlockM) || !rows(&tw3, operand_type(), w3, Cin3, Cout3, Cin3, kChainBN3) ||
+      !rows(&tw1, operand_type(), w1, Cout3, Cout1, Cout3, Cout1) || !rows(&tr, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, residual, Cout3, P, ldr, 64) ||
+      !rows(&ty3, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, y3, Cout3, P, ldy3, 64))
+    return 0;
+  ChainArgs a;
+  a.P = P; a.Cin3 = Cin3; a.Cout3 = Cout3;
+  a.scale3 = scale3; a.shift3 = shift3; a.scale1 = scale1; a.shift1 = shift1;
+  a.y1 = y1; a.ldy1 = ldy1;
+  a.round_stage = g_tf32_tma_type ? 1 : 0;
+  a.nstages = 0;
+  switch (Cout1) {
+    case 64: return launch_chain<64>(tx3, tw3, tw1, tr, ty3, a, st);
+    case 128: return launch_chain<128>(tx3, tw3, tw1, tr, ty3, a, st);
+    default: return launch_chain<256>(tx3, tw3, tw1, tr, ty3, a, st);
+  }
 }

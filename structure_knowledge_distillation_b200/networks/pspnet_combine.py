@@ -122,11 +122,22 @@ class Bottleneck(nn.Module):
         out = self.bn2(self.conv2(out), fuse_relu=True)
         return self.bn3(self.conv3(out), residual=residual, fuse_relu=True)
 
-    def frozen(self, x, out=None):
+    def frozen(self, x, out=None, o1=None, chain=None):
+        """o1: this block's conv1 output, already computed by the previous block's chained launch.  chain: the next block, whose
+        conv1 then runs in the same launch as this block's conv3 (ops.conv1x1_chain) -> (output, the next block's conv1 output)."""
         residual = x if self.downsample is None else self.downsample[0].frozen(x, *_fold(self.downsample[1]))
-        o = self.conv1.frozen(x, *_fold(self.bn1), act="relu")
+        o = o1 if o1 is not None else self.conv1.frozen(x, *_fold(self.bn1), act="relu")
         o = self.conv2.frozen(o, *_fold(self.bn2), act="relu")
+        if chain is not None:
+            return ops.conv1x1_chain(o, ops.weight_ohwi(self.conv3.weight), *_fold(self.bn3), residual,
+                                     ops.weight_ohwi(chain.conv1.weight), *_fold(chain.bn1))
         return self.conv3.frozen(o, *_fold(self.bn3), residual=residual, act="relu", out=out)
+
+    def chains_into(self, nxt):
+        """Whether this block's conv3 and `nxt`'s conv1 can run as one launch: 1x1 pair with no downsample between them and a conv1
+        output the chained kernel's accumulators hold (layer4's 512 channels do not fit)."""
+        return (isinstance(nxt, Bottleneck) and nxt.downsample is None and nxt.conv1.out_channels in ops.CHAIN_COUT1 and
+                self.conv3.out_channels % 64 == 0 and self.conv3.in_channels % 4 == 0)
 
 
 class _Dropout2d(nn.Dropout2d):
@@ -252,9 +263,15 @@ class ResNet(nn.Module):
         x = self.conv3.frozen(x, *_fold(self.bn3), act="relu")
         x, _ = ops.maxpool_fwd(x)
         feats = []
+        chain = ops.conv1x1_chain_enabled()
         for layer in (self.layer1, self.layer2, self.layer3):
-            for blk in layer:
-                x = blk.frozen(x)
+            blocks, o1 = list(layer), None
+            for i, blk in enumerate(blocks):
+                nxt = blocks[i + 1] if i + 1 < len(blocks) else None
+                if chain and isinstance(blk, Bottleneck) and blk.chains_into(nxt):
+                    x, o1 = blk.frozen(x, o1=o1, chain=nxt)
+                else:
+                    x, o1 = (blk.frozen(x, o1=o1) if o1 is not None else blk.frozen(x)), None
             feats.append(x)
         x1, x2, x3 = feats
         bn = self.dsn[1]

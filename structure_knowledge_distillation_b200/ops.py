@@ -200,6 +200,40 @@ def conv2d_fwd(x, w_ohwi, stride, pad, dil, scale=None, shift=None, residual=Non
     return out
 
 
+CHAIN_COUT1 = (64, 128, 256)
+
+
+def conv1x1_chain_enabled():
+    """skd_set_conv_chain: 0 (default) frozen bottlenecks chain conv3 into the next block's conv1, 1 never."""
+    return lib().skd_conv_chain_mode() != 1
+
+
+def conv1x1_chain(x3, w3_ohwi, scale3, shift3, residual, w1_ohwi, scale1, shift1, out3=None):
+    """One launch for a frozen bottleneck's conv3 and the next block's conv1 (both 1x1, folded BN, ReLU):
+    y3 = relu(conv(x3, w3) * scale3 + shift3 + residual), y1 = relu(conv(y3, w1) * scale1 + shift1) -> (y3, y1), each equal bit for
+    bit to its conv2d_fwd.  out3 may be the residual."""
+    _f32(x3, w3_ohwi, residual, w1_ohwi)
+    n, cin3, h, w, ldx = nhwc_meta(x3)
+    cout3, cout1 = w3_ohwi.shape[0], w1_ohwi.shape[0]
+    assert w3_ohwi.shape == (cout3, 1, 1, cin3) and w1_ohwi.shape == (cout1, 1, 1, cout3)
+    assert w3_ohwi.is_contiguous() and w1_ohwi.is_contiguous()
+    if out3 is None:
+        out3 = empty_nhwc(n, cout3, h, w, x3.device)
+    assert nhwc_meta(out3)[:4] == (n, cout3, h, w) and nhwc_meta(residual)[:4] == (n, cout3, h, w)
+    out1 = empty_nhwc(n, cout1, h, w, x3.device)
+    log = CONV_EVENT_LOG
+    if log is not None:
+        ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        ev0.record()
+    lib().skd_conv1x1_chain_sm100(n * h * w, cin3, cout3, cout1, _p(x3), ldx, _p(w3_ohwi), _p(scale3), _p(shift3), _p(residual),
+                                  nhwc_meta(residual)[4], _p(out3), nhwc_meta(out3)[4], _p(w1_ohwi), _p(scale1), _p(shift1), _p(out1),
+                                  cout1, _st())
+    if log is not None:
+        ev1.record()
+        log.append((ev0, ev1, 2.0 * n * h * w * cout3 * (cin3 + cout1), ("fwd", n, cin3, h, w, cout3, "chain1x1->%d" % cout1)))
+    return out3, out1
+
+
 def lo_tf32(t):
     """dense tensor -> lo = rna_tf32(t - rna_tf32(t)), same layout (the hi part is what a TFLOAT32 tensor map makes of t itself)."""
     lo = torch.empty_strided(t.shape, t.stride(), device=t.device, dtype=torch.float32)
