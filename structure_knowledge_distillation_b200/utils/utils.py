@@ -104,6 +104,38 @@ def load_S_model(args, model, with_module=True):
     return None
 
 
+def load_seg_model(args, model, with_module=True):
+    """A network trained by SegModel: ImageNet initialisation by key intersection (`fc.*` and every other key the network lacks is
+    dropped, as load_S_model does) when `is_load_imgnet`, else resume from `<ckpt_path>/model_best.pth.tar` when `resume` -- restoring
+    last_step / start_epoch / best_mean_IU into `args`.  -> 'imagenet', 'resume' or None."""
+    ckpt_dir = getattr(args, "ckpt_path", "")
+    if getattr(args, "is_load_imgnet", False):
+        path = str(getattr(args, "pretrain_model_imgnet", ""))
+        if os.path.isfile(path):
+            saved = _torch_load(path)
+            new = model.state_dict()
+            hit = {k: v for k, v in saved.items() if k in new}
+            new.update(hit)
+            model.load_state_dict(new)
+            logging.info("=> load %s: %d of %d tensors (%d of the network's %d)", path, len(hit), len(saved), len(hit), len(new))
+            return "imagenet"
+        logging.info("=> the pretrain model on imgnet '{}' does not exit".format(path))
+        return None
+    if getattr(args, "resume", False) and ckpt_dir:
+        file = ckpt_dir + '/model_best.pth.tar'
+        if os.path.isfile(file):
+            ck = _torch_load(file)
+            args.last_step = ck.get('step')
+            args.start_epoch = ck.get('epoch')
+            args.best_mean_IU = ck.get('best_mean_IU')
+            model.load_state_dict(_strip_module(ck['state_dict'], with_module))
+            logging.info("=> loaded checkpoint '{}' (epoch:{} step:{} best_mean_IU:{})".format(file, args.start_epoch, args.last_step,
+                                                                                              args.best_mean_IU))
+            return "resume"
+        logging.info("=> checkpoint '{}' does not exit".format(file))
+    return None
+
+
 def load_D_model(args, model, with_module=True):
     """utils/utils.py:129-151."""
     ckpt_dir = getattr(args, "D_ckpt_path", "")
