@@ -101,6 +101,18 @@ int skd_dsn_ce_fwd_train(int N, int C, int h, int w, int H, int W, const float* 
 int skd_dsn_ce_bwd_cols(int N, int C, int h, int w, int H, const float* rows_ws, long long a_sn, long long a_sc, long long a_sp,
                         long long b_sn, long long b_sc, long long b_sp, int heads, float w0, float w1, const float* grad_out,
                         const float* count, float* d0, float* d1, cudaStream_t);
+/* Class-weighted forms (CrossEntropyLoss(weight=class_weight, ignore_index) per head): class_weight is a device array of C floats;
+   loss = w0 * sum_i cw[y_i] nll0_i / sum_i cw[y_i] + w1 * sum_i cw[y_i] nll1_i / sum_i cw[y_i] over the pixels whose label is
+   not ignore_index, and count receives sum_i cw[y_i].  The backward of the training forward is skd_dsn_ce_bwd_cols.
+   A label outside [0, C) that is not ignore_index does not index the table: its weight is 0.
+   If sum_i cw[y_i] = 0 (every label ignored, or every present class weighted 0) the loss is NaN and the gradient 0. */
+int skd_dsn_ce_fwd_weighted(int N, int C, int h, int w, int H, int W, const float* L0, long long a_sn, long long a_sc, long long a_sp,
+                            const float* L1, long long b_sn, long long b_sc, long long b_sp, const long long* labels, int ignore_index,
+                            float w0, float w1, float* loss, float* count, double* workspace, const float* class_weight, cudaStream_t);
+int skd_dsn_ce_fwd_train_weighted(int N, int C, int h, int w, int H, int W, const float* logits0, long long a_sn, long long a_sc,
+                                  long long a_sp, const float* logits1, long long b_sn, long long b_sc, long long b_sp,
+                                  const long long* labels, int ignore_index, float w0, float w1, float* loss, float* count,
+                                  double* partials, float* rows_ws, const float* class_weight, cudaStream_t);
 /* OhemCrossEntropy2d / CriterionOhemDSN (utils/criterion.py:11-90, 190-209), with no host round trip.
    skd_ohem_grid_sample replaces find_threshold's scipy zooms (criterion.py:20-35): for every point of the gh x gw grid (Python
    round(H / factor), round(W / factor)) it writes the zoomed probability of the zoomed label (+inf where that label is

@@ -167,10 +167,19 @@ __device__ __forceinline__ float up_logits(const float* __restrict__ L, Strides 
   return m + __logf(z);
 }
 
+// class weight of a kept label: the table entry, 0 for a label outside [0, C) (it must not index the table)
+__device__ __forceinline__ float class_weight_of(const float* __restrict__ cw, long long lab, int C) {
+  return (lab >= 0 && lab < C) ? __ldg(cw + lab) : 0.f;
+}
+
+// WEIGHTED (CrossEntropyLoss(weight=...)): a kept pixel's loss is multiplied by cw[label] and its count partial is cw[label], so
+// the finalised loss is sum w*nll / sum w (both heads share that denominator)
+template <bool WEIGHTED = false>
 __global__ void __launch_bounds__(256)
 dsn_ce_fwd_kernel(const float* __restrict__ L0, const float* __restrict__ L1, Strides s0, Strides s1,
                   const long long* __restrict__ labels, int N, int C, int h, int w, int H, int W, int ignore, float w0,
-                  float w1, double* __restrict__ part_loss, double* __restrict__ part_cnt) {
+                  float w1, double* __restrict__ part_loss, double* __restrict__ part_cnt,
+                  const float* __restrict__ class_weight = nullptr) {
   __shared__ double sh[32];
   const float sy = H > 1 ? (float)(h - 1) / (float)(H - 1) : 0.f, sx = W > 1 ? (float)(w - 1) / (float)(W - 1) : 0.f;
   double acc = 0.0, cnt = 0.0;
@@ -192,7 +201,12 @@ dsn_ce_fwd_kernel(const float* __restrict__ L0, const float* __restrict__ L1, St
       for (int c = 0; c < kMaxClasses; ++c) if (c == (int)lab) pick = v[c];
       loss += w1 * (lse - pick);
     }
-    acc += (double)loss; cnt += 1.0;
+    if (WEIGHTED) {
+      const float cw = class_weight_of(class_weight, lab, C);
+      acc += (double)cw * (double)loss; cnt += (double)cw;
+    } else {
+      acc += (double)loss; cnt += 1.0;
+    }
   }
   double t = block_sum_d(acc, sh);
   double u = block_sum_d(cnt, sh);
@@ -214,13 +228,16 @@ dsn_ce_fwd_kernel(const float* __restrict__ L0, const float* __restrict__ L1, St
 // OHEM = true (OhemCrossEntropy2d, utils/criterion.py:65-90): head 0 keeps a valid pixel only when its softmax probability of the
 // label is <= *ohem_thr (the device threshold of ohem.cu); dropped pixels contribute neither loss, gradient nor count.  Each head
 // then writes its own count partials (the two heads have different denominators).
+// WEIGHTED = true (class-weighted CE, LOSS only): a kept pixel's G row and loss are multiplied by class_weight[label] and its count
+// partial is that weight; the column phase then divides by the sum of the weights.
 constexpr int kRowsThreads = 512;
-template <bool LOSS, int CT, bool OHEM = false>
+template <bool LOSS, int CT, bool OHEM = false, bool WEIGHTED = false>
 __global__ void __launch_bounds__(kRowsThreads, 2)
 dsn_ce_bwd_rows_kernel(const float* __restrict__ L0, const float* __restrict__ L1, Strides s0, Strides s1,
                        const long long* __restrict__ labels, int N, int C, int h, int w, int H, int W, int ignore,
                        float* __restrict__ T1, int chunk, double* __restrict__ part_loss, double* __restrict__ part_cnt, float w0, float w1,
-                       const float* __restrict__ ohem_thr = nullptr) {
+                       const float* __restrict__ ohem_thr = nullptr, const float* __restrict__ class_weight = nullptr) {
+  static_assert(!(WEIGHTED && (OHEM || !LOSS)), "class weights are a training-forward option without OHEM");
   __shared__ double shd[32];
   double loss_acc = 0.0, cnt_acc = 0.0;
   extern __shared__ float G[];                                 // [C][chunk|1], wa[chunk], wb[chunk], first[w+2], row[w][C]
@@ -283,7 +300,15 @@ dsn_ce_bwd_rows_kernel(const float* __restrict__ L0, const float* __restrict__ L
           for (int c = 0; c < CT; ++c) if (c == (int)lab) e = v[c];
           keep = e * rz <= thr;
         }
-        if (keep) {
+        if (WEIGHTED) {
+          const float cw = class_weight_of(class_weight, lab, C);
+#pragma unroll
+          for (int c = 0; c < CT; ++c) if (c < C) {
+            const float g = v[c] * rz - (c == (int)lab ? 1.f : 0.f);
+            G[c * pitch + j] = g * cw;
+          }
+          loss_acc += (double)cw * (double)(m + __logf(z) - pick); cnt_acc += (double)cw;
+        } else if (keep) {
 #pragma unroll
           for (int c = 0; c < CT; ++c) if (c < C) G[c * pitch + j] = v[c] * rz - (c == (int)lab ? 1.f : 0.f);
           if (LOSS) { loss_acc += (double)(m + __logf(z) - pick); cnt_acc += 1.0; }
@@ -573,13 +598,27 @@ extern "C" int skd_dsn_ce_fwd(int N, int C, int h, int w, int H, int W, const fl
   return finish("skd_dsn_ce_fwd", 2);
 }
 
+extern "C" int skd_dsn_ce_fwd_weighted(int N, int C, int h, int w, int H, int W, const float* L0, long long a_sn, long long a_sc,
+                                       long long a_sp, const float* L1, long long b_sn, long long b_sc, long long b_sp,
+                                       const long long* labels, int ignore_index, float w0, float w1, float* loss, float* count,
+                                       double* workspace, const float* class_weight, cudaStream_t st) {
+  if (C > kMaxClasses) { set_error_msg("skd_dsn_ce_fwd_weighted", "C > 32 classes unsupported"); return 0; }
+  if (!class_weight) { set_error_msg("skd_dsn_ce_fwd_weighted", "class_weight is NULL"); return 0; }
+  const int blocks = red_blocks((long long)N * H * W);
+  dsn_ce_fwd_kernel<true><<<blocks, 256, 0, st>>>(L0, L1, Strides{a_sn, a_sc, a_sp}, Strides{b_sn, b_sc, b_sp}, labels, N, C, h, w,
+                                                 H, W, ignore_index, w0, w1, workspace, workspace + blocks, class_weight);
+  finalize_sum_kernel<<<1, 256, 0, st>>>(workspace, blocks, 1.0, loss, workspace + blocks, 1, count);
+  return finish("skd_dsn_ce_fwd_weighted", 2);
+}
+
 extern "C" long long skd_dsn_ce_bwd_workspace_floats(int N, int C, int w, int H, int heads) {
   return (long long)heads * N * H * C * w;
 }
 
 static int dsn_rows_launch(bool with_loss, int N, int C, int h, int w, int H, int W, const float* L0, Strides a, const float* L1, Strides b,
                            const long long* labels, int ignore_index, float w0, float w1, float* T1, double* part_loss, double* part_cnt,
-                           cudaStream_t st, const char* who, const float* ohem_thr = nullptr) {
+                           cudaStream_t st, const char* who, const float* ohem_thr = nullptr,
+                           const float* class_weight = nullptr) {
   const int heads = L1 ? 2 : 1;
   int chunk = W < 1024 ? W : 1024;
   const size_t smem = ((size_t)C * (chunk | 1) + 2 * (size_t)chunk + (size_t)w + 2 + (size_t)w * C) * sizeof(float);
@@ -592,9 +631,23 @@ static int dsn_rows_launch(bool with_loss, int N, int C, int h, int w, int H, in
     cudaFuncSetAttribute(dsn_ce_bwd_rows_kernel<true, kMaxClasses>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
     cudaFuncSetAttribute(dsn_ce_bwd_rows_kernel<true, 19, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
     cudaFuncSetAttribute(dsn_ce_bwd_rows_kernel<true, kMaxClasses, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+    cudaFuncSetAttribute(dsn_ce_bwd_rows_kernel<true, 19, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+    cudaFuncSetAttribute(dsn_ce_bwd_rows_kernel<true, kMaxClasses, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                         200 * 1024);
     attr_done = true;
   }
   const dim3 grid(H, N, heads);
+  if (class_weight) {
+    if (C <= 19)
+      dsn_ce_bwd_rows_kernel<true, 19, false, true><<<grid, kRowsThreads, smem, st>>>(L0, L1, a, b, labels, N, C, h, w, H, W, ignore_index,
+                                                                                    T1, chunk, part_loss, part_cnt, w0, w1, nullptr,
+                                                                                    class_weight);
+    else
+      dsn_ce_bwd_rows_kernel<true, kMaxClasses, false, true><<<grid, kRowsThreads, smem, st>>>(L0, L1, a, b, labels, N, C, h, w, H, W,
+                                                                                             ignore_index, T1, chunk, part_loss, part_cnt,
+                                                                                             w0, w1, nullptr, class_weight);
+    return 1;
+  }
   if (ohem_thr) {
     if (C <= 19)
       dsn_ce_bwd_rows_kernel<true, 19, true><<<grid, kRowsThreads, smem, st>>>(L0, L1, a, b, labels, N, C, h, w, H, W, ignore_index, T1,
@@ -641,6 +694,21 @@ extern "C" int skd_dsn_ce_fwd_train(int N, int C, int h, int w, int H, int W, co
                        partials, partials + np, st, "skd_dsn_ce_fwd_train")) return 0;
   finalize_sum_kernel<<<1, 256, 0, st>>>(partials, np, 1.0, loss, partials + np, 1, count);
   return finish("skd_dsn_ce_fwd_train", 2);
+}
+
+// Class-weighted training forward: count receives the sum of the kept pixels' class weights, which skd_dsn_ce_bwd_cols divides by
+extern "C" int skd_dsn_ce_fwd_train_weighted(int N, int C, int h, int w, int H, int W, const float* L0, long long a_sn, long long a_sc,
+                                             long long a_sp, const float* L1, long long b_sn, long long b_sc, long long b_sp,
+                                             const long long* labels, int ignore_index, float w0, float w1, float* loss, float* count,
+                                             double* partials, float* rows_ws, const float* class_weight, cudaStream_t st) {
+  if (C > kMaxClasses) { set_error_msg("skd_dsn_ce_fwd_train_weighted", "C > 32 classes unsupported"); return 0; }
+  if (!class_weight) { set_error_msg("skd_dsn_ce_fwd_train_weighted", "class_weight is NULL"); return 0; }
+  const int heads = L1 ? 2 : 1;
+  const int np = heads * N * H;
+  if (!dsn_rows_launch(true, N, C, h, w, H, W, L0, Strides{a_sn, a_sc, a_sp}, L1, Strides{b_sn, b_sc, b_sp}, labels, ignore_index, w0, w1, rows_ws,
+                       partials, partials + np, st, "skd_dsn_ce_fwd_train_weighted", nullptr, class_weight)) return 0;
+  finalize_sum_kernel<<<1, 256, 0, st>>>(partials, np, 1.0, loss, partials + np, 1, count);
+  return finish("skd_dsn_ce_fwd_train_weighted", 2);
 }
 
 // Backward after skd_dsn_ce_fwd_train: only the column phase (d logits = g / count * U_y^T rows_ws)

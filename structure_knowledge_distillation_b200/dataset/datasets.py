@@ -11,6 +11,8 @@ Split of the work:
 `CSDataLoader` chains the two and yields `(images, labels, size, name)` batches resident on the device, i.e. what `set_input` takes.
 `VOCDataSet` differs only in its file layout, its scale rule (`VOC_SCALES`), no label table (class ids 0..20 and 255 pass through)
 and its mean, which is subtracted with numpy's type as the reference does (`numpy_mean`); the same kernel serves both.
+`CamVidDataSet` is `CSDataSet` with the SegNet CamVid label table (11 classes); `class_frequency_weights` gives ENet class weights
+for the task loss of any of these datasets.
 The test split (`CSDataTestSet`, reference datasets.py:212-250) works the same way: raw files from the workers, mean subtraction and
 padding on the GPU (`DeviceTestPreprocess` -> `skd_cs_test_preprocess`), and `CSDataLoader` yields `(images, size, name)`, the
 batches `evaluate_main(type='test')` unpacks.  `VOCDataTestSet` (:84-119) subtracts its own mean and yields `(images, name, size)`.
@@ -98,6 +100,56 @@ def cityscapes_id_tables():
     to_train, to_label = np.zeros(256, np.uint8), np.zeros(256, np.uint8)
     _cabi.lib().skd_cityscapes_id_tables(to_train.ctypes.data, to_label.ctypes.data)
     return to_train, to_label
+
+
+CAMVID_CLASSES = ("Sky", "Building", "Pole", "Road", "Pavement", "Tree", "SignSymbol", "Fence", "Car", "Pedestrian", "Bicyclist")
+
+
+def camvid_label_table(ignore_label=IGNORE_LABEL):
+    """-> uint8[256]: the SegNet CamVid encoding.  Values 0..10 are the classes of `CAMVID_CLASSES` and pass through; every other
+    value, 11 (void) included, becomes `ignore_label`."""
+    table = np.full(256, ignore_label, np.uint8)
+    table[:len(CAMVID_CLASSES)] = np.arange(len(CAMVID_CLASSES), dtype=np.uint8)
+    return table
+
+
+class CamVidDataSet(CSDataSet):
+    """CamVid training / validation loader in the SegNet encoding (11 classes, void and every other value ignored).  It is
+    `CSDataSet` with another label table: the same list format (`image_path label_path` per line, relative to `root`), the same
+    scale rule and random draws (`CS_SCALES`), the same float32 mean, padding, crop and mirror, and `CSDataLoader` yields the same
+    `(images, labels, size, name)` batches.  Evaluate with `scale=False, mirror=False` at crop_size=(360, 480)."""
+
+    def __init__(self, root, list_path, max_iters=None, crop_size=(360, 480), mean=(128, 128, 128), scale=True, mirror=True, ignore_label=255):
+        super().__init__(root, list_path, max_iters, crop_size, mean, scale, mirror, ignore_label)
+        self.label_table = camvid_label_table(ignore_label)
+
+
+def _label_table_of(dataset):
+    """The raw-label -> class table a training loader applies: its own `label_table`, none for VOC, the Cityscapes id table."""
+    table = getattr(dataset, "label_table", None)
+    if table is not None:
+        return table
+    if isinstance(dataset, VOCDataSet):
+        return np.arange(256, dtype=np.uint8)
+    return cityscapes_id_tables()[0]
+
+
+def class_frequency_weights(dataset, num_classes, c=1.02):
+    """-> float32[num_classes] ENet class weights w_k = 1 / ln(c + p_k), p_k = class k's share of the dataset's labelled pixels
+    (those whose class, after the loader's label table, is in 0..num_classes-1).  Reads every label file of `dataset` once (a list
+    repeated by `max_iters` counts each file once) with no augmentation; a one-off host pass meant for `args.class_weights`."""
+    import cv2
+    table = _label_table_of(dataset)
+    counts = np.zeros(num_classes, np.int64)
+    for path in dict.fromkeys(f["label"] for f in dataset.files):
+        label = cv2.imread(path, cv2.IMREAD_GRAYSCALE)
+        if label is None:
+            raise IOError("cannot read %s" % path)
+        counts += np.bincount(table[label].ravel(), minlength=256)[:num_classes]
+    total = counts.sum()
+    if total == 0:
+        raise ValueError("no labelled pixel in 0..%d" % (num_classes - 1))
+    return (1.0 / np.log(c + counts / total)).astype(np.float32)
 
 
 class CSDataTestSet(data.Dataset):
@@ -240,16 +292,24 @@ class DeviceAugment:
     `label_dtype`: torch.float32 is what the reference's `__getitem__` returns; torch.int64 is what `NetModel.set_input` makes of it
     (`labels.long()`, kd_model.py:105) -- the default, it saves that conversion pass.
     `voc`: False (Cityscapes) maps label ids to train ids and subtracts the mean rounded to float32; True (PASCAL VOC) passes labels
-    through and subtracts the mean with numpy's type (`numpy_mean`)."""
+    through and subtracts the mean with numpy's type (`numpy_mean`).
+    `table`: with voc=False, a uint8[256] raw label -> class table to apply instead of the Cityscapes one (`camvid_label_table`)."""
 
-    def __init__(self, crop_size, mean, ignore_label=IGNORE_LABEL, label_dtype=torch.int64, device=None, voc=False):
+    def __init__(self, crop_size, mean, ignore_label=IGNORE_LABEL, label_dtype=torch.int64, device=None, voc=False, table=None):
         from .. import _cabi
         self._lib = _cabi.lib()
         self.crop_h, self.crop_w = crop_size
         if voc:
+            if table is not None:
+                raise ValueError("a VOC loader applies no label table")
             self.mean, self.table = numpy_mean(mean), None
         else:
-            self.mean, self.table = np.array([np.float32(m) for m in mean], np.float64), cityscapes_id_tables()[0]
+            if table is None:
+                table = cityscapes_id_tables()[0]
+            table = np.ascontiguousarray(table, np.uint8)
+            if table.shape != (256,):
+                raise ValueError("label table must have 256 entries (got shape %s)" % (table.shape,))
+            self.mean, self.table = np.array([np.float32(m) for m in mean], np.float64), table
         self.ignore_label = int(ignore_label)
         assert label_dtype in (torch.int64, torch.float32)
         self.label_dtype = label_dtype
@@ -311,7 +371,8 @@ class CSDataLoader:
             mean = numpy_mean(dataset.mean) if self.voc else dataset.mean
             self.augment = DeviceTestPreprocess((dataset.crop_h, dataset.crop_w), mean, device)
         else:
-            self.augment = DeviceAugment((dataset.crop_h, dataset.crop_w), dataset.mean, dataset.ignore_label, label_dtype, device, self.voc)
+            self.augment = DeviceAugment((dataset.crop_h, dataset.crop_w), dataset.mean, dataset.ignore_label, label_dtype, device, self.voc,
+                                         getattr(dataset, "label_table", None))
 
     def __len__(self):
         return len(self.loader)

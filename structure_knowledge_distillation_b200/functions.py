@@ -54,19 +54,21 @@ class PairWiseLoss(torch.autograd.Function):
 
 
 class DsnCrossEntropy(torch.autograd.Function):
-    """CriterionDSN math (utils/criterion.py:179-188): fused upsample + log-softmax + NLL for both heads."""
+    """CriterionDSN math (utils/criterion.py:179-188): fused upsample + log-softmax + NLL for both heads.  `weight` (C fp32 class
+    weights on the device, or None) makes each head's term CrossEntropyLoss(weight=weight)'s weighted mean."""
 
     @staticmethod
-    def forward(ctx, l0, l1, labels, ignore_index, w0, w1):
+    def forward(ctx, l0, l1, labels, ignore_index, w0, w1, weight=None):
         # with a backward to come, the forward pass over the upsampled pixels already leaves the backward's row-phase result behind
         # (one softmax per pixel and step instead of two); inference keeps the plain forward
         ctx.fused = l0.requires_grad or (l1 is not None and l1.requires_grad)
         if ctx.fused:
-            out, rows = ops.dsn_ce_fwd_train(l0, l1, labels, ignore_index, w0, w1)
+            out, rows = ops.dsn_ce_fwd_train(l0, l1, labels, ignore_index, w0, w1, weight)
             ctx.save_for_backward(l0, l1, rows, out)
             ctx.H = labels.shape[1]
         else:
-            out = ops.dsn_ce_fwd(l0, l1, labels, ignore_index, w0, w1)
+            # (no backward can follow: the weighted form needs no unfused backward)
+            out = ops.dsn_ce_fwd(l0, l1, labels, ignore_index, w0, w1, weight)
             ctx.save_for_backward(l0, l1, labels, out)
         ctx.cfg = (ignore_index, w0, w1)
         return out[0].clone()
@@ -81,7 +83,7 @@ class DsnCrossEntropy(torch.autograd.Function):
         else:
             l0, l1, labels, out = ctx.saved_tensors
             d0, d1 = ops.dsn_ce_bwd(l0, l1, labels, ig, w0, w1, g.contiguous(), out[1])
-        return d0, d1, None, None, None, None
+        return d0, d1, None, None, None, None, None
 
 
 class OhemDsnCrossEntropy(torch.autograd.Function):

@@ -25,7 +25,8 @@ from .. import functions as Fn
 from .. import ops
 from ..optim import FlatSGD
 from ..utils.criterion import (CriterionAdditionalGP, CriterionAdv, CriterionAdvForG, CriterionCrossEntropy, CriterionDSN,
-                               CriterionOhemDSN, CriterionPairWiseforWholeFeatAfterPool, CriterionPixelWise)
+                               CriterionOhemDSN, CriterionPairWiseforWholeFeatAfterPool, CriterionPixelWise,
+                               check_task_loss_weights)
 from ..utils.utils import load_D_model, load_S_model, load_T_model
 from .espnet import ESPNet, ESPNet_C
 from .evaluate import evaluate_main
@@ -65,6 +66,7 @@ class NetModel():
         self.args = args
         if not 1 <= int(args.classes_num) <= 32:              # the loss, OHEM and discriminator kernels hold up to 32 classes
             raise ValueError("classes_num must be in 1..32 (got %r)" % (args.classes_num,))
+        class_weights = check_task_loss_weights(args)
         device = torch.device(_arg(args, "device", "cuda"))
         if device.type != "cuda":
             raise RuntimeError("NetModel runs on CUDA (sm_90a) only; there is no CPU path")
@@ -131,9 +133,9 @@ class NetModel():
             # (ESPNet-C: head 0 only, preds[1] is None)
             self.criterion = CriterionOhemDSN(thresh=_arg(args, "ohem_thres", 0.7), min_kept=_arg(args, "ohem_keep", 100000))
         elif self.student_kind in ("espnet_c", "espnet"):         # the ESPNets: no auxiliary head, single-head cross entropy
-            self.criterion = CriterionCrossEntropy()
+            self.criterion = CriterionCrossEntropy(weight=class_weights).to(device)
         else:
-            self.criterion = CriterionDSN()
+            self.criterion = CriterionDSN(weight=class_weights).to(device)
         self.criterion_pixel_wise = CriterionPixelWise()
         self.criterion_pair_wise_for_interfeat = CriterionPairWiseforWholeFeatAfterPool(scale=args.pool_scale, feat_ind=-5)
         self.criterion_adv = CriterionAdv(args.adv_loss_type)

@@ -20,7 +20,7 @@ import torch.distributed as dist
 from .. import functions as Fn
 from .. import ops
 from ..optim import FlatSGD
-from ..utils.criterion import CriterionCrossEntropy, CriterionDSN, CriterionOhemDSN
+from ..utils.criterion import CriterionCrossEntropy, CriterionDSN, CriterionOhemDSN, check_task_loss_weights
 from ..utils.utils import load_seg_model
 from .espnet import ESPNet, ESPNet_C
 from .evaluate import evaluate_main
@@ -77,6 +77,7 @@ class SegModel():
         self.args = args
         if not 1 <= int(args.classes_num) <= 32:              # the loss and OHEM kernels hold up to 32 classes
             raise ValueError("classes_num must be in 1..32 (got %r)" % (args.classes_num,))
+        class_weights = check_task_loss_weights(args)
         self.kind = str(_arg(args, "seg_model", "resnet101"))
         if self.kind not in SEG_MODELS:
             raise ValueError("seg_model must be one of %s (got %r)" % (", ".join(repr(k) for k in SEG_MODELS), self.kind))
@@ -117,9 +118,9 @@ class SegModel():
         if _arg(args, "ohem", False):
             self.criterion = CriterionOhemDSN(thresh=_arg(args, "ohem_thres", 0.7), min_kept=_arg(args, "ohem_keep", 100000))
         elif self.kind in ("espnet_c", "espnet"):                   # no auxiliary head
-            self.criterion = CriterionCrossEntropy()
+            self.criterion = CriterionCrossEntropy(weight=class_weights).to(device)
         else:
-            self.criterion = CriterionDSN()
+            self.criterion = CriterionDSN(weight=class_weights).to(device)
 
         self.overlap_streams = bool(_arg(args, "overlap_streams", True))
         self._graphs = None

@@ -480,7 +480,18 @@ def pixelwise_bwd(S, T, grad_out):
     return dS
 
 
-def dsn_ce_fwd(l0, l1, labels, ignore_index, w0, w1):
+def _class_weight(weight, l0):
+    """The class-weight table as the weighted kernels read it: contiguous fp32, one entry per class, on the logits' device."""
+    if weight.dtype != torch.float32 or not weight.is_contiguous() or weight.dim() != 1 or weight.device != l0.device:
+        raise ValueError("class weight must be a contiguous 1-D float32 tensor on the logits' device")
+    if weight.numel() != l0.shape[1]:
+        raise ValueError("class weight has %d entries for %d classes" % (weight.numel(), l0.shape[1]))
+    return weight
+
+
+def dsn_ce_fwd(l0, l1, labels, ignore_index, w0, w1, weight=None):
+    """-> (loss, count): count is the number of valid pixels, or with `weight` (C class weights, fp32 on the device) the sum of their
+    class weights."""
     _f32(l0, l1)
     n, c, h, w = l0.shape
     H, W = labels.shape[1:]
@@ -488,13 +499,18 @@ def dsn_ce_fwd(l0, l1, labels, ignore_index, w0, w1):
         raise ValueError("labels must be contiguous int64")
     out = torch.empty(2, device=l0.device, dtype=torch.float32)       # loss, valid count
     s1 = pixel_strides(l1) if l1 is not None else (0, 0, 0)
-    lib().skd_dsn_ce_fwd(n, c, h, w, H, W, _p(l0), *pixel_strides(l0), _p(l1), *s1, _p(labels), ignore_index, w0, w1,
-                         _p(out[0]), _p(out[1]), _p(_ws(l0.device)), _st())
+    args = (n, c, h, w, H, W, _p(l0), *pixel_strides(l0), _p(l1), *s1, _p(labels), ignore_index, w0, w1, _p(out[0]), _p(out[1]),
+            _p(_ws(l0.device)))
+    if weight is None:
+        lib().skd_dsn_ce_fwd(*args, _st())
+    else:
+        lib().skd_dsn_ce_fwd_weighted(*args, _p(_class_weight(weight, l0)), _st())
     return out
 
 
-def dsn_ce_fwd_train(l0, l1, labels, ignore_index, w0, w1):
-    """Training forward: (loss, count) tensor AND the backward's row-phase workspace, in one pass over the upsampled pixels."""
+def dsn_ce_fwd_train(l0, l1, labels, ignore_index, w0, w1, weight=None):
+    """Training forward: (loss, count) tensor AND the backward's row-phase workspace, in one pass over the upsampled pixels.
+    With `weight` the loss is class-weighted and count is the sum of the valid pixels' class weights (dsn_ce_bwd_cols divides by it)."""
     _f32(l0, l1)
     n, c, h, w = l0.shape
     H, W = labels.shape[1:]
@@ -506,8 +522,12 @@ def dsn_ce_fwd_train(l0, l1, labels, ignore_index, w0, w1):
     parts = torch.empty(L.skd_dsn_ce_train_partials(n, H, heads), device=l0.device, dtype=torch.float64)
     rows = torch.empty(L.skd_dsn_ce_bwd_workspace_floats(n, c, w, H, heads), device=l0.device, dtype=torch.float32)
     s1 = pixel_strides(l1) if l1 is not None else (0, 0, 0)
-    L.skd_dsn_ce_fwd_train(n, c, h, w, H, W, _p(l0), *pixel_strides(l0), _p(l1), *s1, _p(labels), ignore_index, w0, w1,
-                           _p(out[0]), _p(out[1]), _p(parts), _p(rows), _st())
+    args = (n, c, h, w, H, W, _p(l0), *pixel_strides(l0), _p(l1), *s1, _p(labels), ignore_index, w0, w1, _p(out[0]), _p(out[1]),
+            _p(parts), _p(rows))
+    if weight is None:
+        L.skd_dsn_ce_fwd_train(*args, _st())
+    else:
+        L.skd_dsn_ce_fwd_train_weighted(*args, _p(_class_weight(weight, l0)), _st())
     return out, rows
 
 

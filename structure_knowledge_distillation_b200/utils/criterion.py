@@ -54,29 +54,78 @@ class CriterionPairWiseforWholeFeatAfterPool(nn.Module):
 CriterionPairWise = CriterionPairWiseforWholeFeatAfterPool
 
 
-class CriterionDSN(nn.Module):
-    """DSN : two supervisions, loss1 + 0.4 * loss2."""
+def check_class_weights(weight, classes_num=None):
+    """-> the class weights as a float32 CPU tensor, or None.  `weight` is a 1-D sequence or tensor of non-negative finite floats,
+    not all zero, with `classes_num` entries when that is given; anything else raises ValueError."""
+    if weight is None:
+        return None
+    try:
+        w = torch.as_tensor(weight.detach().cpu() if torch.is_tensor(weight) else weight, dtype=torch.float64)
+    except (TypeError, ValueError, RuntimeError) as e:
+        raise ValueError("class weights must be a 1-D sequence of floats (%s)" % e) from None
+    if w.dim() != 1 or w.numel() == 0:
+        raise ValueError("class weights must be a non-empty 1-D sequence (got shape %s)" % (tuple(w.shape),))
+    if classes_num is not None and w.numel() != int(classes_num):
+        raise ValueError("class weights have %d entries for %d classes" % (w.numel(), int(classes_num)))
+    if not bool(torch.isfinite(w).all()) or bool((w < 0).any()):
+        raise ValueError("class weights must be finite and non-negative (got %s)" % w.tolist())
+    if not bool((w > 0).any()):
+        raise ValueError("class weights are all zero")
+    return w.float()
 
-    def __init__(self, ignore_index=255, use_weight=True, reduce=True):
+
+def check_task_loss_weights(args):
+    """`args.class_weights` (default None) of NetModel / SegModel, validated against `args.classes_num` before any device work.
+    OHEM ignores class weights (so does the reference's OhemCrossEntropy2d), so asking for both raises ValueError."""
+    weight = getattr(args, "class_weights", None)
+    if weight is not None and getattr(args, "ohem", False):
+        raise ValueError("class_weights cannot be combined with ohem=True (the OHEM cross entropy is unweighted)")
+    return check_class_weights(weight, args.classes_num)
+
+
+class _WeightedCE(nn.Module):
+    """Holds the optional class-weight table of the task losses: copied to the device once, at `.to(device)` or at the first call."""
+
+    def __init__(self, weight):
         super().__init__()
+        self.register_buffer("weight", check_class_weights(weight))
+
+    def _weight(self, logits):
+        w = self.weight
+        if w is None:
+            return None
+        if w.numel() != logits.shape[1]:
+            raise ValueError("class weights have %d entries for %d classes" % (w.numel(), logits.shape[1]))
+        if w.device != logits.device:
+            self.weight = w = w.to(logits.device)
+        return w
+
+
+class CriterionDSN(_WeightedCE):
+    """DSN : two supervisions, loss1 + 0.4 * loss2.  `weight`: optional per-class weights of both cross entropies, as
+    torch.nn.CrossEntropyLoss(weight=...) applies them (a weighted mean with the heads' common denominator sum_i weight[y_i])."""
+
+    def __init__(self, ignore_index=255, use_weight=True, reduce=True, weight=None):
+        super().__init__(weight)
         self.ignore_index = ignore_index
         if not reduce:
             print("disabled the reduce.")
 
     def forward(self, preds, target):
-        return Fn.DsnCrossEntropy.apply(preds[0], preds[1], target, self.ignore_index, 1.0, 0.4)
+        return Fn.DsnCrossEntropy.apply(preds[0], preds[1], target, self.ignore_index, 1.0, 0.4, self._weight(preds[0]))
 
 
-class CriterionCrossEntropy(nn.Module):
+class CriterionCrossEntropy(_WeightedCE):
     """Single-head cross entropy, CE(up(preds[0])) with bilinear align_corners to the label size, mean over the valid pixels (the
-    class the reference names for students without an auxiliary head, kd_model.py:79): the task loss of the ESPNet-C student."""
+    class the reference names for students without an auxiliary head, kd_model.py:79): the task loss of the ESPNet-C student.
+    `weight`: optional per-class weights, as torch.nn.CrossEntropyLoss(weight=...) applies them."""
 
-    def __init__(self, ignore_index=255, use_weight=True, reduce=True):
-        super().__init__()
+    def __init__(self, ignore_index=255, use_weight=True, reduce=True, weight=None):
+        super().__init__(weight)
         self.ignore_index = ignore_index
 
     def forward(self, preds, target):
-        return Fn.DsnCrossEntropy.apply(preds[0], None, target, self.ignore_index, 1.0, 0.0)
+        return Fn.DsnCrossEntropy.apply(preds[0], None, target, self.ignore_index, 1.0, 0.0, self._weight(preds[0]))
 
 
 class OhemCrossEntropy2d(nn.Module):

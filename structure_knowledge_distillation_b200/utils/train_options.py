@@ -13,6 +13,7 @@ DEFAULTS = dict(
     lr_g=1e-2, lr_d=4e-4, best_mean_IU=0.0, gpu_num=1,
     cuda_graph=False,        # ours: capture the step into CUDA graphs after 3 eager steps (NetModel.enable_cuda_graphs)
     ohem=False, ohem_thres=0.7, ohem_keep=100000,   # ours: CriterionOhemDSN(thresh=ohem_thres, min_kept=ohem_keep) as the CE term
+    class_weights=None,      # ours: per-class weights of the task cross entropy (e.g. dataset.class_frequency_weights), not with ohem
     student='resnet18', espnet_p=2, espnet_q=8)     # ours: 'resnet18' (ResNet18-PSP), 'espnet_c' (ESPNet-C with p / q ESP blocks), 'espnet' (ESPNet-C + decoder) or 'mobilenetv2' (dilated MobileNetV2 + PSP head)
 
 
