@@ -26,7 +26,7 @@ from .. import ops
 from ..optim import FlatSGD
 from ..utils.criterion import (CriterionAdditionalGP, CriterionAdv, CriterionAdvForG, CriterionCrossEntropy, CriterionDSN,
                                CriterionOhemDSN, CriterionPairWiseforWholeFeatAfterPool, CriterionPixelWise,
-                               check_task_loss_weights)
+                               check_pa_levels, check_task_loss_weights, pair_wise_level_criteria)
 from ..utils.utils import load_D_model, load_S_model, load_T_model
 from .espnet import ESPNet, ESPNet_C
 from .evaluate import evaluate_main
@@ -67,6 +67,9 @@ class NetModel():
         if not 1 <= int(args.classes_num) <= 32:              # the loss, OHEM and discriminator kernels hold up to 32 classes
             raise ValueError("classes_num must be in 1..32 (got %r)" % (args.classes_num,))
         class_weights = check_task_loss_weights(args)
+        # None: scalar lambda_pa / pool_scale, one pair-wise term on preds[-5]; else [(lambda, scale)] per level, level `ind` on
+        # preds[-(ind + 1)] (x1, x2, x3, x4, PSP features)
+        self.pa_levels = check_pa_levels(args)
         device = torch.device(_arg(args, "device", "cuda"))
         if device.type != "cuda":
             raise RuntimeError("NetModel runs on CUDA (sm_90a) only; there is no CPU path")
@@ -137,7 +140,10 @@ class NetModel():
         else:
             self.criterion = CriterionDSN(weight=class_weights).to(device)
         self.criterion_pixel_wise = CriterionPixelWise()
-        self.criterion_pair_wise_for_interfeat = CriterionPairWiseforWholeFeatAfterPool(scale=args.pool_scale, feat_ind=-5)
+        if self.pa_levels is None:
+            self.criterion_pair_wise_for_interfeat = CriterionPairWiseforWholeFeatAfterPool(scale=args.pool_scale, feat_ind=-5)
+        else:                                                     # the reference's multi-level form (kd_model.py:81)
+            self.criterion_pair_wise_for_interfeat = pair_wise_level_criteria(self.pa_levels)
         self.criterion_adv = CriterionAdv(args.adv_loss_type)
         if args.adv_loss_type == 'wgan-gp':
             self.criterion_AdditionalGP = CriterionAdditionalGP(self.parallel_D, args.lambda_gp)
@@ -151,7 +157,7 @@ class NetModel():
             self.enable_cuda_graphs()
         self.mc_G_loss = 0.0
         self.pi_G_loss = 0.0
-        self.pa_G_loss = 0.0
+        self.pa_G_loss = 0.0 if self.pa_levels is None else [0.0] * len(self.pa_levels)
         self.D_loss = 0.0
         self.G_loss = 0.0
         snap = _arg(args, "snapshot_dir", None)
@@ -227,13 +233,18 @@ class NetModel():
 
     def _resample_teacher(self):
         """Students on another grid than the teacher (ESPNet-C: 45x60 at 360x480, PSPNet's ceil-mode pool: 46x61; the full ESPNet's
-        logits: 360x480): the two teacher tensors the distillation terms read, preds_T[0] and preds_T[-5], are each resized onto the
-        grid of their own student counterpart, preds_S[0] and preds_S[-5] (bilinear, align_corners=True; forward only, the teacher is
-        frozen).  Equal grids (the ResNet18 student): nothing runs.  The teacher's own logits stay in `logits_T` for the
-        discriminator of a full-resolution student."""
+        logits: 360x480): the teacher tensors the distillation terms read -- preds_T[0] and preds_T[-5], or with pair-wise levels
+        preds_T[0] and the preds_T[-(ind + 1)] of every level with a non-zero weight -- are each resized onto the grid of their own
+        student counterpart (bilinear, align_corners=True; forward only, the teacher is frozen).  Equal grids (the ResNet18
+        student): nothing runs.  The teacher's own logits stay in `logits_T` for the discriminator of a full-resolution student."""
         self.logits_T = self.preds_T[0]
         preds = list(self.preds_T)
-        for i in (0, len(preds) - 5):
+        if self.pa_levels is None:
+            read = (0, len(preds) - 5)
+        else:
+            read = [0] + ([len(preds) - 1 - ind for ind, (lam, _) in enumerate(self.pa_levels) if lam != 0.0]
+                          if self.args.pa == True else [])
+        for i in read:
             size = tuple(self.preds_S[i].shape[2:])
             if tuple(preds[i].shape[2:]) != size:
                 preds[i] = ops.resample_nhwc(preds[i], *size)
@@ -258,7 +269,9 @@ class NetModel():
             temp = args.lambda_pi * self.criterion_pixel_wise(self.preds_S, self.preds_T)
             self.pi_G_loss = _LazyScalar(temp)
             G_loss = G_loss + temp
-        if args.pa == True:
+        if args.pa == True and self.pa_levels is not None:
+            G_loss = self._pa_levels_loss(G_loss)
+        elif args.pa == True:
             temp1 = self.criterion_pair_wise_for_interfeat(self.preds_S, self.preds_T)
             self.pa_G_loss = _LazyScalar(temp1)
             G_loss = G_loss + args.lambda_pa * temp1
@@ -289,6 +302,24 @@ class NetModel():
                 self.G_solver.finish_overlapped_reduce()
         self._g_reduced = overlap
         self.G_loss = _LazyScalar(G_loss)
+
+    def _pa_levels_loss(self, G_loss):
+        """G_loss + sum over levels of lambda_pa[ind] * Pa(preds[-(ind + 1)]) (kd_model.py:137-143).  A level with lambda 0 launches
+        nothing and logs 0.0; pa_G_loss holds each level's unweighted term as a lazy device scalar."""
+        pa = []
+        for ind, ((lam, scale), crit) in enumerate(zip(self.pa_levels, self.criterion_pair_wise_for_interfeat)):
+            if lam == 0.0:
+                pa.append(0.0)
+                continue
+            h, w = self.preds_T[crit.feat_ind].shape[2:]
+            if int(h * scale) < 1 or int(w * scale) < 1:
+                raise ValueError("pair-wise level %d (preds[%d], %dx%d): pool_scale %r gives a %dx%d pooling window; raise the "
+                                 "scale or the input size" % (ind, crit.feat_ind, h, w, scale, int(h * scale), int(w * scale)))
+            temp = crit(self.preds_S, self.preds_T)
+            pa.append(_LazyScalar(temp))
+            G_loss = G_loss + lam * temp
+        self.pa_G_loss = pa
+        return G_loss
 
     def discriminator_backward(self):
         self._discriminator_phase()
@@ -415,9 +446,13 @@ class NetModel():
         return mean_IU, IU_array
 
     def print_info(self, epoch, step):
-        logging.info('step:{:5d} G_lr:{:.6f} G_loss:{:.5f}(mc:{:.5f} pixelwise:{:.5f} pairwise:{:.5f}) D_lr:{:.6f} D_loss:{:.5f}'.format(
+        if isinstance(self.pa_G_loss, list):                        # one unweighted term per pair-wise level
+            pa = '[' + ', '.join('{:.5f}'.format(float(v)) for v in self.pa_G_loss) + ']'
+        else:
+            pa = '{:.5f}'.format(float(self.pa_G_loss))
+        logging.info('step:{:5d} G_lr:{:.6f} G_loss:{:.5f}(mc:{:.5f} pixelwise:{:.5f} pairwise:{}) D_lr:{:.6f} D_loss:{:.5f}'.format(
             step, self.G_solver.param_groups[-1]['lr'], float(self.G_loss), float(self.mc_G_loss), float(self.pi_G_loss),
-            float(self.pa_G_loss), self.D_solver.param_groups[-1]['lr'], float(self.D_loss)))
+            pa, self.D_solver.param_groups[-1]['lr'], float(self.D_loss)))
 
     def save_ckpt(self, epoch, step, mean_IU, IU_array):
         if self.world > 1 and dist.get_rank() != 0:

@@ -19,6 +19,8 @@ Differences, on purpose:
   * with several ranks each rank thresholds its own shard (the reference's per-replica criterion semantics);
   * when no pixel is kept the loss is NaN, as torch's cross entropy returns, and the gradient is zero.
 """
+import math
+
 import torch
 import torch.nn as nn
 
@@ -52,6 +54,44 @@ class CriterionPairWiseforWholeFeatAfterPool(nn.Module):
 
 
 CriterionPairWise = CriterionPairWiseforWholeFeatAfterPool
+
+PA_LEVELS_MAX = 5          # preds[-1] .. preds[-5]: x1, x2, x3, x4 and the PSP features of every student
+
+
+def check_pa_levels(args):
+    """`args.lambda_pa` / `args.pool_scale` of NetModel, validated before any device work.  Two scalars (the defaults): None, the
+    single pair-wise term on preds[-5].  Two lists (or tuples) of equal length L, 1 <= L <= 5: the multi-level form of the
+    reference's kd_model.py:81,137-143, returned as [(lambda, scale), ...] where entry `ind` distils preds[-(ind + 1)] -- 0 is x1
+    (layer1), 1 x2, 2 x3, 3 x4, 4 the PSP features; so a one-entry list distils x1, not preds[-5].  Each lambda finite and >= 0
+    (0 skips the level), each scale in (0, 1]; anything else raises ValueError."""
+    lam, scale = getattr(args, "lambda_pa", 0.5), getattr(args, "pool_scale", 0.5)
+    lam_list, scale_list = isinstance(lam, (list, tuple)), isinstance(scale, (list, tuple))
+    if not lam_list and not scale_list:
+        return None
+    if lam_list != scale_list:
+        raise ValueError("lambda_pa and pool_scale must both be scalars or both be lists (got %r and %r)" % (lam, scale))
+    if len(lam) != len(scale):
+        raise ValueError("lambda_pa and pool_scale lists differ in length (%d and %d)" % (len(lam), len(scale)))
+    if not 1 <= len(lam) <= PA_LEVELS_MAX:
+        raise ValueError("lambda_pa / pool_scale lists must have 1..%d entries (got %d)" % (PA_LEVELS_MAX, len(lam)))
+    levels = []
+    for ind, (l, s) in enumerate(zip(lam, scale)):
+        try:
+            l, s = float(l), float(s)
+        except (TypeError, ValueError):
+            raise ValueError("pair-wise level %d: lambda_pa and pool_scale must be numbers (got %r, %r)" % (ind, l, s)) from None
+        if not math.isfinite(l) or l < 0:
+            raise ValueError("pair-wise level %d: lambda_pa must be finite and >= 0 (got %r)" % (ind, l))
+        if not (math.isfinite(s) and 0 < s <= 1):
+            raise ValueError("pair-wise level %d: pool_scale must be in (0, 1] (got %r)" % (ind, s))
+        levels.append((l, s))
+    return levels
+
+
+def pair_wise_level_criteria(levels):
+    """One CriterionPairWiseforWholeFeatAfterPool per level of check_pa_levels(), level `ind` on preds[-(ind + 1)]
+    (kd_model.py:81)."""
+    return [CriterionPairWiseforWholeFeatAfterPool(scale=s, feat_ind=-(ind + 1)) for ind, (_, s) in enumerate(levels)]
 
 
 def check_class_weights(weight, classes_num=None):
