@@ -87,7 +87,8 @@ def test_valid_levels_and_scalars():
 
 def test_print_info_prints_one_term_per_level(caplog):
     import logging
-    from structure_knowledge_distillation_b200.networks.kd_model import NetModel, _LazyScalar
+    from structure_knowledge_distillation_b200.networks.kd_model import NetModel
+    from structure_knowledge_distillation_b200.networks.step_model import _LazyScalar
     groups = types.SimpleNamespace(param_groups=[{"lr": 0.01}])
     m = types.SimpleNamespace(G_solver=groups, D_solver=groups, G_loss=_LazyScalar(torch.tensor(3.0)), mc_G_loss=1.0, pi_G_loss=2.0,
                               pa_G_loss=[_LazyScalar(torch.tensor(0.25)), 0.0, _LazyScalar(torch.tensor(0.125))], D_loss=0.5)

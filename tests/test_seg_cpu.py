@@ -64,7 +64,7 @@ def test_seg_model_validation(kw, msg):
 
 def test_seg_network_kinds():
     from structure_knowledge_distillation_b200.networks.pspnet_combine import BasicBlock, Bottleneck
-    from structure_knowledge_distillation_b200.networks.seg_model import SEG_MODELS, build_seg_network
+    from structure_knowledge_distillation_b200.networks.step_model import SEG_MODELS, build_seg_network
     assert SEG_MODELS[0] == "resnet101"
     r101 = build_seg_network("resnet101", 21)
     assert isinstance(r101.layer3[0], Bottleneck) and len(r101.layer3) == 23 and r101.head.out_channels == 21
@@ -79,7 +79,8 @@ def test_precision_policies():
     """The policies set exactly the convolutions they name, and SegModel's choice leaves the ResNet constructor's flags alone (NetModel's
     student and teacher keep them)."""
     from structure_knowledge_distillation_b200.networks.pspnet_combine import Conv2d
-    from structure_knowledge_distillation_b200.networks.seg_model import DEFAULT_PRECISION, build_seg_network, set_precision_policy
+    from structure_knowledge_distillation_b200.networks.seg_model import DEFAULT_PRECISION, set_precision_policy
+    from structure_knowledge_distillation_b200.networks.step_model import build_seg_network
     net = build_seg_network("resnet101", 19)
     fresh = {n: m.precise for n, m in net.named_modules() if isinstance(m, Conv2d)}
     early = {n for n, p in fresh.items() if p}
@@ -110,7 +111,7 @@ def _imagenet_state(net, seed=0):
 
 
 def test_imagenet_init_loads_by_intersection(tmp_path, caplog):
-    from structure_knowledge_distillation_b200.networks.seg_model import build_seg_network
+    from structure_knowledge_distillation_b200.networks.step_model import build_seg_network
     from structure_knowledge_distillation_b200.utils.utils import load_seg_model
     net = build_seg_network("resnet101", 19)
     sd = _imagenet_state(net)
@@ -132,7 +133,7 @@ def test_imagenet_init_loads_by_intersection(tmp_path, caplog):
 
 
 def test_resume_restores_state_and_last_step(tmp_path):
-    from structure_knowledge_distillation_b200.networks.seg_model import build_seg_network
+    from structure_knowledge_distillation_b200.networks.step_model import build_seg_network
     from structure_knowledge_distillation_b200.utils.utils import load_seg_model
     src = build_seg_network("resnet18", 19)
     torch.save(dict(state_dict={"module." + k: v for k, v in src.state_dict().items()}, step=1234, epoch=3, best_mean_IU=0.5),
