@@ -47,9 +47,10 @@ int skd_elu_backward_cuda(int N, const float* x, float* dx, cudaStream_t);
 int skd_elu_inv_cuda(int N, float* x, cudaStream_t);
 
 /* ---- B. fused NHWC ABN used between the wgmma convolutions (same math: libs/functions.py:81-109,113-162) ---- */
-int skd_abn_num_splits(long long P, int C);   /* workspace = splits*C*2 floats */
+int skd_abn_num_splits(long long P, int C);   /* workspace = splits*C*6 floats (stats), splits*C*2 floats (bwd reduce) */
 /* batch stats of x[P][C] -> mean,var (biased); running EMA with n/(n-1) (functions.py:90-91); scale=(|w|+eps)*rsqrt(var+eps),
-   shift=b-mean*scale for the apply pass */
+   shift=b-mean*scale for the apply pass.  One pass of sums shifted by the first row, kept in float and in double; a channel whose
+   first row lies more than 8 std from its mean takes the double sums.  workspace: 16-byte aligned */
 int skd_abn_stats_nhwc(long long P, int C, const float* x, const float* weight, const float* bias, float eps, float momentum,
                        float* running_mean, float* running_var, float* mean, float* var, float* scale, float* shift,
                        float* workspace, int splits, cudaStream_t);

@@ -280,54 +280,70 @@ int elementwise_grid_y(int C, long long per_channel) {
 // ------------------------------------------------------------------------------------------------
 // Part B: NHWC kernels.  x is [P][C] (P = N*H*W rows), C % 4 == 0.
 // ------------------------------------------------------------------------------------------------
-// partial[r][c] = (sum_rows (x-K), sum_rows (x-K)^2) over the rows owned by split r, K = x[0][c]
+// Shifted one-pass sums lose (m / std)^2 of float's precision, m = mean - K: ~3e-6 of the variance when the first row lies a few std
+// from the mean, 1e-4 at 16 std, 1e-3 at 100.  The same pass therefore also keeps the sums in double, and a channel whose first row
+// lies more than kShiftStd std from the mean takes its statistics from those; every other channel keeps the float result.
+constexpr float kShiftStd = 8.f;
+
+// partial[r][c] = (sum_rows (x-K), sum_rows (x-K)^2) over the rows owned by split r, K = x[0][c], in float; partial_d[r][c] the same
+// sums in double
 __global__ void __launch_bounds__(256)
-nhwc_stats_partial_kernel(const float* __restrict__ x, float2* __restrict__ partial, long long P, int C) {
+nhwc_stats_partial_kernel(const float* __restrict__ x, float2* __restrict__ partial, double2* __restrict__ partial_d, long long P,
+                          int C) {
   __shared__ float4 sh1[256], sh2[256];
+  __shared__ double4 shd1[256], shd2[256];
   const int C4 = C >> 2;
-  const int TC = C4 < 256 ? C4 : 256;                   // threads across channels (power of two by construction)
+  const int TC = C4 < 256 ? C4 : 256;                   // threads across channels
   const int TR = 256 / TC;                              // rows in flight per block
   const int tx = threadIdx.x % TC, ty = threadIdx.x / TC;
   const int c4 = blockIdx.y * TC + tx;
   const bool active = c4 < C4 && ty < TR;
   float4 K = active ? __ldg(reinterpret_cast<const float4*>(x) + c4) : make_float4(0, 0, 0, 0);
   float4 s1 = make_float4(0, 0, 0, 0), s2 = make_float4(0, 0, 0, 0);
+  double4 d1 = make_double4(0, 0, 0, 0), d2 = d1;
   if (active) {
     const long long rows_per = (P + gridDim.x - 1) / gridDim.x;
     const long long r0 = (long long)blockIdx.x * rows_per;
     long long r1 = r0 + rows_per; if (r1 > P) r1 = P;
     const float4* base = reinterpret_cast<const float4*>(x) + c4;
     long long r = r0 + ty;
+#define ACCD(v, f) { const double e = (double)v.f - (double)K.f; d1.f += e; d2.f = fma(e, e, d2.f); }
+#define ACC(v) { float a = v.x - K.x, b = v.y - K.y, c = v.z - K.z, d = v.w - K.w; \
+                 s1.x += a; s1.y += b; s1.z += c; s1.w += d; s2.x += a * a; s2.y += b * b; s2.z += c * c; s2.w += d * d; \
+                 ACCD(v, x) ACCD(v, y) ACCD(v, z) ACCD(v, w) }
     for (; r + 3LL * TR < r1; r += 4LL * TR) {          // 4 independent 16B loads in flight per thread
       float4 v0 = ld_stream(base + r * C4), v1 = ld_stream(base + (r + TR) * C4);
       float4 v2 = ld_stream(base + (r + 2LL * TR) * C4), v3 = ld_stream(base + (r + 3LL * TR) * C4);
-#define ACC(v) { float a = v.x - K.x, b = v.y - K.y, c = v.z - K.z, d = v.w - K.w; \
-                 s1.x += a; s1.y += b; s1.z += c; s1.w += d; s2.x += a * a; s2.y += b * b; s2.z += c * c; s2.w += d * d; }
       ACC(v0) ACC(v1) ACC(v2) ACC(v3)
     }
     for (; r < r1; r += TR) { float4 v = ld_stream(base + r * C4); ACC(v) }
 #undef ACC
+#undef ACCD
   }
-  sh1[threadIdx.x] = s1; sh2[threadIdx.x] = s2;
+  sh1[threadIdx.x] = s1; sh2[threadIdx.x] = s2; shd1[threadIdx.x] = d1; shd2[threadIdx.x] = d2;
   __syncthreads();
   if (ty == 0 && active) {
     for (int k = 1; k < TR; ++k) {
       float4 a = sh1[k * TC + tx], b = sh2[k * TC + tx];
       s1.x += a.x; s1.y += a.y; s1.z += a.z; s1.w += a.w; s2.x += b.x; s2.y += b.y; s2.z += b.z; s2.w += b.w;
+      const double4 p = shd1[k * TC + tx], q = shd2[k * TC + tx];
+      d1.x += p.x; d1.y += p.y; d1.z += p.z; d1.w += p.w; d2.x += q.x; d2.y += q.y; d2.z += q.z; d2.w += q.w;
     }
     float2* out = partial + (size_t)blockIdx.x * C + 4 * (size_t)c4;
     out[0] = make_float2(s1.x, s2.x); out[1] = make_float2(s1.y, s2.y);
     out[2] = make_float2(s1.z, s2.z); out[3] = make_float2(s1.w, s2.w);
+    double2* od = partial_d + (size_t)blockIdx.x * C + 4 * (size_t)c4;
+    od[0] = make_double2(d1.x, d2.x); od[1] = make_double2(d1.y, d2.y);
+    od[2] = make_double2(d1.z, d2.z); od[3] = make_double2(d1.w, d2.w);
   }
 }
 
 // mean/var from the split partials (+ running-stat EMA, + folded scale/shift for the apply pass)
-__global__ void nhwc_stats_finalize_kernel(const float* __restrict__ x, const float2* __restrict__ partial, int R,
-                                           int C, float count, const float* __restrict__ weight,
-                                           const float* __restrict__ bias, float eps, float momentum,
-                                           float* running_mean, float* running_var, float* __restrict__ mean,
-                                           float* __restrict__ var, float* __restrict__ scale,
-                                           float* __restrict__ shift) {
+__global__ void nhwc_stats_finalize_kernel(const float* __restrict__ x, const float2* __restrict__ partial,
+                                           const double2* __restrict__ partial_d, int R, int C, float count,
+                                           const float* __restrict__ weight, const float* __restrict__ bias, float eps,
+                                           float momentum, float* running_mean, float* running_var, float* __restrict__ mean,
+                                           float* __restrict__ var, float* __restrict__ scale, float* __restrict__ shift) {
   // one WARP per channel (8 channels per block): the R (~600) split partials of a channel are read by 32 lanes -- ~19 dependent loads
   // per thread instead of 37 -- and folded with shuffles (the 2-block version was latency-bound, 58 times a step)
   const int lane = threadIdx.x & 31;
@@ -336,11 +352,20 @@ __global__ void nhwc_stats_finalize_kernel(const float* __restrict__ x, const fl
   float s1 = 0.f, s2 = 0.f;
   for (int r = lane; r < R; r += 32) { float2 p = partial[(size_t)r * C + c]; s1 += p.x; s2 += p.y; }
   s1 = warp_sum(s1); s2 = warp_sum(s2);
-  if (lane != 0) return;
   const float K = x[c];
   const float m = s1 / count;
-  const float mu = K + m;
-  const float v = fmaxf(s2 / count - m * m, 0.f);
+  float mu = K + m;
+  float v = fmaxf(__fsub_rn(s2 / count, __fmul_rn(m, m)), 0.f);   // product and difference rounded separately, never fused
+  if (fabsf(m) > kShiftStd * sqrtf(v)) {                           // the whole warp: the same s1, s2 in every lane
+    double t1 = 0.0, t2 = 0.0;
+    for (int r = lane; r < R; r += 32) { const double2 p = partial_d[(size_t)r * C + c]; t1 += p.x; t2 += p.y; }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) { t1 += __shfl_xor_sync(0xffffffffu, t1, o); t2 += __shfl_xor_sync(0xffffffffu, t2, o); }
+    const double md = t1 / (double)count;
+    mu = (float)((double)K + md);
+    v = (float)fmax(t2 / (double)count - md * md, 0.0);
+  }
+  if (lane != 0) return;
   mean[c] = mu; var[c] = v;
   if (running_mean) {                                              // libs/functions.py:90-91
     running_mean[c] = running_mean[c] * (1.f - momentum) + momentum * mu;
@@ -401,7 +426,14 @@ __device__ __forceinline__ float dact(float o, float g, int act, float slope) {
   return g;
 }
 
-// partial[r][c] = (sum dz, sum y*dz), dz = dout * chan_mul * act'(out), y = (x-mean)*invstd
+// The stored output is act(.) * chan_mul: ELU's derivative (o + 1 where o < 0) needs o before the mask.  A zero mask zeroes g,
+// so its o does not matter.  (relu / leaky only read the sign, which a positive mask keeps.)
+__device__ __forceinline__ void unmask(float4& o, const float4 m) {
+  o.x = m.x != 0.f ? o.x / m.x : 0.f; o.y = m.y != 0.f ? o.y / m.y : 0.f;
+  o.z = m.z != 0.f ? o.z / m.z : 0.f; o.w = m.w != 0.f ? o.w / m.w : 0.f;
+}
+
+// partial[r][c] = (sum dz, sum y*dz), dz = dout * chan_mul * act'(out / chan_mul), y = (x-mean)*invstd
 __global__ void __launch_bounds__(256)
 nhwc_bwd_partial_kernel(const float* __restrict__ x, const float* __restrict__ out, const float* __restrict__ dout,
                         float2* __restrict__ partial, long long P, int C, int S, const float* __restrict__ mean,
@@ -437,6 +469,7 @@ nhwc_bwd_partial_kernel(const float* __restrict__ x, const float* __restrict__ o
       if (chan_mul) {
         const float4 m = __ldg(reinterpret_cast<const float4*>(chan_mul) + (r / S) * C4 + c4);
         g.x *= m.x; g.y *= m.y; g.z *= m.z; g.w *= m.w;
+        if (act == ACT_ELU) unmask(ov, m);
       }
       g.x = dact(ov.x, g.x, act, slope); g.y = dact(ov.y, g.y, act, slope);
       g.z = dact(ov.z, g.z, act, slope); g.w = dact(ov.w, g.w, act, slope);
@@ -514,6 +547,7 @@ nhwc_bwd_dx_kernel(const float* __restrict__ x, const float* __restrict__ out, c
       const long long row = i / C4;
       const float4 m = __ldg(reinterpret_cast<const float4*>(chan_mul) + (row / S) * C4 + c4);
       g.x *= m.x; g.y *= m.y; g.z *= m.z; g.w *= m.w;
+      if (act == ACT_ELU) unmask(ov, m);
     }
     g.x = dact(ov.x, g.x, act, slope); g.y = dact(ov.y, g.y, act, slope);
     g.z = dact(ov.z, g.z, act, slope); g.w = dact(ov.w, g.w, act, slope);
@@ -614,10 +648,11 @@ extern "C" int skd_abn_stats_nhwc(long long P, int C, const float* x, const floa
   if (!nhwc_check("skd_abn_stats_nhwc", C, x, workspace, nullptr)) return 0;
   if (P <= 0) return 1;
   const int chunks = (C / 4 + 255) / 256;
-  nhwc_stats_partial_kernel<<<dim3(splits, chunks), 256, 0, st>>>(x, reinterpret_cast<float2*>(workspace), P, C);
-  nhwc_stats_finalize_kernel<<<(C + 7) / 8, 256, 0, st>>>(x, reinterpret_cast<const float2*>(workspace), splits, C,
-                                                             (float)P, weight, bias, eps, momentum, running_mean,
-                                                             running_var, mean, var, scale, shift);
+  float2* part = reinterpret_cast<float2*>(workspace);
+  double2* part_d = reinterpret_cast<double2*>(workspace + (size_t)splits * C * 2);
+  nhwc_stats_partial_kernel<<<dim3(splits, chunks), 256, 0, st>>>(x, part, part_d, P, C);
+  nhwc_stats_finalize_kernel<<<(C + 7) / 8, 256, 0, st>>>(x, part, part_d, splits, C, (float)P, weight, bias, eps, momentum,
+                                                             running_mean, running_var, mean, var, scale, shift);
   return finish("skd_abn_stats_nhwc", 2);
 }
 

@@ -100,7 +100,7 @@ def abn_stats(x, weight, bias, eps, momentum, running_mean, running_var):
     L = lib()
     splits = L.skd_abn_num_splits(P, c)
     dev = x.device
-    ws = torch.empty(splits * c * 2, device=dev)
+    ws = torch.empty(splits * c * 6, device=dev)     # float (s1, s2) and double (s1, s2) partials per split and channel
     out = torch.empty(4, c, device=dev)              # mean, var, scale, shift
     L.skd_abn_stats_nhwc(P, c, _p(x), _p(weight), _p(bias), eps, momentum, _p(running_mean), _p(running_var),
                          _p(out[0]), _p(out[1]), _p(out[2]), _p(out[3]), _p(ws), splits, _st())
