@@ -20,7 +20,7 @@
 //   TMA_EPI         (short-K flat / im2col launches with a residual) the residual comes in and the output goes out through a
 //                   shared-memory tile: thread 32 of warpgroup 0 loads the tile's residual by TMA while the K loop runs, and each
 //                   consumer warpgroup hands its finished 64 rows to one TMA store and starts the next tile's wgmmas without waiting.
-//   BLOCK_M = 256   (long-K flat / im2col launches) 256-pixel tiles: the producer loads A as two 128-row boxes, warpgroup g owns
+//   BLOCK_M = 256   (flat / im2col, BLOCK_N 128) 256-pixel tiles: the producer loads A as two 128-row boxes, warpgroup g owns
 //                   rows 128g .. 128g+127 as two m64 sub-tiles sharing each B read, so a stage brings 48 KB for twice the MMA work
 //                   of a 32 KB 128-row stage.  setmaxnreg moves registers from the producer warpgroup to the two accumulators.
 #include <cuda.h>
@@ -41,7 +41,9 @@ constexpr int kBoxBytes = kBlockM * kBlockK * 4;
 constexpr int kProducerRegs = 40;           // BLOCK_M = 256: per-thread registers of the producer / consumer warpgroups after
 constexpr int kConsumerRegs = 232;          //   setmaxnreg; 128 * 40 + 256 * 232 = 64 512 <= the 65 536 of the SM
 constexpr int kTmaEpiMaxK = 16;             // longest K loop (taps x 32-channel chunks) that takes the TMA epilogue
-constexpr int kTile256MinK = 128;           // shortest K loop that takes 256-row tiles
+constexpr int kTile256MinK = 2;             // K loops (taps x 32-channel chunks) that take 256-row tiles: at least 2 steps,
+constexpr int kTile256OneNMinK = 18;        //   and 18 .. 72 steps for a launch with a single N tile
+constexpr int kTile256OneNMaxK = 72;
 constexpr int kEpiBoxBytes = 64 * kBlockK * 4;   // TMA epilogue box: 64 rows x 32 channels
 
 struct ConvArgs {
@@ -409,33 +411,42 @@ conv_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_co
             }
           }
         }
-        // Pass 2: activation, rounding, sum of squares, stores
+        // Pass 2: activation, rounding, sum of squares, stores.  One copy of the pass per activation, chosen once per tile: with the
+        // activation chosen per value, the inlined ELU made every column pair 2 KB of code, and a 256-row tile's epilogue took
+        // 50 - 58 us instead of 8 (DESIGN.md §3.1, §6).
+        auto pass2 = [&](auto act) {
 #pragma unroll
-        for (int s = 0; s < MS; ++s) {
+          for (int s = 0; s < MS; ++s) {
 #pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            if (!in[s][h]) continue;
-            float part = 0.f;
+            for (int h = 0; h < 2; ++h) {
+              if (!in[s][h]) continue;
+              float part = 0.f;
 #pragma unroll
-            for (int j = 0; j < BLOCK_N / 8; ++j) {
-              const int c = c0 + 8 * j;
-              if (c >= a.Cout) continue;
-              const bool two = c + 1 < a.Cout;
-              float v0 = acc[s][4 * j + 2 * h], v1 = acc[s][4 * j + 2 * h + 1];
-              v0 = epi_act(v0, a.act, a.slope); v1 = epi_act(v1, a.act, a.slope);
-              if (a.round_out) { v0 = ptx::round_tf32(v0); v1 = ptx::round_tf32(v1); }
-              if (a.sumsq) part = fmaf(v0, v0, two ? fmaf(v1, v1, part) : part);
-              if (a.no_store) continue;
-              float* y = yrow[s][h];
-              if (two && !((reinterpret_cast<uintptr_t>(y + c)) & 7)) {
-                *reinterpret_cast<float2*>(y + c) = make_float2(v0, v1);
-              } else {
-                y[c] = v0;
-                if (two) y[c + 1] = v1;
+              for (int j = 0; j < BLOCK_N / 8; ++j) {
+                const int c = c0 + 8 * j;
+                if (c >= a.Cout) continue;
+                const bool two = c + 1 < a.Cout;
+                float v0 = act(acc[s][4 * j + 2 * h]), v1 = act(acc[s][4 * j + 2 * h + 1]);
+                if (a.round_out) { v0 = ptx::round_tf32(v0); v1 = ptx::round_tf32(v1); }
+                if (a.sumsq) part = fmaf(v0, v0, two ? fmaf(v1, v1, part) : part);
+                if (a.no_store) continue;
+                float* y = yrow[s][h];
+                if (two && !((reinterpret_cast<uintptr_t>(y + c)) & 7)) {
+                  *reinterpret_cast<float2*>(y + c) = make_float2(v0, v1);
+                } else {
+                  y[c] = v0;
+                  if (two) y[c + 1] = v1;
+                }
               }
+              sq_acc += (double)part;                           // fp32 within a row of the tile, fp64 across rows and tiles
             }
-            sq_acc += (double)part;                             // fp32 within a row of the tile, fp64 across rows and tiles
           }
+        };
+        switch (a.act) {
+          case ACT_RELU: pass2([](float v) { return epi_act(v, ACT_RELU, 0.f); }); break;
+          case ACT_LEAKY: pass2([&](float v) { return epi_act(v, ACT_LEAKY, a.slope); }); break;
+          case ACT_ELU: pass2([](float v) { return epi_act(v, ACT_ELU, 0.f); }); break;
+          default: pass2([](float v) { return v; }); break;
         }
       }
     }
@@ -988,16 +999,19 @@ static int conv_fwd_impl(int N, int H, int W, int Cin, int Cout, int KH, int KW,
     };
     if (!encode_rows(&ty, y, ldy) || !encode_rows(&tr, residual, ldr)) return 0;
   }
-  // 256-row tiles (two 128-row A boxes per stage, same maps) for the long-K launches, where a 128x128 tile is bound by the operand
-  // bytes per FLOP rather than by the tensor cores: K loops of at least kTile256MinK steps and more than one N tile (DESIGN.md §6:
-  // the 1x1 convolutions, K = 32 / 64, and the 3x3 256-channel ones, K = 72, lose with half the stages and twice the epilogue per
-  // tile; a lone N tile lost as well).  And only where halving the work-unit count adds no ragged wave of 132 CTAs: a 256-row unit
-  // takes two 128-row unit times.
+  // 256-row tiles (two 128-row A boxes per stage, same maps): a 48 KB stage carries twice the MMA work of a 32 KB 128-row stage, and
+  // the operand bytes per FLOP bound both tile shapes (DESIGN.md §3.1, §6).  Measured: with more than one N tile 256 rows won at
+  // every K from 2 to 1152 steps; with a single N tile they won at K = 18 and 72 and lost at K = 16 (1x1 512->128) and K = 288
+  // (3x3 1024->128).  And only where the halved unit count costs no extra time in ragged waves of 132 CTAs: a 256-row unit took
+  // 1.3 - 1.8 times a 128-row unit of the same launch, so the 256-row waves, counted at 1.8 each, must not outlast the 128-row waves.
   const bool tile256_legal = (flat || a.im2col) && bn == 128 && !split3 && a.splits == 1 && !tma_epi && !sumsq && !no_store;
   const long long units128 = (long long)a.m_tiles * a.n_tiles, units256 = (P + 2 * kBlockM - 1) / (2 * kBlockM) * a.n_tiles;
+  const long long waves128 = (units128 + kNumSMs - 1) / kNumSMs, waves256 = (units256 + kNumSMs - 1) / kNumSMs;
+  const int k_steps = KH * KW * a.k_chunks;
   const bool tile256 = tile256_legal && g_tile_m != 1 &&
-                       (g_tile_m == 2 || (KH * KW * a.k_chunks >= kTile256MinK && a.n_tiles > 1 &&
-                                          2 * ((units256 + kNumSMs - 1) / kNumSMs) <= (units128 + kNumSMs - 1) / kNumSMs));
+                       (g_tile_m == 2 ||
+                        (k_steps >= kTile256MinK && (a.n_tiles > 1 || (k_steps >= kTile256OneNMinK && k_steps <= kTile256OneNMaxK)) &&
+                         9 * waves256 <= 5 * waves128));
   if (tile256) { a.BW = 2 * kBlockM; a.tiles_x = (a.OW + a.BW - 1) / a.BW; a.m_tiles = a.tiles_x; }
   a.kc_outer = kc_outer;
   a.reverse = (g_tile_order == 2) ? (g_tile_flip ^= 1) : g_tile_order;
