@@ -235,6 +235,12 @@ void skd_set_conv_tile_m(int mode);    /* wgmma conv M tile: 0 (default) 256 row
 int skd_conv1x1_chain_sm100(int P, int Cin3, int Cout3, int Cout1, const float* x3, int ldx3, const float* w3, const float* scale3,
                             const float* shift3, const float* residual, int ldr, float* y3, int ldy3, const float* w1,
                             const float* scale1, const float* shift1, float* y1, int ldy1, cudaStream_t);
+/* what the host-side dispatch chose for the last wgmma forward launch (any skd_conv2d_fwd_sm100* entry or skd_gemm_nt_sm100):
+   out[7] = {M tile mode (0 flat, 1 im2col, 2 rect), tile rows (128 or 256), BLOCK_N, K splits, TMA epilogue, channel chunks outermost
+   (kc_outer), tile order reversed}.  Reports only; launches are unchanged. */
+void skd_conv_fwd_last_plan(int* out);
+/* the same for the last skd_conv2d_wgrad_sm100: out[3] = {BLOCK_N, linear 32-pixel K blocks, K splits} */
+void skd_conv_wgrad_last_plan(int* out);
 void skd_set_conv_chain(int mode);     /* frozen bottlenecks: 0 (default) chain conv3 with the next block's conv1 where the shapes allow; 1 never */
 int skd_conv_chain_mode(void);
 

@@ -487,6 +487,7 @@ int g_tile_order = 0;             // 0 front-to-back, 1 back-to-front, 2 alterna
 int g_tile_flip = 0;
 int g_k_order = 0;                // 0: by working set (channel chunks outermost when Cin >= 2048); 1: taps outermost; 2: chunks outermost
 int g_tile_m = 0;                 // 0: 256-row tiles by the launch's shape; 1: always 128; 2: 256 wherever the 256-row path can run
+int g_last_plan[7] = {0, 0, 0, 0, 0, 0, 0};   // what conv_fwd_impl chose for its last launch (skd_conv_fwd_last_plan)
 
 EncodeTiledFn get_encode_tiled() {
   static EncodeTiledFn fn = nullptr;
@@ -847,6 +848,7 @@ extern "C" void skd_set_conv_k_order(int mode) { g_k_order = mode; }
 extern "C" void skd_set_conv_tile_m(int mode) { g_tile_m = mode; }
 extern "C" void skd_set_conv_chain(int mode) { g_conv_chain = mode; }
 extern "C" int skd_conv_chain_mode(void) { return g_conv_chain; }
+extern "C" void skd_conv_fwd_last_plan(int* out) { for (int i = 0; i < 7; ++i) out[i] = g_last_plan[i]; }
 
 // ---- split-K for convolutions with few output tiles and a long K loop (the discriminator: 256 .. 4096 output pixels, K up to 4096) ----
 // Without it a 4x8-pixel map at batch 8 is 2 x 2 tiles: 4 of 132 SMs walk 128 K steps each.  Units = tiles x K ranges fill the
@@ -1017,6 +1019,8 @@ static int conv_fwd_impl(int N, int H, int W, int Cin, int Cout, int KH, int KW,
   a.reverse = (g_tile_order == 2) ? (g_tile_flip ^= 1) : g_tile_order;
   a.nstages = 0; a.sumsq = sumsq; a.no_store = no_store;
   if (strided_out && residual) { set_error_msg(who, "strided output takes no residual"); return 0; }
+  const int plan[7] = {flat ? 0 : (a.im2col ? 1 : 2), tile256 ? 2 * kBlockM : kBlockM, bn, a.splits, tma_epi ? 1 : 0, kc_outer ? 1 : 0, a.reverse};
+  for (int i = 0; i < 7; ++i) g_last_plan[i] = plan[i];
   int ok;
   switch (bn) {
     case 128:

@@ -278,6 +278,7 @@ EncodeTiledFn get_encode() {
 struct Plan { int OH, OW, BHk, BWk, kb_x, kb_y, kb_total, bn, m_tiles, n_tiles, taps, splits, kb_per_split, linear; };
 
 int g_wgrad_linear = 1;
+int g_last_plan[3] = {0, 0, 0};   // what skd_conv2d_wgrad_sm100 chose for its last launch (skd_conv_wgrad_last_plan)
 
 Plan make_plan(int N, int H, int W, int Cin, int Cout, int KH, int KW, int stride, int pad, int dil) {
   Plan p;
@@ -335,6 +336,7 @@ int launch(const CUtensorMap& tdy, const CUtensorMap& tx, const WgArgs& a, int u
 }  // namespace
 
 extern "C" void skd_set_wgrad_linear(int on) { g_wgrad_linear = on ? 1 : 0; }
+extern "C" void skd_conv_wgrad_last_plan(int* out) { for (int i = 0; i < 3; ++i) out[i] = g_last_plan[i]; }
 
 extern "C" long long skd_conv2d_wgrad_sm100_workspace_floats(int N, int H, int W, int Cin, int Cout, int KH, int KW, int stride,
                                                              int pad, int dil) {
@@ -416,6 +418,7 @@ extern "C" int skd_conv2d_wgrad_sm100(int N, int H, int W, int Cin, int Cout, in
   a.ws = p.splits == 1 ? dw : workspace;
   a.linear = p.linear;
   const int units = p.m_tiles * p.n_tiles * p.taps * p.splits;
+  g_last_plan[0] = p.bn; g_last_plan[1] = p.linear; g_last_plan[2] = p.splits;
   int ok;
   switch (p.bn) {
     case 128: ok = launch<128>(tdy, tx, a, units, st); break;

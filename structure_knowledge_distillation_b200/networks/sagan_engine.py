@@ -39,6 +39,19 @@ def _f(*shape, dev):
     return torch.empty(shape, device=dev, dtype=torch.float32)
 
 
+def _logged(key, flop, launch):
+    """Run `launch()`; with ops.CONV_EVENT_LOG set, bracket it with CUDA events and log it the way ops.conv2d_fwd does.  Keys are
+    (kind, n, cin, h, w, cout, k, stride, dil) with kind "disc_fwd" or "disc_wgrad"."""
+    log = ops.CONV_EVENT_LOG
+    if log is None:
+        return launch()
+    ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    ev0.record()
+    launch()
+    ev1.record()
+    log.append((ev0, ev1, flop, key))
+
+
 class _Tape:
     pass
 
@@ -136,8 +149,11 @@ class DiscEngine:
         # few output tiles + long K (4x8 .. 16x32 maps): split-K over (tile, K range) units, partial planes in a workspace
         nws = L.skd_conv2d_fwd_sm100_splitk_workspace_floats(n, h, w, cin, cout, k, k, stride, pad, 1, out_hw[0], out_hw[1]) if self.split_k else 0
         ws = torch.empty(nws, device=y.device, dtype=torch.float32) if nws else None
-        L.skd_conv2d_fwd_sm100_splitk(n, h, w, cin, cout, k, k, stride, pad, 1, _p(x), _p(x_lo), ldx, _p(wgt), _p(wgt_lo), _p(y), ldy,
-                                      out_hw[0], out_hw[1], _p(scale), _p(shift), _p(residual), ldr, act, slope, _p(ws), nws, _st())
+        oh, ow = (out_hw[0] or (h + 2 * pad - k) // stride + 1), (out_hw[1] or (w + 2 * pad - k) // stride + 1)
+        _logged(("disc_fwd", n, cin, h, w, cout, k, stride, 1), 2.0 * n * oh * ow * cout * cin * k * k,
+                lambda: L.skd_conv2d_fwd_sm100_splitk(n, h, w, cin, cout, k, k, stride, pad, 1, _p(x), _p(x_lo), ldx, _p(wgt), _p(wgt_lo), _p(y),
+                                                      ldy, out_hw[0], out_hw[1], _p(scale), _p(shift), _p(residual), ldr, act, slope, _p(ws), nws,
+                                                      _st()))
 
     def _split(self, t, rows=None):
         """lo part of the first `rows` leading entries of t (whole tensor by default), same shape as t"""
@@ -285,7 +301,9 @@ class DiscEngine:
                     dw = _f(a["ldq"], a["c"], dev=dev)
                     nws = L.skd_conv2d_wgrad_sm100_workspace_floats(nb, oh, ow, a["c"], a["ldq"], 1, 1, 1, 0, 1)
                     wsg = _f(max(nws, 4), dev=dev)
-                    L.skd_conv2d_wgrad_sm100(nb, oh, ow, a["c"], a["ldq"], 1, 1, 1, 0, 1, _p(hx), a["c"], _p(gqkv), a["ldq"], _p(dw), _p(wsg), st)
+                    _logged(("disc_wgrad", nb, a["c"], oh, ow, a["ldq"], 1, 1, 1), 2.0 * nb * oh * ow * a["c"] * a["ldq"],
+                            lambda: L.skd_conv2d_wgrad_sm100(nb, oh, ow, a["c"], a["ldq"], 1, 1, 1, 0, 1, _p(hx), a["c"], _p(gqkv), a["ldq"], _p(dw),
+                                                             _p(wsg), st))
                     db = _f(a["ldq"], dev=dev)
                     L.skd_colsum(B * n, a["ldq"], _p(gqkv), a["ldq"], _p(db), st)    # the tangent projections carry no bias
                     off = 0
@@ -319,7 +337,9 @@ class DiscEngine:
                 dwn = _f(cout, 16, cin_p, dev=dev)
                 nws = L.skd_conv2d_wgrad_sm100_workspace_floats(nb, hin_hw[0], hin_hw[1], cin_p, cout, 4, 4, 2, 1, 1)
                 wsg = _f(max(nws, 4), dev=dev)
-                L.skd_conv2d_wgrad_sm100(nb, hin_hw[0], hin_hw[1], cin_p, cout, 4, 4, 2, 1, 1, _p(hin), cin_p, _p(g), cout, _p(dwn), _p(wsg), st)
+                _logged(("disc_wgrad", nb, cin_p, hin_hw[0], hin_hw[1], cout, 4, 2, 1), 2.0 * nb * oh * ow * cout * cin_p * 16,
+                        lambda: L.skd_conv2d_wgrad_sm100(nb, hin_hw[0], hin_hw[1], cin_p, cout, 4, 4, 2, 1, 1, _p(hin), cin_p, _p(g), cout, _p(dwn),
+                                                         _p(wsg), st))
                 dw, acc = self._grad_buf(sink, names[li] + ".weight_bar", m.weight_bar)
                 # d sigma / d w_bar = u v^T with the module's CURRENT u, v, not this forward's: the reference rebinds `u.data` / `v.data`
                 # in every forward (spectral.py:30-31) and autograd's saved references to u and v see the latest values, so the backward
@@ -616,8 +636,9 @@ class SNConvFn(torch.autograd.Function):
         L.skd_sn_power_iter(cout, taps, cin, _p(wq), _p(m.weight_u), _p(m.weight_v), _p(s["u"]), _p(s["v"]), _p(s["sigma"]), _p(s["inv"]), cout, st)
         oh, ow = ops.conv_out_hw(h, w, (kh, kw), m.stride, m.padding, m.dilation)
         y = ops.empty_nhwc(n, cout, oh, ow, dev)
-        L.skd_conv2d_fwd_sm100_ex(n, h, w, cin, cout, kh, kw, m.stride, m.padding, m.dilation, _p(x), None, ldx, _p(wq), None, _p(y), cout, 0, 0,
-                                  _p(s["inv"]), _p(bias), None, 0, ACT_NONE, 0.0, st)
+        _logged(("disc_fwd", n, cin, h, w, cout, kh, m.stride, m.dilation), 2.0 * n * oh * ow * cout * cin * kh * kw,
+                lambda: L.skd_conv2d_fwd_sm100_ex(n, h, w, cin, cout, kh, kw, m.stride, m.padding, m.dilation, _p(x), None, ldx, _p(wq), None, _p(y),
+                                                  cout, 0, 0, _p(s["inv"]), _p(bias), None, 0, ACT_NONE, 0.0, st))
         ctx.save_for_backward(x, w_bar, s["u"], s["v"], s["sigma"])
         ctx.m = m
         ctx.has_bias = bias is not None
@@ -665,8 +686,9 @@ class SelfAttnFn(torch.autograd.Function):
         x_lo, w_lo = torch.empty_like(x), torch.empty_like(wcat)
         L.skd_split_tf32(x.numel(), _p(x), None, _p(x_lo), st)
         L.skd_split_tf32(wcat.numel(), _p(wcat), None, _p(w_lo), st)
-        L.skd_conv2d_fwd_sm100_ex(1, 1, n_img * n, c, ldq, 1, 1, 1, 0, 1, _p(x), _p(x_lo), c, _p(wcat), _p(w_lo), _p(qkv), ldq, 0, 0, None, _p(bias),
-                                  None, 0, ACT_NONE, 0.0, st)
+        _logged(("disc_fwd", 1, c, 1, n_img * n, ldq, 1, 1, 1), 2.0 * n_img * n * c * ldq,
+                lambda: L.skd_conv2d_fwd_sm100_ex(1, 1, n_img * n, c, ldq, 1, 1, 1, 0, 1, _p(x), _p(x_lo), c, _p(wcat), _p(w_lo), _p(qkv), ldq, 0, 0,
+                                                  None, _p(bias), None, 0, ACT_NONE, 0.0, st))
         attn, o = _f(n_img, n, n, dev=dev), _f(n_img * n, c, dev=dev)
         y = ops.empty_nhwc(n_img, c, h, w, dev)
         L.skd_attn_fwd(n_img, n, c, d, _p(qkv), ldq, _p(x), _p(A.gamma), _p(attn), _p(o), _p(y), None, st)
@@ -693,14 +715,16 @@ class SelfAttnFn(torch.autograd.Function):
                        _p(wsf), st)
         dw = _f(ldq, c, dev=dev)
         wsg = _f(max(L.skd_conv2d_wgrad_sm100_workspace_floats(n_img, h, w, c, ldq, 1, 1, 1, 0, 1), 4), dev=dev)
-        L.skd_conv2d_wgrad_sm100(n_img, h, w, c, ldq, 1, 1, 1, 0, 1, _p(x), c, _p(gqkv), ldq, _p(dw), _p(wsg), st)
+        _logged(("disc_wgrad", n_img, c, h, w, ldq, 1, 1, 1), 2.0 * n_img * n * c * ldq,
+                lambda: L.skd_conv2d_wgrad_sm100(n_img, h, w, c, ldq, 1, 1, 1, 0, 1, _p(x), c, _p(gqkv), ldq, _p(dw), _p(wsg), st))
         db = _f(ldq, dev=dev)
         L.skd_colsum(n_img * n, ldq, _p(gqkv), ldq, _p(db), st)
         wt = _f(c, ldq, dev=dev)
         L.skd_weight_flip_transpose(ldq, c, 1, 1, _p(wcat), _p(wt), 0, st)
         gx = ops.empty_nhwc(n_img, c, h, w, dev)
-        L.skd_conv2d_fwd_sm100_ex(1, 1, n_img * n, ldq, c, 1, 1, 1, 0, 1, _p(gqkv), None, ldq, _p(wt), None, _p(gx), c, 0, 0, None, None, _p(gy), c,
-                                  ACT_NONE, 0.0, st)
+        _logged(("disc_fwd", 1, ldq, 1, n_img * n, c, 1, 1, 1), 2.0 * n_img * n * c * ldq,
+                lambda: L.skd_conv2d_fwd_sm100_ex(1, 1, n_img * n, ldq, c, 1, 1, 1, 0, 1, _p(gqkv), None, ldq, _p(wt), None, _p(gx), c, 0, 0, None,
+                                                  None, _p(gy), c, ACT_NONE, 0.0, st))
         by_name = {"query_conv.weight": dw[:d].view(d, c, 1, 1), "query_conv.bias": db[:d], "key_conv.weight": dw[d:2 * d].view(d, c, 1, 1),
                    "key_conv.bias": db[d:2 * d], "value_conv.weight": dw[2 * d:].view(c, c, 1, 1), "value_conv.bias": db[2 * d:], "gamma": ggam}
         return (None, gx) + tuple(by_name[nm] for nm, _ in A.named_parameters())
