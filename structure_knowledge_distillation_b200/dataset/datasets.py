@@ -22,6 +22,7 @@ import collections
 import ctypes
 import os.path as osp
 import random
+import struct
 
 import numpy as np
 import torch
@@ -61,9 +62,82 @@ def draw_augmentation(src_h, src_w, crop_size, scale=True, mirror=True, scales=C
     return Augmentation(scale_idx, f_scale, sh, sw, h_off, w_off, flip)
 
 
+_SOF = {0xC0, 0xC1, 0xC2, 0xC3, 0xC5, 0xC6, 0xC7, 0xC9, 0xCA, 0xCB, 0xCD, 0xCE, 0xCF}
+
+
+def _header_size(path):
+    """(height, width) of a PNG or JPEG file from its header, or None when the header does not settle what `cv2.imread(path,
+    IMREAD_COLOR)` returns: another format, or EXIF data, whose orientation tag cv2 applies (it may swap the two)."""
+    with open(path, "rb") as f:
+        head = f.read(8)
+        if head == b"\x89PNG\r\n\x1a\n":
+            size = None
+            while True:
+                chunk = f.read(8)
+                if len(chunk) < 8:
+                    return None
+                n, typ = struct.unpack(">I4s", chunk)
+                if typ == b"IHDR":
+                    w, h = struct.unpack(">II", f.read(8))
+                    size = (h, w)
+                    f.seek(n - 8 + 4, 1)
+                elif typ == b"eXIf":
+                    return None
+                elif typ == b"IDAT":
+                    return size
+                else:
+                    f.seek(n + 4, 1)
+        if head[:2] != b"\xff\xd8":
+            return None
+        f.seek(2)
+        while True:
+            b = f.read(1)
+            while b == b"\xff":                                          # fill bytes before a marker
+                m = f.read(1)
+                if m != b"\xff":
+                    break
+            else:
+                return None
+            if not m:
+                return None
+            m = m[0]
+            if m == 0x01 or 0xD0 <= m <= 0xD8:                          # markers without a length
+                continue
+            if m == 0xD9:                                                # end of image before any frame header
+                return None
+            seg = f.read(2)
+            if len(seg) < 2:
+                return None
+            n = struct.unpack(">H", seg)[0]
+            if m in _SOF:
+                _, h, w = struct.unpack(">BHH", f.read(5))
+                return h, w
+            if m == 0xE1 and f.read(6) == b"Exif\x00\x00":
+                return None
+            if m == 0xE1:
+                f.seek(n - 2 - 6, 1)
+            else:
+                f.seek(n - 2, 1)
+
+
+def image_size(path):
+    """(height, width) of the image `cv2.imread(path, cv2.IMREAD_COLOR)` returns.  Read from the PNG / JPEG header (no decode); other
+    formats and files with EXIF data are decoded in full (for a 2048 x 1024 PNG, the cost of one `__getitem__`'s image read)."""
+    size = _header_size(path)
+    if size is not None:
+        return size
+    import cv2
+    image = cv2.imread(path, cv2.IMREAD_COLOR)
+    if image is None:
+        raise IOError("cannot read %s" % path)
+    return image.shape[:2]
+
+
 class CSDataSet(data.Dataset):
     """Same constructor as the reference (datasets.py:122).  `__getitem__` returns the RAW decoded files and the drawn augmentation:
     (image uint8 H x W x 3 BGR, label uint8 H x W, aug float64[7], size int[3], name)."""
+
+    scales = CS_SCALES
 
     def __init__(self, root, list_path, max_iters=None, crop_size=(321, 321), mean=(128, 128, 128), scale=True, mirror=True, ignore_label=255):
         self.root, self.list_path = root, list_path
@@ -89,7 +163,7 @@ class CSDataSet(data.Dataset):
         label = cv2.imread(f["label"], cv2.IMREAD_GRAYSCALE)
         if image is None or label is None:
             raise IOError("cannot read %s / %s" % (f["img"], f["label"]))
-        aug = draw_augmentation(image.shape[0], image.shape[1], (self.crop_h, self.crop_w), self.scale, self.is_mirror)
+        aug = draw_augmentation(image.shape[0], image.shape[1], (self.crop_h, self.crop_w), self.scale, self.is_mirror, self.scales)
         return (torch.from_numpy(image), torch.from_numpy(label), torch.tensor(aug, dtype=torch.float64), np.array(image.shape), f["name"])
 
 
@@ -192,6 +266,8 @@ class VOCDataSet(data.Dataset):
     decoded files and the drawn augmentation (image uint8 H x W x 3 BGR, label uint8 H x W, aug float64[7], size int[3], name).
     Labels are class ids and pass through unchanged; the mean is subtracted on the GPU with numpy's type (`numpy_mean`)."""
 
+    scales = VOC_SCALES
+
     def __init__(self, root, list_path, max_iters=None, crop_size=(321, 321), mean=(128, 128, 128), scale=True, mirror=True, ignore_label=255):
         self.root, self.list_path = root, list_path
         self.crop_h, self.crop_w = crop_size
@@ -213,7 +289,7 @@ class VOCDataSet(data.Dataset):
         label = cv2.imread(f["label"], cv2.IMREAD_GRAYSCALE)
         if image is None or label is None:
             raise IOError("cannot read %s / %s" % (f["img"], f["label"]))
-        aug = draw_augmentation(image.shape[0], image.shape[1], (self.crop_h, self.crop_w), self.scale, self.is_mirror, VOC_SCALES)
+        aug = draw_augmentation(image.shape[0], image.shape[1], (self.crop_h, self.crop_w), self.scale, self.is_mirror, self.scales)
         return (torch.from_numpy(image), torch.from_numpy(label), torch.tensor(aug, dtype=torch.float64), np.array(image.shape), f["name"])
 
 
@@ -353,11 +429,37 @@ def _collate(batch):
             torch.from_numpy(np.stack(sizes)), list(names))
 
 
+class _ReplayDraws:
+    """worker_init_fn of a resumed iteration: worker `w` makes, without reading the files, the `draw_augmentation` calls it made for
+    the batches it loaded before batch `start` of the interrupted iteration (batches go to the workers round-robin: batch b to worker
+    b % num_workers), so its `random` / `np.random` continue where they were.  Image sizes come from the file headers (`image_size`),
+    once per distinct file."""
+
+    def __init__(self, dataset, order, batch_size, start, num_workers):
+        self.dataset, self.order, self.batch_size, self.start, self.num_workers = dataset, order, batch_size, start, num_workers
+
+    def __call__(self, worker_id):
+        ds, sizes = self.dataset, {}
+        for b in range(worker_id, self.start, self.num_workers):
+            for index in self.order[b * self.batch_size:(b + 1) * self.batch_size]:
+                path = ds.files[index]["img"]
+                if path not in sizes:
+                    sizes[path] = image_size(path)
+                h, w = sizes[path]
+                draw_augmentation(h, w, (ds.crop_h, ds.crop_w), ds.scale, ds.is_mirror, ds.scales)
+
+
 class CSDataLoader:
     """Drop-in for `data.DataLoader(CSDataSet(...), batch_size=..., shuffle=True, num_workers=4, pin_memory=True)` of
     train_and_eval.py:13-15: iterating it yields `(images, labels, size, name)` with images / labels already augmented and on the GPU,
     for a `CSDataSet` or a `VOCDataSet`.  With a `CSDataTestSet` (test.py:9-10) it yields `(images, size, name)`, with a
-    `VOCDataTestSet` `(images, name, size)` (the reference's orders), images mean-subtracted and padded on the GPU."""
+    `VOCDataTestSet` `(images, name, size)` (the reference's orders), images mean-subtracted and padded on the GPU.
+
+    A training loader can be resumed: `state_dict()` is the position of the current iteration, and after `load_state_dict(sd)` the
+    next iteration yields the batches that iteration had not yet yielded -- the same samples in the same order with the same
+    augmentation draws.  With num_workers > 0 the workers' draws are replayed; with num_workers == 0 they come from this process's
+    `random` / `np.random`, which must be restored too (`StepModel.load_training_state` does both).  Without a loaded position every
+    iteration is torch's DataLoader's, unchanged."""
 
     def __init__(self, dataset, batch_size=1, shuffle=False, num_workers=0, pin_memory=True, drop_last=False, label_dtype=torch.int64,
                  device=None):
@@ -373,6 +475,8 @@ class CSDataLoader:
         else:
             self.augment = DeviceAugment((dataset.crop_h, dataset.crop_w), dataset.mean, dataset.ignore_label, label_dtype, device, self.voc,
                                          getattr(dataset, "label_table", None))
+        self._shuffle = shuffle
+        self._iter_rng, self._yielded, self._resume = None, 0, None
 
     def __len__(self):
         return len(self.loader)
@@ -382,6 +486,68 @@ class CSDataLoader:
             for images, sizes, names in self.loader:
                 yield (self.augment(images), names, sizes) if self.voc else (self.augment(images), sizes, names)
             return
-        for images, labels, augs, sizes, names in self.loader:
+        for images, labels, augs, sizes, names in self.host_batches():
             out_i, out_l = self.augment(images, labels, augs)
             yield out_i, out_l, sizes, names
+
+    # ---- resuming ---------------------------------------------------------------------------------------------------------------
+    def host_batches(self):
+        """One iteration's raw training batches `(images, labels, augs, sizes, names)` as the workers return them, before the device
+        step (what `__iter__` augments): the rest of an interrupted iteration after `load_state_dict`, else a whole new one."""
+        if self.test:
+            raise ValueError("only a training loader (CSDataSet / VOCDataSet) yields augmentation batches")
+        resume, self._resume = self._resume, None
+        if resume is None:
+            # torch's iterator draws the workers' base seed and then the sampler's seed from the default generator: its state here
+            # fixes both
+            self._iter_rng, self._yielded = torch.get_rng_state(), 0
+            it, skip = iter(self.loader), 0
+        else:
+            self._iter_rng, self._yielded = resume
+            it, skip = self._resumed(*resume)
+        for batch in it:
+            if skip:
+                skip -= 1
+                continue
+            self._yielded += 1
+            yield batch
+
+    def _resumed(self, rng, start):
+        """-> (iterator, batches to drop): torch's iterator of the interrupted iteration, rebuilt from the default generator's state
+        `rng` at its start, beginning at the first batch >= start - num_workers + 1 whose worker is the one that loaded it then."""
+        n, bs, workers = len(self.dataset), self.loader.batch_size, self.loader.num_workers
+        g = torch.Generator()
+        g.set_state(rng)
+        torch.empty((), dtype=torch.int64).random_(generator=g)              # the workers' base seed
+        order = list(range(n))
+        if self._shuffle:                                                    # RandomSampler: a seed, then randperm from it
+            seed = int(torch.empty((), dtype=torch.int64).random_(generator=g).item())
+            order = torch.randperm(n, generator=torch.Generator().manual_seed(seed)).tolist()
+        first = start - start % workers if workers else start
+        base = torch.Generator()
+        base.set_state(rng)                                                  # the DataLoader draws the same base seed from it
+        loader = data.DataLoader(self.dataset, batch_size=bs, sampler=order[first * bs:], num_workers=workers,
+                                 pin_memory=self.loader.pin_memory, drop_last=self.loader.drop_last, collate_fn=self.loader.collate_fn,
+                                 generator=base, worker_init_fn=_ReplayDraws(self.dataset, order, bs, first, workers) if first else None)
+        return iter(loader), start - first
+
+    def state_dict(self):
+        """The position of the current (or last) iteration: the default generator's state when it began, and the number of batches
+        it has yielded."""
+        if self.test:
+            raise ValueError("only a training loader (CSDataSet / VOCDataSet) can be resumed")
+        return dict(version=1, rng_state=self._iter_rng, batches=self._yielded, num_samples=len(self.dataset),
+                    batch_size=self.loader.batch_size, shuffle=self._shuffle, num_workers=self.loader.num_workers)
+
+    def load_state_dict(self, sd):
+        """The next iteration continues the one `sd` describes (state_dict of a loader over the same list, batch size, shuffle and
+        worker count); a mismatch raises ValueError naming the field, and changes nothing."""
+        if self.test:
+            raise ValueError("only a training loader (CSDataSet / VOCDataSet) can be resumed")
+        want = dict(version=1, num_samples=len(self.dataset), batch_size=self.loader.batch_size, shuffle=self._shuffle,
+                    num_workers=self.loader.num_workers)
+        for k, v in want.items():
+            if sd.get(k) != v:
+                raise ValueError("loader state does not match the loader: %s is %r, the loader's %r" % (k, sd.get(k), v))
+        if sd["rng_state"] is not None:                                      # None: no iteration had begun, nothing to skip
+            self._resume = (sd["rng_state"].clone(), int(sd["batches"]))

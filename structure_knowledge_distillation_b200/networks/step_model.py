@@ -7,16 +7,22 @@ once and replayed from staged inputs.
 
 A subclass builds its networks and defines two hooks: `_phase()`, everything a step does before the optimizer updates (what the
 CUDA graph captures), and `_update()`, the updates that stay eager after it (StepModel's: the student's all-reduce and SGD step).
+
+`save_training_state` / `load_training_state` write and restore everything a run needs to continue where it stopped (DESIGN.md §8).
 """
 import os
 import os.path as osp
+import random
+import tempfile
 
+import numpy as np
 import torch
 import torch.distributed as dist
 
 from .. import functions as Fn
 from ..optim import FlatSGD
 from ..utils.criterion import CriterionCrossEntropy, CriterionDSN, CriterionOhemDSN, check_task_loss_weights
+from ..utils.utils import _torch_load
 from .espnet import ESPNet, ESPNet_C
 from .evaluate import evaluate_main
 from .mobilenet import MobileNetV2
@@ -46,6 +52,45 @@ class _LazyScalar:
 
 def _arg(args, name, default):
     return getattr(args, name, default)
+
+
+TRAINING_STATE_FORMAT = "skd-training-state"
+TRAINING_STATE_VERSION = 1
+
+
+def _cpu_state(module):
+    return {k: v.detach().cpu().clone() for k, v in module.state_dict().items()}
+
+
+def _check_state_dict(field, have, saved):
+    """ValueError naming `field` unless `saved` has exactly the keys and shapes of the module state dict `have`."""
+    if not isinstance(saved, dict) or set(saved) != set(have):
+        missing, extra = sorted(set(have) - set(saved or ())), sorted(set(saved or ()) - set(have))
+        raise ValueError("training state does not match the model: %s keys differ (missing %s, unexpected %s)"
+                         % (field, missing[:5], extra[:5]))
+    for k, v in have.items():
+        if tuple(saved[k].shape) != tuple(v.shape):
+            raise ValueError("training state does not match the model: %s[%r] has shape %s, the model's %s"
+                             % (field, k, tuple(saved[k].shape), tuple(v.shape)))
+
+
+def _rng_states(device, loader):
+    """This process's random streams: torch CPU, the CUDA generator of `device`, Python `random`, numpy's global generator (as plain
+    values, so the file loads with weights_only=True), and `loader`'s position."""
+    name, keys, pos, has_gauss, gauss = np.random.get_state()
+    return dict(torch=torch.get_rng_state(), cuda=torch.cuda.get_rng_state(device) if device.type == "cuda" else None,
+                random=random.getstate(), numpy=(name, torch.from_numpy(keys.astype(np.int64)), int(pos), int(has_gauss), float(gauss)),
+                loader=None if loader is None else loader.state_dict())
+
+
+def _set_rng_states(st, device):
+    torch.set_rng_state(st["torch"])
+    if st["cuda"] is not None and device.type == "cuda":
+        # sets the generator's seed and Philox offset in place: a captured CUDA graph reads both from the generator at every replay
+        torch.cuda.set_rng_state(st["cuda"], device)
+    random.setstate(st["random"])
+    name, keys, pos, has_gauss, gauss = st["numpy"]
+    np.random.set_state((name, keys.numpy().astype(np.uint32), pos, has_gauss, gauss))
 
 
 def build_seg_network(kind, classes_num, args=None):
@@ -81,7 +126,7 @@ class StepModel():
         kind = str(_arg(self.args, option, default))
         if kind not in kinds:
             raise ValueError("%s must be one of %s (got %r)" % (option, ", ".join(repr(k) for k in kinds), kind))
-        self.kind = kind
+        self.kind, self.kind_option = kind, option
         # the ESPNets have no auxiliary head (single-head cross entropy) and issue their weight gradients on the main stream
         self.espnet = kind in ("espnet_c", "espnet")
         if _arg(self.args, "sync_bn", False) and (self.espnet or kind == "mobilenetv2"):
@@ -273,3 +318,116 @@ class StepModel():
         path = osp.join(self.args.snapshot_dir, 'CS_scenes_' + str(step) + '_' + str(mean_IU) + '.pth')
         torch.save(self._net.state_dict(), path)
         return path
+
+    # ---- resuming a run --------------------------------------------------------------------------------------------------------
+    def _trained(self):
+        """[(field prefix, module, FlatSGD)]: the trained network, and NetModel's discriminator."""
+        parts = [("", self._net, self.G_solver)]
+        if getattr(self, "D_solver", None) is not None:
+            parts.append(("D_", self.D_model, self.D_solver))
+        return parts
+
+    def save_training_state(self, path, step, epoch=0, best_mean_IU=None, IU_array=None, loader=None):
+        """Writes everything needed to continue this run after step `step` (best_mean_IU defaults to self.best_mean_IU) to `path`,
+        one torch.save dict:
+          * `state_dict`, `step`, `epoch`, `best_mean_IU`, `IU_array` -- the reference's checkpoint keys: renamed to model_best.pth.tar
+            in S_ckpt_path / ckpt_path, the file loads through load_S_model / load_seg_model (S_resume / resume) like the reference's;
+          * `D_state_dict` (spectral-norm u / v, BN buffers included), `G_solver` / `D_solver` (momentum, steps, lr, flat length);
+          * `ranks`: per rank, the torch CPU and CUDA generators, Python `random`, numpy's global generator and `loader.state_dict()`;
+          * `format`, `version`, `world_size`, `kind`, `classes_num`: what load_training_state checks.
+        Collective: every rank calls it.  Rank 0 writes a temporary file beside `path` and renames it over `path`, so an interrupted
+        write leaves the previous file as it was; no rank returns before the file is complete (or before every rank raised)."""
+        rank = dist.get_rank() if self.world > 1 else 0
+        solvers = {prefix + "solver": dict(s.state_dict(), numel=s.flat_m.numel()) for prefix, _, s in self._trained()}  # collective (NVLS)
+        mine = _rng_states(self.device, loader)
+        ranks = [None] * self.world
+        if self.world > 1:
+            dist.all_gather_object(ranks, mine)
+        else:
+            ranks[0] = mine
+        err = None
+        if rank == 0:
+            state = dict(format=TRAINING_STATE_FORMAT, version=TRAINING_STATE_VERSION, world_size=self.world,
+                         kind=(self.kind_option, self.kind), classes_num=int(self.args.classes_num),
+                         step=int(step), epoch=int(epoch), best_mean_IU=float(self.best_mean_IU if best_mean_IU is None else best_mean_IU),
+                         IU_array=None if IU_array is None else np.asarray(IU_array, dtype=np.float64), ranks=ranks)
+            for prefix, module, _ in self._trained():
+                state[prefix + "state_dict"] = _cpu_state(module)
+            state["G_solver"] = solvers["solver"]
+            state["D_solver"] = solvers.get("D_solver")
+            for k in ("G_solver", "D_solver"):
+                if state[k] is not None:
+                    state[k]["momentum"] = state[k]["momentum"].cpu()
+            err = self._write_atomically(state, path)
+        if self.world > 1:
+            box = [err]
+            dist.broadcast_object_list(box, 0)                     # doubles as the barrier: rank 0 has renamed (or failed)
+            err = box[0]
+        if err is not None:
+            raise RuntimeError("writing the training state to %s failed: %s" % (path, err))
+
+    @staticmethod
+    def _write_atomically(state, path):
+        """torch.save to a temporary file in `path`'s directory, fsync, rename over `path` -> None, or the error's text (the temporary
+        file removed, `path` untouched)."""
+        d = osp.dirname(osp.abspath(path))
+        fd, tmp = tempfile.mkstemp(dir=d, prefix="." + osp.basename(path) + ".", suffix=".tmp")
+        try:
+            with os.fdopen(fd, "wb") as f:
+                torch.save(state, f)
+                f.flush()
+                os.fsync(f.fileno())
+            os.replace(tmp, path)
+        except Exception as e:                                     # noqa: BLE001
+            if osp.exists(tmp):
+                os.remove(tmp)
+            return repr(e)
+        return None
+
+    def load_training_state(self, path, loader=None):
+        """Restores what save_training_state wrote, in place: the network's and the discriminator's parameters (copied into the
+        existing flat buffers), BN buffers and spectral-norm u / v, both solvers' momentum, step counts and lr, and this rank's random
+        generators -- so a step already captured in a CUDA graph keeps replaying, now from the restored state -- and, when `loader`
+        is given, its position (CSDataLoader.load_state_dict: the next iteration yields the rest of the interrupted one).  Sets
+        args.last_step / start_epoch / best_mean_IU and self.best_mean_IU -> the saved step.
+        A file that does not match this model (format version, kind, classes_num, world size, flat-buffer lengths, state-dict keys or
+        shapes, a loader position when `loader` is given) raises ValueError naming the field before anything is modified."""
+        ck = _torch_load(path)
+        rank = dist.get_rank() if self.world > 1 else 0
+
+        def mismatch(field, got, want):
+            raise ValueError("training state %s does not match the model: %s is %r, the model's %r" % (path, field, got, want))
+
+        if not isinstance(ck, dict) or ck.get("format") != TRAINING_STATE_FORMAT:
+            mismatch("format", ck.get("format") if isinstance(ck, dict) else type(ck).__name__, TRAINING_STATE_FORMAT)
+        if ck.get("version") != TRAINING_STATE_VERSION:
+            mismatch("version", ck.get("version"), TRAINING_STATE_VERSION)
+        if tuple(ck["kind"]) != (self.kind_option, self.kind):
+            mismatch("kind", tuple(ck["kind"]), (self.kind_option, self.kind))
+        if ck["classes_num"] != int(self.args.classes_num):
+            mismatch("classes_num", ck["classes_num"], int(self.args.classes_num))
+        if ck["world_size"] != self.world:
+            mismatch("world_size", ck["world_size"], self.world)
+        parts = self._trained()
+        for prefix, module, solver in parts:
+            field = "G_solver" if prefix == "" else "D_solver"
+            got = None if ck.get(field) is None else ck[field]["numel"]
+            if got != solver.flat_m.numel() or tuple(ck[field]["momentum"].shape) != (solver.flat_m.numel(),):
+                mismatch(field + ".numel", got, solver.flat_m.numel())
+            _check_state_dict(prefix + "state_dict", module.state_dict(), ck.get(prefix + "state_dict"))
+        if len(parts) == 1 and ck.get("D_solver") is not None:
+            mismatch("D_solver", "a discriminator", None)
+        mine = ck["ranks"][rank]
+        if loader is not None:
+            if mine.get("loader") is None:
+                mismatch("ranks[%d].loader" % rank, None, "a CSDataLoader position")
+            loader.load_state_dict(mine["loader"])                  # checks its fields first; sets nothing but the pending position
+
+        with torch.no_grad():
+            for prefix, module, solver in parts:
+                module.load_state_dict(ck[prefix + "state_dict"])      # copy_ into the existing tensors (flat-buffer views)
+                solver.load_state_dict(ck["G_solver" if prefix == "" else "D_solver"])
+        _set_rng_states(mine, self.device)
+        self.args.last_step, self.args.start_epoch = ck["step"], ck["epoch"]
+        self.args.best_mean_IU = self.best_mean_IU = ck["best_mean_IU"]
+        return ck["step"]
