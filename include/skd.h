@@ -241,6 +241,13 @@ int skd_conv1x1_chain_sm100(int P, int Cin3, int Cout3, int Cout1, const float* 
 void skd_conv_fwd_last_plan(int* out);
 /* the same for the last skd_conv2d_wgrad_sm100: out[3] = {BLOCK_N, linear 32-pixel K blocks, K splits} */
 void skd_conv_wgrad_last_plan(int* out);
+/* weight-gradient work units run two to a CTA: for Cout >= 256 (BLOCK_N 128) two adjacent full 128-row Cout tiles with the same
+   split, tap and Cin tile, sharing one X transposition; for Cout <= 64 (BLOCK_N <= 64) any two units, one per consumer warpgroup.
+   Every dW bit is the same in all modes.  0: never; 1 (default): the number of pairs that minimises the predicted makespan over the
+   persistent CTAs; 2: every such pair */
+void skd_set_wgrad_pairing(int mode);
+/* the number of pair units of the last skd_conv2d_wgrad_sm100: out[0] */
+void skd_conv_wgrad_last_pairs(int* out);
 void skd_set_conv_chain(int mode);     /* frozen bottlenecks: 0 (default) chain conv3 with the next block's conv1 where the shapes allow; 1 never */
 int skd_conv_chain_mode(void);
 
