@@ -321,8 +321,9 @@ def test_discriminator_wgangp_matches_reference_golden():
     Parameter gradients: per-tensor norm within 1e-2, the 16 sampled elements within 1e-1 rel-L2.  Why not tighter: the forward is
     fp32-grade (3xTF32, ~1e-5 per convolution) but not bit-identical, and LeakyReLU'(z) jumps from 0.1 to 1 at z = 0 -- one
     activation among the 32 768 of the top layer whose sign differs moves every gradient below it by 0.9 / sqrt(32768) = 5e-3
-    (tools/debug_disc_chain.py shows the adjoint exact to 7e-7 up to the first mask and 4e-3 right after it; the reference's own
-    stock path on this GPU, cuDNN with TF32 allowed, deviates 2e-2 from float64 by the same mechanism)."""
+    (the reference's own stock path on this GPU, cuDNN with TF32 allowed, deviates 2e-2 from float64 by the same mechanism).
+    tests/test_disc_pinned_gpu.py removes that cause: its float64 oracle runs with the masks the GPU chose, and the same sequence
+    agrees to fp32 rounding (3e-5, TF32 weight gradients 1.5e-3)."""
     from oracle import cases, port
     from structure_knowledge_distillation_b200.networks.sagan_models import Discriminator
     from structure_knowledge_distillation_b200.utils.criterion import CriterionAdditionalGP, CriterionAdv
