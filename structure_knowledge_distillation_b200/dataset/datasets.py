@@ -43,23 +43,46 @@ CS_SCALES = (0.7, 14)                     # CSDataSet.generate_scale_label (data
 VOC_SCALES = (0.5, 11)                    # VOCDataSet.generate_scale_label (datasets.py:40)
 
 
-def draw_augmentation(src_h, src_w, crop_size, scale=True, mirror=True, scales=CS_SCALES):
+def draw_augmentation(src_h, src_w, crop_size, scale=True, mirror=True, scales=CS_SCALES, py_random=random, np_random=np.random):
     """The random numbers of one `CSDataSet.__getitem__` call (`VOCDataSet` with scales=VOC_SCALES), drawn in the reference's order
     from the same generators: `random.randint(0, 14)` (datasets.py:156; VOC: randint(0, 11), :40), `random.randint` for h_off then
-    w_off (:196-197), `np.random.choice(2)` (:204)."""
+    w_off (:196-197), `np.random.choice(2)` (:204).  `py_random` / `np_random` replace the module-level `random` / `np.random`
+    streams (a `random.Random` and a `np.random.RandomState`, as `keyed_generators` returns)."""
     crop_h, crop_w = crop_size
     scale_idx, f_scale, sh, sw = -1, 1.0, src_h, src_w
     if scale:
-        scale_idx = random.randint(0, scales[1])
+        scale_idx = py_random.randint(0, scales[1])
         f_scale = scales[0] + scale_idx / 10.0
         sh, sw = _cv_round(src_h * f_scale), _cv_round(src_w * f_scale)
     img_h, img_w = max(sh, crop_h), max(sw, crop_w)                    # after padding (:183-193)
-    h_off = random.randint(0, img_h - crop_h)
-    w_off = random.randint(0, img_w - crop_w)
+    h_off = py_random.randint(0, img_h - crop_h)
+    w_off = py_random.randint(0, img_w - crop_w)
     flip = 1
     if mirror:
-        flip = int(np.random.choice(2)) * 2 - 1
+        flip = int(np_random.choice(2)) * 2 - 1
     return Augmentation(scale_idx, f_scale, sh, sw, h_off, w_off, flip)
+
+
+# The first spawn-key word keeps the permutation's stream and the draws' streams apart; numpy pads the seed's words before the key,
+# so no two (seed, key) pairs share a stream.
+_ORDER_KEY, _DRAW_KEY = 0, 1
+
+
+def partition_order(n, seed, iteration, shuffle=True):
+    """-> the sample order of iteration `iteration` of a partitioned `CSDataLoader` over `n` samples: a permutation of range(n)
+    keyed by (seed, iteration), or the identity without `shuffle`.  The same on every rank and in every process."""
+    if not shuffle:
+        return list(range(n))
+    ss = np.random.SeedSequence(seed, spawn_key=(_ORDER_KEY, iteration, 0))
+    return np.random.Generator(np.random.PCG64(ss)).permutation(n).tolist()
+
+
+def keyed_generators(seed, iteration, position):
+    """-> (random.Random, np.random.RandomState) for the augmentation draws of the sample at global position `position` of
+    iteration `iteration` of a partitioned `CSDataLoader` seeded with `seed`: fixed by the key alone, whichever rank or worker
+    loads the sample."""
+    words = np.random.SeedSequence(seed, spawn_key=(_DRAW_KEY, iteration, position)).generate_state(8)
+    return random.Random(int.from_bytes(words[:4].astype("<u4").tobytes(), "little")), np.random.RandomState(words[4:])
 
 
 _SOF = {0xC0, 0xC1, 0xC2, 0xC3, 0xC5, 0xC6, 0xC7, 0xC9, 0xCA, 0xCB, 0xCD, 0xCE, 0xCF}
@@ -157,14 +180,19 @@ class CSDataSet(data.Dataset):
         return len(self.files)
 
     def __getitem__(self, index):
-        import cv2                                                      # decode stays on the host, as in the reference (:172-173)
-        f = self.files[index]
-        image = cv2.imread(f["img"], cv2.IMREAD_COLOR)
-        label = cv2.imread(f["label"], cv2.IMREAD_GRAYSCALE)
-        if image is None or label is None:
-            raise IOError("cannot read %s / %s" % (f["img"], f["label"]))
-        aug = draw_augmentation(image.shape[0], image.shape[1], (self.crop_h, self.crop_w), self.scale, self.is_mirror, self.scales)
-        return (torch.from_numpy(image), torch.from_numpy(label), torch.tensor(aug, dtype=torch.float64), np.array(image.shape), f["name"])
+        return _training_sample(self, index)
+
+
+def _training_sample(ds, index, py_random=random, np_random=np.random):
+    """`__getitem__` of a training set (CSDataSet, CamVidDataSet, VOCDataSet) with its draws from the given streams."""
+    import cv2                                                          # decode stays on the host, as in the reference (:172-173)
+    f = ds.files[index]
+    image = cv2.imread(f["img"], cv2.IMREAD_COLOR)
+    label = cv2.imread(f["label"], cv2.IMREAD_GRAYSCALE)
+    if image is None or label is None:
+        raise IOError("cannot read %s / %s" % (f["img"], f["label"]))
+    aug = draw_augmentation(image.shape[0], image.shape[1], (ds.crop_h, ds.crop_w), ds.scale, ds.is_mirror, ds.scales, py_random, np_random)
+    return (torch.from_numpy(image), torch.from_numpy(label), torch.tensor(aug, dtype=torch.float64), np.array(image.shape), f["name"])
 
 
 def cityscapes_id_tables():
@@ -283,14 +311,7 @@ class VOCDataSet(data.Dataset):
         return len(self.files)
 
     def __getitem__(self, index):
-        import cv2
-        f = self.files[index]
-        image = cv2.imread(f["img"], cv2.IMREAD_COLOR)
-        label = cv2.imread(f["label"], cv2.IMREAD_GRAYSCALE)
-        if image is None or label is None:
-            raise IOError("cannot read %s / %s" % (f["img"], f["label"]))
-        aug = draw_augmentation(image.shape[0], image.shape[1], (self.crop_h, self.crop_w), self.scale, self.is_mirror, self.scales)
-        return (torch.from_numpy(image), torch.from_numpy(label), torch.tensor(aug, dtype=torch.float64), np.array(image.shape), f["name"])
+        return _training_sample(self, index)
 
 
 class VOCDataTestSet(data.Dataset):
@@ -449,6 +470,23 @@ class _ReplayDraws:
                 draw_augmentation(h, w, (ds.crop_h, ds.crop_w), ds.scale, ds.is_mirror, ds.scales)
 
 
+class _KeyedSamples(data.Dataset):
+    """The dataset as a partitioned loader reads it: item (index, iteration, position) -> sample `index`, its augmentation drawn from
+    `keyed_generators(seed, iteration, position)`; a test split makes no draws."""
+
+    def __init__(self, dataset, seed, test):
+        self.dataset, self.seed, self.test = dataset, seed, test
+
+    def __len__(self):
+        return len(self.dataset)
+
+    def __getitem__(self, item):
+        index, iteration, position = item
+        if self.test:
+            return self.dataset[index]
+        return _training_sample(self.dataset, index, *keyed_generators(self.seed, iteration, position))
+
+
 class CSDataLoader:
     """Drop-in for `data.DataLoader(CSDataSet(...), batch_size=..., shuffle=True, num_workers=4, pin_memory=True)` of
     train_and_eval.py:13-15: iterating it yields `(images, labels, size, name)` with images / labels already augmented and on the GPU,
@@ -459,10 +497,29 @@ class CSDataLoader:
     next iteration yields the batches that iteration had not yet yielded -- the same samples in the same order with the same
     augmentation draws.  With num_workers > 0 the workers' draws are replayed; with num_workers == 0 they come from this process's
     `random` / `np.random`, which must be restored too (`StepModel.load_training_state` does both).  Without a loaded position every
-    iteration is torch's DataLoader's, unchanged."""
+    iteration is torch's DataLoader's, unchanged.
+
+    Data parallel: with `rank` and `world_size` (e.g. `dist.get_rank()`, `dist.get_world_size()`) the loader yields this rank's share
+    of one order common to all ranks.  Iteration e (counted from 0 over the calls to `__iter__` / `host_batches`) takes the order
+    `partition_order(len(dataset), seed, e, shuffle)`; global batch g is its positions [g*W*b, (g+1)*W*b) and rank r yields
+    [g*W*b + r*b, g*W*b + (r+1)*b) of them (W = world_size, b = batch_size).  A partial last global batch is dropped on every rank
+    with `drop_last=True` (all ranks yield len(self) batches), and shared out in rank order otherwise (a rank may get a short batch
+    or none: with b = 1 and no shuffle rank r gets samples r, r + W, ...).  The augmentation of the sample at global position p is
+    drawn from `keyed_generators(seed, e, p)`: rank, worker count and resume point do not change it, and the process's `random`,
+    `np.random` and torch streams are not used.  So the W ranks' batch g, concatenated in rank order, is batch g of a
+    `world_size=1, batch_size=W*b` loader with the same seed.  `seed` means nothing without `rank` / `world_size`."""
 
     def __init__(self, dataset, batch_size=1, shuffle=False, num_workers=0, pin_memory=True, drop_last=False, label_dtype=torch.int64,
-                 device=None):
+                 device=None, rank=None, world_size=None, seed=0):
+        if (rank is None) != (world_size is None):
+            raise ValueError("rank and world_size are given together (got rank=%r, world_size=%r)" % (rank, world_size))
+        if world_size is not None:
+            ints = all(isinstance(v, int) and not isinstance(v, bool) for v in (rank, world_size, seed))
+            if not ints or world_size < 1 or not 0 <= rank < world_size or seed < 0:
+                raise ValueError("a partitioned loader needs integers 0 <= rank < world_size and seed >= 0 (got rank=%r, world_size=%r, "
+                                 "seed=%r)" % (rank, world_size, seed))
+        self.rank, self.world_size, self.seed = rank, world_size, seed
+        self._iteration, self._current = 0, None          # partitioned: the next iteration's index, the current (or last) one's
         self.dataset = dataset
         self.voc = isinstance(dataset, (VOCDataSet, VOCDataTestSet))
         self.test = isinstance(dataset, (CSDataTestSet, VOCDataTestSet))
@@ -479,11 +536,15 @@ class CSDataLoader:
         self._iter_rng, self._yielded, self._resume = None, 0, None
 
     def __len__(self):
-        return len(self.loader)
+        if self.world_size is None:
+            return len(self.loader)
+        n, b, step = len(self.dataset), self.loader.batch_size, self.world_size * self.loader.batch_size
+        full = n // step
+        return full if self.loader.drop_last else full + int(n - full * step > self.rank * b)
 
     def __iter__(self):
         if self.test:
-            for images, sizes, names in self.loader:
+            for images, sizes, names in (self.loader if self.world_size is None else self._partitioned()):
                 yield (self.augment(images), names, sizes) if self.voc else (self.augment(images), sizes, names)
             return
         for images, labels, augs, sizes, names in self.host_batches():
@@ -496,6 +557,9 @@ class CSDataLoader:
         step (what `__iter__` augments): the rest of an interrupted iteration after `load_state_dict`, else a whole new one."""
         if self.test:
             raise ValueError("only a training loader (CSDataSet / VOCDataSet) yields augmentation batches")
+        if self.world_size is not None:
+            yield from self._partitioned()
+            return
         resume, self._resume = self._resume, None
         if resume is None:
             # torch's iterator draws the workers' base seed and then the sampler's seed from the default generator: its state here
@@ -531,23 +595,57 @@ class CSDataLoader:
                                  generator=base, worker_init_fn=_ReplayDraws(self.dataset, order, bs, first, workers) if first else None)
         return iter(loader), start - first
 
+    def _rank_batches(self, iteration):
+        """-> this rank's batches of partitioned iteration `iteration`, each a list of (dataset index, iteration, global position)."""
+        n, b, step = len(self.dataset), self.loader.batch_size, self.world_size * self.loader.batch_size
+        order = partition_order(n, self.seed, iteration, self._shuffle)
+        stop = n - n % step if self.loader.drop_last else n
+        return [[(order[p], iteration, p) for p in range(start, min(start + b, stop))] for start in range(self.rank * b, stop, step)]
+
+    def _partitioned(self):
+        """One partitioned iteration's raw batches: the rest of an interrupted one after `load_state_dict`, else the next one."""
+        resume, self._resume = self._resume, None
+        iteration, start = (self._iteration, 0) if resume is None else resume
+        self._iteration, self._current, self._yielded = iteration + 1, iteration, start
+        batches = self._rank_batches(iteration)[start:]
+        if not batches:
+            return
+        # a private generator for the workers' base seed, so that the default one is left alone
+        loader = data.DataLoader(_KeyedSamples(self.dataset, self.seed, self.test), batch_sampler=batches,
+                                 num_workers=self.loader.num_workers, pin_memory=self.loader.pin_memory, collate_fn=self.loader.collate_fn,
+                                 generator=torch.Generator())
+        for batch in loader:
+            self._yielded += 1
+            yield batch
+
     def state_dict(self):
         """The position of the current (or last) iteration: the default generator's state when it began, and the number of batches
-        it has yielded."""
+        it has yielded.  A partitioned loader (version 2) holds its iteration index instead of a generator state, with its `rank`,
+        `world_size`, `seed` and `drop_last`."""
         if self.test:
             raise ValueError("only a training loader (CSDataSet / VOCDataSet) can be resumed")
-        return dict(version=1, rng_state=self._iter_rng, batches=self._yielded, num_samples=len(self.dataset),
-                    batch_size=self.loader.batch_size, shuffle=self._shuffle, num_workers=self.loader.num_workers)
+        sd = dict(version=1, rng_state=self._iter_rng, batches=self._yielded, num_samples=len(self.dataset),
+                  batch_size=self.loader.batch_size, shuffle=self._shuffle, num_workers=self.loader.num_workers)
+        if self.world_size is not None:
+            sd.update(version=2, rng_state=None, rank=self.rank, world_size=self.world_size, seed=self.seed, iteration=self._current,
+                      drop_last=self.loader.drop_last)
+        return sd
 
     def load_state_dict(self, sd):
         """The next iteration continues the one `sd` describes (state_dict of a loader over the same list, batch size, shuffle and
-        worker count); a mismatch raises ValueError naming the field, and changes nothing."""
+        worker count, and for a partitioned loader the same rank, world size, seed and drop_last); a mismatch raises ValueError naming
+        the field, and changes nothing."""
         if self.test:
             raise ValueError("only a training loader (CSDataSet / VOCDataSet) can be resumed")
-        want = dict(version=1, num_samples=len(self.dataset), batch_size=self.loader.batch_size, shuffle=self._shuffle,
-                    num_workers=self.loader.num_workers)
+        want = dict(rank=self.rank, world_size=self.world_size)
+        if self.world_size is not None:
+            want.update(seed=self.seed, drop_last=self.loader.drop_last)
+        want.update(version=1 if self.world_size is None else 2, num_samples=len(self.dataset), batch_size=self.loader.batch_size,
+                    shuffle=self._shuffle, num_workers=self.loader.num_workers)
         for k, v in want.items():
             if sd.get(k) != v:
                 raise ValueError("loader state does not match the loader: %s is %r, the loader's %r" % (k, sd.get(k), v))
-        if sd["rng_state"] is not None:                                      # None: no iteration had begun, nothing to skip
+        if self.world_size is not None:                                      # iteration None: none had begun, start at the first
+            self._resume = (0, 0) if sd["iteration"] is None else (int(sd["iteration"]), int(sd["batches"]))
+        elif sd["rng_state"] is not None:                                    # None: no iteration had begun, nothing to skip
             self._resume = (sd["rng_state"].clone(), int(sd["batches"]))

@@ -13,6 +13,7 @@ from math import ceil
 
 import numpy as np
 import torch
+import torch.distributed as dist
 
 from .. import ops
 from .._cabi import lib
@@ -166,15 +167,39 @@ class _PngWriter:
         self._raise()
 
 
+def _sum_over_ranks(counts):
+    """All-reduce (sum) of an integer count tensor over the default process group: in place on the device under NCCL, through a
+    host copy under a CPU backend (gloo)."""
+    if "nccl" in str(dist.get_backend()) and counts.is_cuda:
+        dist.all_reduce(counts)
+        return counts
+    host = counts.cpu()
+    dist.all_reduce(host)
+    return host
+
+
 def evaluate_main(model, loader, gpu_id, input_size, num_classes, whole=False, recurrence=1, type='val', save_dir=None, scales=(1.0,),
-                  flip=False, png_dir=None):
+                  flip=False, png_dir=None, distributed=False):
     """-> (mean_IU, IU_array) over `loader` batches (image (1,3,H,W), label (1,H,W), size, name); type='test' batches are
     (image, size, name), count nothing, and their output is the PNGs.
 
     scales / flip: predict_multiscale's (whole=True only; the reference's sliding path has neither).  The defaults run the single
     whole-image pass.  png_dir: write <png_dir>/<name>.png, the arg-max of the whole image as an 8-bit palette image
-    (get_palette(256)), in Cityscapes label ids for type='test' (19 classes); with save_dir too, the .pt maps are the same values."""
+    (get_palette(256)), in Cityscapes label ids for type='test' (19 classes); with save_dir too, the .pt maps are the same values.
+
+    Sharded evaluation: when `loader` is a partitioned `CSDataLoader` with world_size > 1, or with `distributed=True` (a caller's own
+    sharded loader), every rank of the default process group calls this on its share of the images and the confusion counts are
+    summed over the ranks (one all-reduce of num_classes^2 int64 counts: on the device under NCCL, through the host otherwise), so
+    every rank returns the (mean_IU, IU_array) of the whole set, bit for bit the one-process result.  png_dir / save_dir files are
+    written by the rank that scored the image."""
     scales = _check_scales(scales)
+    from ..dataset.datasets import CSDataLoader
+    sharded = bool(distributed) or (isinstance(loader, CSDataLoader) and (loader.world_size or 1) > 1)
+    if sharded:
+        if not (dist.is_available() and dist.is_initialized()):
+            raise ValueError("sharded evaluation needs an initialised torch.distributed process group")
+        if isinstance(loader, CSDataLoader) and loader.world_size is not None and loader.world_size != dist.get_world_size():
+            raise ValueError("the loader is partitioned over %d ranks, the process group has %d" % (loader.world_size, dist.get_world_size()))
     multi = scales != (1.0,) or bool(flip)
     if multi and not whole:
         raise ValueError("scales other than (1.0,) and flip need whole=True: the sliding-window path is single-scale")
@@ -237,6 +262,8 @@ def evaluate_main(model, loader, gpu_id, input_size, num_classes, whole=False, r
             writer.close()
         if was_training:
             model.train()
+    if sharded:
+        conf = _sum_over_ranks(conf)
     cm = conf.cpu().numpy().astype(np.float64)
     pos, res, tp = cm.sum(1), cm.sum(0), np.diag(cm)
     IU_array = tp / np.maximum(1.0, pos + res - tp)

@@ -305,9 +305,11 @@ class StepModel():
         g["graph"].replay()
         self._update()
 
-    def evalute_model(self, model, loader, gpu_id, input_size, num_classes, whole):
-        """evaluate_main on `model`: the eval-mode path, BN folded from the current running statistics."""
-        mean_IU, IU_array = evaluate_main(model=model, loader=loader, gpu_id=gpu_id, input_size=input_size, num_classes=num_classes, whole=whole)
+    def evalute_model(self, model, loader, gpu_id, input_size, num_classes, whole, distributed=False):
+        """evaluate_main on `model`: the eval-mode path, BN folded from the current running statistics.  Sharded over the ranks when
+        `loader` is a partitioned CSDataLoader or `distributed` is true (evaluate_main's rule); every rank gets the whole set's IU."""
+        mean_IU, IU_array = evaluate_main(model=model, loader=loader, gpu_id=gpu_id, input_size=input_size, num_classes=num_classes, whole=whole,
+                                          distributed=distributed)
         return mean_IU, IU_array
 
     def save_ckpt(self, epoch, step, mean_IU, IU_array):
