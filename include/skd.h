@@ -504,6 +504,24 @@ int skd_bnact_bwd_reduce(long long P, int C, int relu6, const float* x, int ldx,
 int skd_bnact_bwd_dx(long long P, int C, int relu6, const float* x, int ldx, const float* dout, int ldd, const float* mean, const float* var,
                      const float* weight, const float* bias, float eps, int training, const float* coef, float* dx, int lddx, cudaStream_t);
 
+/* ---- J. feature-level distillation baselines (csrc/feature_kd.cu).  Maps are fp32 NHWC rows [P = N*H*W][C] at a row pitch in floats
+        (ld >= C; channel slices of a concat buffer in place), read in float4 groups when C, the pitch and the base are 16-byte aligned.
+        Fixed-order reductions, no atomics: two calls give bit-identical results. ---- */
+/* attention transfer, at(x) = F.normalize(x.pow(2).mean(1).view(N, -1)): q = mean_c a_c^2 per pixel of the student map S (CS channels)
+   and the teacher map T (CT channels, same N and HW); qhat [2][N*HW] = q / max(||q||_2, 1e-12) per sample (student, then teacher),
+   norms [2][N] = ||q||_2; loss = mean over N*HW of (qhat_S - qhat_T)^2 */
+int skd_at_fwd(int N, int HW, int CS, const float* S, int lds, int CT, const float* T, int ldt, float* qhat, float* norms, float* loss,
+               cudaStream_t);
+/* its gradient dS = (2 / C) a_c g with g = (h - qhat_S <qhat_S, h>) / ||q_S|| (h / 1e-12 where the norm is below the clamp),
+   h = 2 (qhat_S - qhat_T) / (N*HW) * grad_out[0]; g: N*HW floats of workspace; dS at pitch ldd */
+int skd_at_bwd(int N, int HW, int C, const float* S, int lds, const float* qhat, const float* norms, const float* grad_out, float* g,
+               float* dS, int ldd, cudaStream_t);
+/* MIMIC's F.mse_loss(R, T): loss = mean of (R - T)^2 over P*C; workspace: skd_loss_max_partials() doubles */
+int skd_mse_fwd(long long P, int C, const float* R, int ldr, const float* T, int ldt, float* loss, double* workspace, cudaStream_t);
+/* its gradient dR = 2 (R - T) / (P*C) * grad_out[0], at pitch ldd */
+int skd_mse_bwd(long long P, int C, const float* R, int ldr, const float* T, int ldt, const float* grad_out, float* dR, int ldd,
+                cudaStream_t);
+
 #ifdef __cplusplus
 }
 #endif

@@ -53,6 +53,38 @@ class PairWiseLoss(torch.autograd.Function):
         return ops.pairwise_bwd(E, pS, rS, arg, g.contiguous(), feat_S), None, None, None
 
 
+class AttentionTransferLoss(torch.autograd.Function):
+    """Attention transfer (Zagoruyko & Komodakis): mean over N*H*W of (at(S) - at(T))^2 with at(x) = F.normalize(x.pow(2).mean(1)
+    .view(N, -1)).  The forward keeps the normalised maps and the student's norms for the backward; the teacher gets no gradient."""
+
+    @staticmethod
+    def forward(ctx, feat_S, feat_T):
+        loss, qhat, norms = ops.at_fwd(feat_S, feat_T)
+        ctx.save_for_backward(feat_S, qhat, norms)
+        return loss
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        feat_S, qhat, norms = ctx.saved_tensors
+        return ops.at_bwd(feat_S, qhat, norms, g.contiguous()), None
+
+
+class MseLoss(torch.autograd.Function):
+    """F.mse_loss(r, t) with t frozen: MIMIC's regression of the teacher's feature map from the adapter output r."""
+
+    @staticmethod
+    def forward(ctx, r, t):
+        ctx.save_for_backward(r, t)
+        return ops.mse_fwd(r, t)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        r, t = ctx.saved_tensors
+        return ops.mse_bwd(r, t, g.contiguous()), None
+
+
 class DsnCrossEntropy(torch.autograd.Function):
     """CriterionDSN math (utils/criterion.py:179-188): fused upsample + log-softmax + NLL for both heads.  `weight` (C fp32 class
     weights on the device, or None) makes each head's term CrossEntropyLoss(weight=weight)'s weighted mean."""

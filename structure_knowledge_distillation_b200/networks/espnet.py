@@ -131,6 +131,11 @@ class ESPNet_Encoder(nn.Module):
     def dropouts(self):
         return []
 
+    def level_channels(self):
+        """Widths of preds[-1] .. preds[-5]: b1, level2's output, b2, level3's output and b3 (`feat`)."""
+        return (self.b1.bn.num_features, self.level2[-1].bn.bn.num_features, self.b2.bn.num_features,
+                self.level3[-1].bn.bn.num_features, self.b3.bn.num_features)
+
     def _br(self, br, pieces, image=None, ipa=0):
         bn = br.bn
         return Fn.EspBnPrelu.apply(image, ipa, bn.weight, bn.bias, br.act.weight, bn.running_mean, bn.running_var,
@@ -193,6 +198,10 @@ class ESPNet(nn.Module):
 
     def dropouts(self):
         return []
+
+    def level_channels(self):
+        """Widths of preds[-1] .. preds[-5], the encoder's."""
+        return self.encoder.level_channels()
 
     def _bn(self, bn, alpha, pieces):
         return Fn.EspBnPrelu.apply(None, 0, bn.weight, bn.bias, alpha, bn.running_mean, bn.running_var, bn.num_batches_tracked,

@@ -3,7 +3,8 @@
 Kept surface: NetModel(args), .set_input(data), .forward(), .student_backward(), .discriminator_backward(),
 .optimize_parameters(), .adjust_learning_rate(base_lr, optimizer, i_iter), .lr_poly, .print_info, .save_ckpt,
 .evalute_model; attributes .student .teacher .G_solver .D_solver .preds_S .preds_T .G_loss .mc_G_loss .pi_G_loss
-.pa_G_loss .D_loss (train_and_eval.py:19-30 reads them).
+.pa_G_loss .D_loss (train_and_eval.py:19-30 reads them).  Ours: .at_G_loss / .mimic_G_loss (attention transfer and MIMIC, the
+paper's feature-level baselines; None while off) and .mimic_adapters.
 
 The step machinery it shares with SegModel is StepModel's (networks/step_model.py); NetModel adds the frozen teacher, the
 discriminator and the distillation terms.
@@ -20,16 +21,26 @@ What changed underneath (DESIGN.md):
 import logging
 
 import torch
+import torch.nn as nn
 
 from .. import functions as Fn
 from .. import ops
-from ..utils.criterion import (CriterionAdditionalGP, CriterionAdv, CriterionAdvForG, CriterionPairWiseforWholeFeatAfterPool,
-                               CriterionPixelWise, check_pa_levels, pair_wise_level_criteria)
+from ..utils.criterion import (CriterionAdditionalGP, CriterionAdv, CriterionAdvForG, CriterionAT, CriterionMimic,
+                               CriterionPairWiseforWholeFeatAfterPool, CriterionPixelWise, check_feature_levels, check_pa_levels,
+                               feature_level_criteria, pair_wise_level_criteria)
 from ..utils.utils import load_D_model, load_S_model, load_T_model
+from .pspnet_combine import Conv2d
 from .sagan_models import Discriminator
 from .step_model import StepModel, _LazyScalar, _arg, build_seg_network
 
 STUDENTS = ("resnet18", "espnet_c", "espnet", "mobilenetv2")
+
+def mimic_adapters(student, teacher, levels):
+    """MIMIC's 1x1 adapters (with bias, nn.Conv2d's init), one per level of check_feature_levels() with a non-zero weight, from the
+    student's width at that level to the teacher's, as the two networks' level_channels() give them: key `level<ind>` for
+    preds[-(ind + 1)]."""
+    cs, ct = student.level_channels(), teacher.level_channels()
+    return nn.ModuleDict({"level%d" % (-i - 1): Conv2d(cs[-i - 1], ct[-i - 1], 1, bias=True) for i, w in levels if w != 0.0})
 
 
 class NetModel(StepModel):
@@ -41,6 +52,10 @@ class NetModel(StepModel):
         # None: scalar lambda_pa / pool_scale, one pair-wise term on preds[-5]; else [(lambda, scale)] per level, level `ind` on
         # preds[-(ind + 1)] (x1, x2, x3, x4, PSP features)
         self.pa_levels = check_pa_levels(args)
+        # [(feat_ind, weight)]: a scalar weight is one term on preds[-5], a list one per level as for Pa
+        self.at_levels = check_feature_levels(args, "lambda_at", "attention-transfer", 500.0)
+        self.mimic_levels = check_feature_levels(args, "lambda_mimic", "MIMIC", 1.0)
+        self.at, self.mimic = _arg(args, "at", False) == True, _arg(args, "mimic", False) == True
         self._check_device()
         self._check_kind("student", "resnet18", STUDENTS)
         device = self.device
@@ -64,7 +79,10 @@ class NetModel(StepModel):
         self.D_model = D_model.float().to(device).train()
         self.parallel_D = self.D_model
 
-        self._init_training(self.student, self.D_model)
+        self.mimic_adapters = None
+        if self.mimic:                                            # trained with the student: same flat buffer, decay, exchange, graph
+            self.mimic_adapters = mimic_adapters(self.student, self.teacher, self.mimic_levels).float().to(device).train()
+        self._init_training(self.student, self.D_model, extra=self.mimic_adapters)
         self.criterion_pixel_wise = CriterionPixelWise()
         if self.pa_levels is None:
             self.criterion_pair_wise_for_interfeat = CriterionPairWiseforWholeFeatAfterPool(scale=args.pool_scale, feat_ind=-5)
@@ -74,11 +92,16 @@ class NetModel(StepModel):
         if args.adv_loss_type == 'wgan-gp':
             self.criterion_AdditionalGP = CriterionAdditionalGP(self.parallel_D, args.lambda_gp)
         self.criterion_adv_for_G = CriterionAdvForG(args.adv_loss_type)
+        self.criterion_at = feature_level_criteria(self.at_levels, CriterionAT) if self.at else []
+        self.criterion_mimic = feature_level_criteria(
+            self.mimic_levels, lambda i: CriterionMimic(i, self.mimic_adapters["level%d" % (-i - 1)])) if self.mimic else []
 
         self._teacher_stream = None
         self._d_stream = None
         self.pi_G_loss = 0.0
         self.pa_G_loss = 0.0 if self.pa_levels is None else [0.0] * len(self.pa_levels)
+        self.at_G_loss = self._zero_terms(self.at_levels, "lambda_at") if self.at else None
+        self.mimic_G_loss = self._zero_terms(self.mimic_levels, "lambda_mimic") if self.mimic else None
         self.D_loss = 0.0
 
     def forward(self):
@@ -106,7 +129,8 @@ class NetModel(StepModel):
     def _resample_teacher(self):
         """Students on another grid than the teacher (ESPNet-C: 45x60 at 360x480, PSPNet's ceil-mode pool: 46x61; the full ESPNet's
         logits: 360x480): the teacher tensors the distillation terms read -- preds_T[0] and preds_T[-5], or with pair-wise levels
-        preds_T[0] and the preds_T[-(ind + 1)] of every level with a non-zero weight -- are each resized onto the grid of their own
+        preds_T[0] and the preds_T[-(ind + 1)] of every level with a non-zero weight, plus those of the weighted attention-transfer
+        and MIMIC levels -- are each resized onto the grid of their own
         student counterpart (bilinear, align_corners=True; forward only, the teacher is frozen).  Equal grids (the ResNet18
         student): nothing runs.  The teacher's own logits stay in `logits_T` for the discriminator of a full-resolution student."""
         self.logits_T = self.preds_T[0]
@@ -116,6 +140,9 @@ class NetModel(StepModel):
         else:
             read = [0] + ([len(preds) - 1 - ind for ind, (lam, _) in enumerate(self.pa_levels) if lam != 0.0]
                           if self.args.pa == True else [])
+        read = list(read)
+        for terms_on, levels in ((self.at, self.at_levels), (self.mimic, self.mimic_levels)):
+            read += [len(preds) + i for i, w in levels if terms_on and w != 0.0 and len(preds) + i not in read]
         for i in read:
             size = tuple(self.preds_S[i].shape[2:])
             if tuple(preds[i].shape[2:]) != size:
@@ -147,6 +174,10 @@ class NetModel(StepModel):
             temp1 = self.criterion_pair_wise_for_interfeat(self.preds_S, self.preds_T)
             self.pa_G_loss = _LazyScalar(temp1)
             G_loss = G_loss + args.lambda_pa * temp1
+        if self.at:
+            G_loss, self.at_G_loss = self._feature_terms(G_loss, self.at_levels, self.criterion_at, "lambda_at")
+        if self.mimic:
+            G_loss, self.mimic_G_loss = self._feature_terms(G_loss, self.mimic_levels, self.criterion_mimic, "lambda_mimic")
         if args.ho == True:
             d_out_S = self.parallel_D(self._d_inputs()[0])
             G_loss = G_loss + args.lambda_d * self.criterion_adv_for_G(d_out_S, d_out_S)
@@ -176,6 +207,27 @@ class NetModel(StepModel):
             G_loss = G_loss + lam * temp
         self.pa_G_loss = pa
         return G_loss
+
+    def _zero_terms(self, levels, name):
+        """What at_G_loss / mimic_G_loss log before the first step: 0.0, or one 0.0 per level when args.<name> is a list."""
+        return [0.0] * len(levels) if isinstance(_arg(self.args, name, None), (list, tuple)) else 0.0
+
+    def _feature_terms(self, G_loss, levels, crits, name):
+        """G_loss + sum over levels of weight * term -> (that sum, the unweighted terms as lazy device scalars: a list when args.<name>
+        is one, else the single term).  A level with weight 0 launches nothing and logs 0.0."""
+        terms = []
+        for (_, w), crit in zip(levels, crits):
+            if crit is None:
+                terms.append(0.0)
+                continue
+            temp = crit(self.preds_S, self.preds_T)
+            terms.append(_LazyScalar(temp))
+            G_loss = G_loss + w * temp
+        return G_loss, (terms if isinstance(_arg(self.args, name, None), (list, tuple)) else terms[0])
+
+    def _extra_states(self):
+        adapters = getattr(self, "mimic_adapters", None)
+        return {} if adapters is None else {"mimic_state_dict": adapters}
 
     def discriminator_backward(self):
         self._discriminator_phase()
@@ -244,10 +296,13 @@ class NetModel(StepModel):
             self.D_solver.step()
 
     def print_info(self, epoch, step):
-        if isinstance(self.pa_G_loss, list):                        # one unweighted term per pair-wise level
-            pa = '[' + ', '.join('{:.5f}'.format(float(v)) for v in self.pa_G_loss) + ']'
-        else:
-            pa = '{:.5f}'.format(float(self.pa_G_loss))
+        def terms(v):                                               # a list: one unweighted term per level
+            return '[' + ', '.join('{:.5f}'.format(float(t)) for t in v) + ']' if isinstance(v, list) else '{:.5f}'.format(float(v))
+        pa = terms(self.pa_G_loss)
+        for name in ('at', 'mimic'):                                # appended only while the term is on
+            v = getattr(self, name + '_G_loss', None)
+            if v is not None:
+                pa += ' {}:{}'.format(name, terms(v))
         logging.info('step:{:5d} G_lr:{:.6f} G_loss:{:.5f}(mc:{:.5f} pixelwise:{:.5f} pairwise:{}) D_lr:{:.6f} D_loss:{:.5f}'.format(
             step, self.G_solver.param_groups[-1]['lr'], float(self.G_loss), float(self.mc_G_loss), float(self.pi_G_loss),
             pa, self.D_solver.param_groups[-1]['lr'], float(self.D_loss)))

@@ -121,6 +121,10 @@ class MobileNetV2Dilated(nn.Module):
     def dropouts(self):
         return [self.pspmodule.bottleneck[2], self.dsn[2]]
 
+    def level_channels(self):
+        """Widths of preds[-1] .. preds[-5]: features[3], [6], [13], [17] (their projection's output) and the PSP features."""
+        return tuple(self.features[i].conv[-2].out_channels for i in (3, 6, 13, 17)) + (self.pspmodule.bottleneck[0].out_channels,)
+
     def forward(self, x):
         # the (N,3,H,W) image, or the 4-channel NHWC image NetModel.forward builds for the teacher
         x = ops.pad_channels(x, 4) if x.shape[1] == 3 else ops.to_nhwc(x)

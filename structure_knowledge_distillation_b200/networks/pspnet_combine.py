@@ -238,6 +238,12 @@ class ResNet(nn.Module):
     def dropouts(self):
         return [self.pspmodule.bottleneck[2], self.dsn[2]]
 
+    def level_channels(self):
+        """Widths of preds[-1] .. preds[-5]: x1, x2, x3, x4 and the PSP features."""
+        last = [layer[-1] for layer in (self.layer1, self.layer2, self.layer3, self.layer4)]
+        return tuple((b.conv3 if isinstance(b, Bottleneck) else b.conv2).out_channels for b in last) + \
+            (self.pspmodule.bottleneck[0].out_channels,)
+
     def forward(self, x):
         # the 3-channel image travels as 4 channels (16-byte pixel rows for TMA); a caller that feeds two networks
         # (NetModel.forward) pads once and passes the 4-channel tensor to both

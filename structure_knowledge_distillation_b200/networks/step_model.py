@@ -132,9 +132,10 @@ class StepModel():
         if _arg(self.args, "sync_bn", False) and (self.espnet or kind == "mobilenetv2"):
             raise ValueError("sync_bn is only available with the ResNet networks (the BatchNorm statistics of %r are per rank)" % kind)
 
-    def _init_training(self, net, D_model=None):
+    def _init_training(self, net, D_model=None, extra=None):
         """Training state for `net` (on the device): sync_bn, FlatSGD G_solver (and D_solver for NetModel's discriminator `D_model`),
-        the gradient exchange across ranks, the task criterion, the CUDA-graph option and the snapshot directory."""
+        the gradient exchange across ranks, the task criterion, the CUDA-graph option and the snapshot directory.  `extra`: a module
+        trained with `net` (NetModel's MIMIC adapters), its parameters after net's in G_solver's flat buffer."""
         args = self.args
         if _arg(args, "sync_bn", False):                          # cross-rank batch statistics (the reference's InPlaceABNSync semantics)
             from ..libs import InPlaceABNSync
@@ -149,7 +150,8 @@ class StepModel():
         if self.allreduce not in ("nccl", "nvls", "none"):
             raise ValueError("allreduce must be 'nccl' or 'nvls'")
         sym = self.allreduce == "nvls"
-        self.G_solver = FlatSGD([p for p in net.parameters() if p.requires_grad], args.lr_g, momentum=args.momentum,
+        trained = list(net.parameters()) + (list(extra.parameters()) if extra is not None else [])
+        self.G_solver = FlatSGD([p for p in trained if p.requires_grad], args.lr_g, momentum=args.momentum,
                                 weight_decay=args.weight_decay, direct_grads=True, symmetric=sym)
         solvers, modules = [self.G_solver], [net]
         if D_model is not None:
@@ -329,12 +331,17 @@ class StepModel():
             parts.append(("D_", self.D_model, self.D_solver))
         return parts
 
+    def _extra_states(self):
+        """{field: module} saved and restored beside the trained network (NetModel: `mimic_state_dict`, the MIMIC adapters)."""
+        return {}
+
     def save_training_state(self, path, step, epoch=0, best_mean_IU=None, IU_array=None, loader=None):
         """Writes everything needed to continue this run after step `step` (best_mean_IU defaults to self.best_mean_IU) to `path`,
         one torch.save dict:
           * `state_dict`, `step`, `epoch`, `best_mean_IU`, `IU_array` -- the reference's checkpoint keys: renamed to model_best.pth.tar
             in S_ckpt_path / ckpt_path, the file loads through load_S_model / load_seg_model (S_resume / resume) like the reference's;
           * `D_state_dict` (spectral-norm u / v, BN buffers included), `G_solver` / `D_solver` (momentum, steps, lr, flat length);
+          * with MIMIC, `mimic_state_dict`: the adapters (their momentum is in G_solver);
           * `ranks`: per rank, the torch CPU and CUDA generators, Python `random`, numpy's global generator and `loader.state_dict()`;
           * `format`, `version`, `world_size`, `kind`, `classes_num`: what load_training_state checks.
         Collective: every rank calls it.  Rank 0 writes a temporary file beside `path` and renames it over `path`, so an interrupted
@@ -355,6 +362,8 @@ class StepModel():
                          IU_array=None if IU_array is None else np.asarray(IU_array, dtype=np.float64), ranks=ranks)
             for prefix, module, _ in self._trained():
                 state[prefix + "state_dict"] = _cpu_state(module)
+            for field, module in self._extra_states().items():
+                state[field] = _cpu_state(module)
             state["G_solver"] = solvers["solver"]
             state["D_solver"] = solvers.get("D_solver")
             for k in ("G_solver", "D_solver"):
@@ -419,6 +428,12 @@ class StepModel():
             _check_state_dict(prefix + "state_dict", module.state_dict(), ck.get(prefix + "state_dict"))
         if len(parts) == 1 and ck.get("D_solver") is not None:
             mismatch("D_solver", "a discriminator", None)
+        extra = self._extra_states()
+        for field, module in extra.items():
+            _check_state_dict(field, module.state_dict(), ck.get(field))
+        for field in ck:
+            if field.endswith("_state_dict") and field not in ("state_dict", "D_state_dict") and field not in extra:
+                mismatch(field, "present", None)
         mine = ck["ranks"][rank]
         if loader is not None:
             if mine.get("loader") is None:
@@ -429,6 +444,8 @@ class StepModel():
             for prefix, module, solver in parts:
                 module.load_state_dict(ck[prefix + "state_dict"])      # copy_ into the existing tensors (flat-buffer views)
                 solver.load_state_dict(ck["G_solver" if prefix == "" else "D_solver"])
+            for field, module in extra.items():
+                module.load_state_dict(ck[field])
         _set_rng_states(mine, self.device)
         self.args.last_step, self.args.start_epoch = ck["step"], ck["epoch"]
         self.args.best_mean_IU = self.best_mean_IU = ck["best_mean_IU"]

@@ -480,6 +480,49 @@ def pixelwise_bwd(S, T, grad_out):
     return dS
 
 
+def at_fwd(S, T):
+    """Attention transfer (csrc/feature_kd.cu) of NHWC-stored (pitch allowed) student / teacher maps on one grid -> (loss, qhat
+    (2, N*H*W): the normalised maps of S and T, norms (2, N): the per-sample norms of the unnormalised maps)."""
+    _f32(S, T)
+    n, cs, h, w, lds = nhwc_meta(S)
+    nt, ct, ht, wt, ldt = nhwc_meta(T)
+    if (nt, ht, wt) != (n, h, w):
+        raise ValueError("attention transfer: student %s and teacher %s maps differ in batch or grid" % (tuple(S.shape), tuple(T.shape)))
+    qhat = torch.empty((2, n * h * w), device=S.device, dtype=torch.float32)
+    norms = torch.empty((2, n), device=S.device, dtype=torch.float32)
+    loss = torch.empty((), device=S.device, dtype=torch.float32)
+    lib().skd_at_fwd(n, h * w, cs, _p(S), lds, ct, _p(T), ldt, _p(qhat), _p(norms), _p(loss), _st())
+    return loss, qhat, norms
+
+
+def at_bwd(S, qhat, norms, grad_out):
+    """d loss / d S of at_fwd, in S's layout."""
+    n, c, h, w, lds = nhwc_meta(S)
+    dS = torch.empty_strided(S.shape, S.stride(), device=S.device, dtype=torch.float32)
+    g = torch.empty(n * h * w, device=S.device, dtype=torch.float32)
+    lib().skd_at_bwd(n, h * w, c, _p(S), lds, _p(qhat), _p(norms), _p(grad_out), _p(g), _p(dS), lds, _st())
+    return dS
+
+
+def mse_fwd(R, T):
+    """F.mse_loss(R, T) of NHWC-stored (pitch allowed) maps of one shape (csrc/feature_kd.cu)."""
+    _f32(R, T)
+    if tuple(R.shape) != tuple(T.shape):
+        raise ValueError("mse: shapes %s and %s differ" % (tuple(R.shape), tuple(T.shape)))
+    n, c, h, w, ldr = nhwc_meta(R)
+    loss = torch.empty((), device=R.device, dtype=torch.float32)
+    lib().skd_mse_fwd(n * h * w, c, _p(R), ldr, _p(T), nhwc_meta(T)[4], _p(loss), _p(_ws(R.device)), _st())
+    return loss
+
+
+def mse_bwd(R, T, grad_out):
+    """d mse_fwd(R, T) / d R, dense NHWC."""
+    n, c, h, w, ldr = nhwc_meta(R)
+    dR = empty_nhwc(n, c, h, w, R.device)
+    lib().skd_mse_bwd(n * h * w, c, _p(R), ldr, _p(T), nhwc_meta(T)[4], _p(grad_out), _p(dR), c, _st())
+    return dR
+
+
 def _class_weight(weight, l0):
     """The class-weight table as the weighted kernels read it: contiguous fp32, one entry per class, on the logits' device."""
     if weight.dtype != torch.float32 or not weight.is_contiguous() or weight.dim() != 1 or weight.device != l0.device:

@@ -10,6 +10,8 @@
   CriterionOhemDSN                            utils/criterion.py:190-209
   CriterionAdv / CriterionAdvForG             utils/criterion.py:122-166
   CriterionAdditionalGP                       utils/criterion.py:92-120
+  CriterionAT / CriterionMimic                the feature-level baselines the paper compares with (no reference source: attention
+                                              transfer after Zagoruyko & Komodakis, MIMIC after Li et al.)
 
 The OHEM criteria follow the reference's threshold rule (scipy's zoom to a 1/factor grid with its exact arithmetic, the order
 statistic, pixels with p[label] <= threshold kept) but compute it on the device, without the reference's host round trip.
@@ -72,19 +74,52 @@ def check_pa_levels(args):
         raise ValueError("lambda_pa and pool_scale must both be scalars or both be lists (got %r and %r)" % (lam, scale))
     if len(lam) != len(scale):
         raise ValueError("lambda_pa and pool_scale lists differ in length (%d and %d)" % (len(lam), len(scale)))
-    if not 1 <= len(lam) <= PA_LEVELS_MAX:
-        raise ValueError("lambda_pa / pool_scale lists must have 1..%d entries (got %d)" % (PA_LEVELS_MAX, len(lam)))
+    _check_level_count("lambda_pa / pool_scale lists", len(lam))
     levels = []
     for ind, (l, s) in enumerate(zip(lam, scale)):
         try:
             l, s = float(l), float(s)
         except (TypeError, ValueError):
             raise ValueError("pair-wise level %d: lambda_pa and pool_scale must be numbers (got %r, %r)" % (ind, l, s)) from None
-        if not math.isfinite(l) or l < 0:
-            raise ValueError("pair-wise level %d: lambda_pa must be finite and >= 0 (got %r)" % (ind, l))
+        _check_level_weight("pair-wise level %d: lambda_pa" % ind, l)
         if not (math.isfinite(s) and 0 < s <= 1):
             raise ValueError("pair-wise level %d: pool_scale must be in (0, 1] (got %r)" % (ind, s))
         levels.append((l, s))
+    return levels
+
+
+def _check_level_count(what, n):
+    if not 1 <= n <= PA_LEVELS_MAX:
+        raise ValueError("%s must have 1..%d entries (got %d)" % (what, PA_LEVELS_MAX, n))
+
+
+def _check_level_weight(what, w):
+    if not math.isfinite(w) or w < 0:
+        raise ValueError("%s must be finite and >= 0 (got %r)" % (what, w))
+
+
+def check_feature_levels(args, name, term, default):
+    """`args.<name>` (lambda_at / lambda_mimic) of NetModel, validated before any device work -> [(feat_ind, weight)]: a scalar is
+    one term on preds[-5] (the PSP features); a list (or tuple) of L weights, 1 <= L <= 5, puts level `ind` on preds[-(ind + 1)] as
+    the pair-wise levels do (check_pa_levels).  Each weight finite and >= 0 (0 skips the level); anything else raises ValueError
+    naming `term`."""
+    lam = getattr(args, name, default)
+    if not isinstance(lam, (list, tuple)):
+        try:
+            lam = float(lam)
+        except (TypeError, ValueError):
+            raise ValueError("%s must be a number or a list of numbers (got %r)" % (name, lam)) from None
+        _check_level_weight(name, lam)
+        return [(-5, lam)]
+    _check_level_count(name + " list", len(lam))
+    levels = []
+    for ind, l in enumerate(lam):
+        try:
+            l = float(l)
+        except (TypeError, ValueError):
+            raise ValueError("%s level %d: %s must be a number (got %r)" % (term, ind, name, l)) from None
+        _check_level_weight("%s level %d: %s" % (term, ind, name), l)
+        levels.append((-(ind + 1), l))
     return levels
 
 
@@ -92,6 +127,36 @@ def pair_wise_level_criteria(levels):
     """One CriterionPairWiseforWholeFeatAfterPool per level of check_pa_levels(), level `ind` on preds[-(ind + 1)]
     (kd_model.py:81)."""
     return [CriterionPairWiseforWholeFeatAfterPool(scale=s, feat_ind=-(ind + 1)) for ind, (_, s) in enumerate(levels)]
+
+
+class CriterionAT(nn.Module):
+    """Attention transfer (Zagoruyko & Komodakis) between preds_S[feat_ind] and preds_T[feat_ind]: mean over N*H*W of
+    (at(S) - at(T))^2 with at(x) = F.normalize(x.pow(2).mean(1).view(N, -1)) (p = 2).  Channel-agnostic: the two widths may differ."""
+
+    def __init__(self, feat_ind):
+        super().__init__()
+        self.feat_ind = feat_ind
+
+    def forward(self, preds_S, preds_T):
+        return Fn.AttentionTransferLoss.apply(preds_S[self.feat_ind], preds_T[self.feat_ind].detach())
+
+
+class CriterionMimic(nn.Module):
+    """MIMIC (Li et al.): F.mse_loss(adapter(preds_S[feat_ind]), preds_T[feat_ind]), `adapter` a 1x1 convolution with bias from the
+    student's to the teacher's width (networks/pspnet_combine.Conv2d, on the wgmma kernels)."""
+
+    def __init__(self, feat_ind, adapter):
+        super().__init__()
+        self.feat_ind = feat_ind
+        self.adapter = adapter
+
+    def forward(self, preds_S, preds_T):
+        return Fn.MseLoss.apply(self.adapter(preds_S[self.feat_ind]), preds_T[self.feat_ind].detach())
+
+
+def feature_level_criteria(levels, make):
+    """One criterion `make(feat_ind)` per level of check_feature_levels() with a non-zero weight, None for the others."""
+    return [make(i) if w != 0.0 else None for i, w in levels]
 
 
 def check_class_weights(weight, classes_num=None):

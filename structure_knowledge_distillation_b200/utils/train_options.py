@@ -14,7 +14,8 @@ DEFAULTS = dict(
     cuda_graph=False,        # ours: capture the step into CUDA graphs after 3 eager steps (NetModel.enable_cuda_graphs)
     ohem=False, ohem_thres=0.7, ohem_keep=100000,   # ours: CriterionOhemDSN(thresh=ohem_thres, min_kept=ohem_keep) as the CE term
     class_weights=None,      # ours: per-class weights of the task cross entropy (e.g. dataset.class_frequency_weights), not with ohem
-    student='resnet18', espnet_p=2, espnet_q=8)     # ours: 'resnet18' (ResNet18-PSP), 'espnet_c' (ESPNet-C with p / q ESP blocks), 'espnet' (ESPNet-C + decoder) or 'mobilenetv2' (dilated MobileNetV2 + PSP head)
+    student='resnet18', espnet_p=2, espnet_q=8,     # ours: 'resnet18' (ResNet18-PSP), 'espnet_c' (ESPNet-C with p / q ESP blocks), 'espnet' (ESPNet-C + decoder) or 'mobilenetv2' (dilated MobileNetV2 + PSP head)
+    at=False, lambda_at=500.0, mimic=False, lambda_mimic=1.0)   # ours: attention-transfer / MIMIC feature terms; a scalar weight: the PSP features, a list: one per level like lambda_pa
 
 
 def make_args(**overrides):
