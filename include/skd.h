@@ -522,6 +522,23 @@ int skd_mse_fwd(long long P, int C, const float* R, int ldr, const float* T, int
 int skd_mse_bwd(long long P, int C, const float* R, int ldr, const float* T, int ldt, const float* grad_out, float* dR, int ldd,
                 cudaStream_t);
 
+/* ---- K. local pair-wise distillation (csrc/pairwise_local.cu): the pair-wise term with node i = (y, x) of the pooled h x w grid
+        connected to j = (y + t d, x + u d), t, u in -r..r (r = (k - 1) / 2, j = i included) inside the grid.  Inputs are
+        skd_pairwise_pool's dense rows pooled[N][h*w][C] (any C >= 1) and rnorm[N][h*w]; k odd in 3..15, d in 1..8.  fp32 FMA dot
+        products, fixed-order double reduction of the loss, no atomics, no allocation: two calls give bit-identical results. ---- */
+/* connected ordered pairs per image, P = (sum_y c_h(y)) * (sum_x c_w(x)), c_h(y) = #{t : 0 <= y + t d < h} */
+long long skd_pairwise_local_pairs(int h, int w, int k, int d);
+/* doubles of `partials` skd_pairwise_local_fwd needs */
+long long skd_pairwise_local_partials(int N, int h, int w, int k, int d);
+/* loss = sum over pairs of (a^T_ij - a^S_ij)^2 / (N * P), a_ij = (f_i . f_j) rnorm_i rnorm_j; E[N][h*w][k*k] (may be NULL) receives
+   a^T - a^S at offset o = (t + r) k + (u + r), 0 where j lies outside the grid */
+int skd_pairwise_local_fwd(int N, int h, int w, int CS, int CT, const float* pooled_S, const float* pooled_T, const float* rnorm_S,
+                           const float* rnorm_T, int k, int d, float* E, float* loss, double* partials, cudaStream_t);
+/* dpooled[N][h*w][CS] = -4 grad_out[0] / (N * P) * rnorm_S[i] * sum_o E[i][o] rnorm_S[j] pooled_S[j]; skd_pairwise_scatter finishes
+   the feature gradient */
+int skd_pairwise_local_bwd(int N, int h, int w, int CS, const float* E, const float* pooled_S, const float* rnorm_S, int k, int d,
+                           const float* grad_out, float* dpooled, cudaStream_t);
+
 #ifdef __cplusplus
 }
 #endif

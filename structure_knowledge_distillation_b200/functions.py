@@ -53,6 +53,28 @@ class PairWiseLoss(torch.autograd.Function):
         return ops.pairwise_bwd(E, pS, rS, arg, g.contiguous(), feat_S), None, None, None
 
 
+class PairWiseLocalLoss(torch.autograd.Function):
+    """The pair-wise term with each pooled node connected to its `window` x `window` neighbours at `dilation` (the pooled grid's
+    nodes j = (y + t d, x + u d) inside the grid, t, u in -r..r): sum over those pairs of (a^T_ij - a^S_ij)^2 / (N * P), P the connected
+    pairs per image.  Pooling and the detached norm are PairWiseLoss's; E is (N, nodes, window^2), never nodes^2."""
+
+    @staticmethod
+    def forward(ctx, feat_S, feat_T, ph, pw, window, dilation):
+        pS, arg, rS = ops.pairwise_pool(feat_S, ph, pw, True)
+        pT, _, rT = ops.pairwise_pool(feat_T, ph, pw, False)
+        h, w = -(-feat_S.shape[2] // ph), -(-feat_S.shape[3] // pw)
+        loss, E = ops.pairwise_local_fwd(pS, pT, rS, rT, h, w, window, dilation, feat_S.requires_grad)
+        ctx.grid = (h, w, window, dilation)
+        ctx.save_for_backward(E, pS, rS, arg, feat_S)
+        return loss
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        E, pS, rS, arg, feat_S = ctx.saved_tensors
+        return ops.pairwise_local_bwd(E, pS, rS, *ctx.grid, arg, g.contiguous(), feat_S), None, None, None, None, None
+
+
 class AttentionTransferLoss(torch.autograd.Function):
     """Attention transfer (Zagoruyko & Komodakis): mean over N*H*W of (at(S) - at(T))^2 with at(x) = F.normalize(x.pow(2).mean(1)
     .view(N, -1)).  The forward keeps the normalised maps and the student's norms for the backward; the teacher gets no gradient."""

@@ -26,8 +26,8 @@ import torch.nn as nn
 from .. import functions as Fn
 from .. import ops
 from ..utils.criterion import (CriterionAdditionalGP, CriterionAdv, CriterionAdvForG, CriterionAT, CriterionMimic,
-                               CriterionPairWiseforWholeFeatAfterPool, CriterionPixelWise, check_feature_levels, check_pa_levels,
-                               feature_level_criteria, pair_wise_level_criteria)
+                               CriterionPairWiseforWholeFeatAfterPool, CriterionPairWiseLocal, CriterionPixelWise, check_feature_levels,
+                               check_pa_levels, check_pa_windows, feature_level_criteria, pair_wise_level_criteria)
 from ..utils.utils import load_D_model, load_S_model, load_T_model
 from .pspnet_combine import Conv2d
 from .sagan_models import Discriminator
@@ -52,6 +52,9 @@ class NetModel(StepModel):
         # None: scalar lambda_pa / pool_scale, one pair-wise term on preds[-5]; else [(lambda, scale)] per level, level `ind` on
         # preds[-(ind + 1)] (x1, x2, x3, x4, PSP features)
         self.pa_levels = check_pa_levels(args)
+        # None: every pair-wise level fully connected (the default); else (window, dilation) of the scalar term, or a list with one
+        # (window or None, dilation) per level -- a window connects each pooled node to its k x k neighbours only
+        self.pa_windows = check_pa_windows(args)
         # [(feat_ind, weight)]: a scalar weight is one term on preds[-5], a list one per level as for Pa
         self.at_levels = check_feature_levels(args, "lambda_at", "attention-transfer", 500.0)
         self.mimic_levels = check_feature_levels(args, "lambda_mimic", "MIMIC", 1.0)
@@ -84,10 +87,14 @@ class NetModel(StepModel):
             self.mimic_adapters = mimic_adapters(self.student, self.teacher, self.mimic_levels).float().to(device).train()
         self._init_training(self.student, self.D_model, extra=self.mimic_adapters)
         self.criterion_pixel_wise = CriterionPixelWise()
-        if self.pa_levels is None:
+        if self.pa_levels is None and self.pa_windows is None:
             self.criterion_pair_wise_for_interfeat = CriterionPairWiseforWholeFeatAfterPool(scale=args.pool_scale, feat_ind=-5)
+        elif self.pa_levels is None:
+            window, dilation = self.pa_windows
+            self.criterion_pair_wise_for_interfeat = CriterionPairWiseLocal(scale=args.pool_scale, feat_ind=-5, window=window,
+                                                                            dilation=dilation)
         else:                                                     # the reference's multi-level form (kd_model.py:81)
-            self.criterion_pair_wise_for_interfeat = pair_wise_level_criteria(self.pa_levels)
+            self.criterion_pair_wise_for_interfeat = pair_wise_level_criteria(self.pa_levels, self.pa_windows)
         self.criterion_adv = CriterionAdv(args.adv_loss_type)
         if args.adv_loss_type == 'wgan-gp':
             self.criterion_AdditionalGP = CriterionAdditionalGP(self.parallel_D, args.lambda_gp)

@@ -718,6 +718,39 @@ def pairwise_affinity_bwd_sm100(E, pS, rS, arg, grad_out, feat_like):
     return dF
 
 
+def pairwise_local_pairs(h, w, k, d):
+    """Connected ordered pairs per image of the local pair-wise term on an h x w node grid (window k, dilation d)."""
+    return int(lib().skd_pairwise_local_pairs(h, w, k, d))
+
+
+def pairwise_local_fwd(pS, pT, rS, rT, h, w, k, d, want_E):
+    """Local pair-wise term over pairwise_pool's rows on their h x w node grid (csrc/pairwise_local.cu): loss (0-dim) and
+    E (N, h*w, k*k) or None."""
+    n, nodes, cs = pS.shape
+    ct = pT.shape[2]
+    if nodes != h * w or pT.shape[:2] != pS.shape[:2]:
+        raise ValueError("local pair-wise: pooled rows %s / %s do not cover a %dx%d grid" % (tuple(pS.shape), tuple(pT.shape), h, w))
+    L = lib()
+    E = torch.empty((n, nodes, k * k), device=pS.device, dtype=torch.float32) if want_E else None
+    parts = torch.empty(L.skd_pairwise_local_partials(n, h, w, k, d), device=pS.device, dtype=torch.float64)
+    loss = torch.empty((), device=pS.device, dtype=torch.float32)
+    L.skd_pairwise_local_fwd(n, h, w, cs, ct, _p(pS), _p(pT), _p(rS), _p(rT), k, d, _p(E), _p(loss), _p(parts), _st())
+    return loss, E
+
+
+def pairwise_local_bwd(E, pS, rS, h, w, k, d, arg, grad_out, feat_like):
+    """d loss / d feature of pairwise_local_fwd: the pooled rows' gradient, scattered through the max-pool argmax (in feat_like's
+    layout, channels-last when feat_like is)."""
+    n, nodes, cs = pS.shape
+    dpooled = torch.empty_like(pS)
+    L = lib()
+    L.skd_pairwise_local_bwd(n, h, w, cs, _p(E), _p(pS), _p(rS), k, d, _p(grad_out), _p(dpooled), _st())
+    dF = torch.zeros(feat_like.shape, device=feat_like.device, dtype=torch.float32).contiguous(memory_format=torch.channels_last) \
+        if feat_like.dim() == 4 and feat_like.stride(1) == 1 else torch.zeros_like(feat_like)
+    L.skd_pairwise_scatter(n, nodes, cs, _p(dpooled), _p(arg), _p(dF), *pixel_strides(dF), _st())
+    return dF
+
+
 # ------------------------------------------------------------------------------------------------ ESPNet-C (csrc/espnet.cu)
 def _rows(t):
     """-> (P, C, pitch) of an NHWC-stored (possibly channel-sliced) tensor."""

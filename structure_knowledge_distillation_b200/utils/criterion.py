@@ -4,6 +4,8 @@
   CriterionPixelWise                          utils/criterion.py:211-226
   CriterionPairWiseforWholeFeatAfterPool      utils/criterion.py:228-245   (alias: CriterionPairWise, the name the
                                               north star uses; it does not exist in the reference tree)
+  CriterionPairWiseLocal                      the pair-wise term over k x k node neighbourhoods (no reference source; it equals
+                                              the class above when the window covers the grid at dilation 1)
   CriterionDSN                                utils/criterion.py:168-188
   CriterionCrossEntropy                       named at kd_model.py:79 (single head: the ESPNet-C student's task loss)
   OhemCrossEntropy2d                          utils/criterion.py:11-90
@@ -22,6 +24,7 @@ Differences, on purpose:
   * when no pixel is kept the loss is NaN, as torch's cross entropy returns, and the gradient is zero.
 """
 import math
+import numbers
 
 import torch
 import torch.nn as nn
@@ -57,7 +60,32 @@ class CriterionPairWiseforWholeFeatAfterPool(nn.Module):
 
 CriterionPairWise = CriterionPairWiseforWholeFeatAfterPool
 
-PA_LEVELS_MAX = 5          # preds[-1] .. preds[-5]: x1, x2, x3, x4 and the PSP features of every student
+
+class CriterionPairWiseLocal(nn.Module):
+    """Local pair-wise loss: pooling and normalisation as CriterionPairWiseforWholeFeatAfterPool's, but node i = (y, x) of the pooled
+    h x w grid is compared only with the nodes j = (y + t * dilation, x + u * dilation), t, u in -r..r (r = (window - 1) / 2), that lie
+    inside the grid, j = i included: L = sum_n sum_i sum_{j in W(i)} (a^T_ij - a^S_ij)^2 / (N * P), P the connected ordered pairs per
+    image.  With dilation 1 and a window covering the grid it is the fully connected term.  pool_scale = 1 / h gives one node per pixel
+    (when w < 2h)."""
+
+    def __init__(self, scale, feat_ind, window, dilation=1):
+        super().__init__()
+        self.feat_ind = feat_ind
+        self.scale = scale
+        self.window = _check_pa_window("pa_window", window)
+        self.dilation = _check_pa_dilation("pa_dilation", dilation)
+
+    def forward(self, preds_S, preds_T):
+        feat_S = preds_S[self.feat_ind]
+        feat_T = preds_T[self.feat_ind].detach()
+        total_w, total_h = feat_T.shape[2], feat_T.shape[3]
+        patch_w, patch_h = int(total_w * self.scale), int(total_h * self.scale)
+        return Fn.PairWiseLocalLoss.apply(feat_S, feat_T, patch_w, patch_h, self.window, self.dilation)
+
+
+PA_WINDOW_MAX, PA_DILATION_MAX = 15, 8
+
+PA_LEVELS_MAX = 5         # preds[-1] .. preds[-5]: x1, x2, x3, x4 and the PSP features of every student
 
 
 def check_pa_levels(args):
@@ -85,6 +113,64 @@ def check_pa_levels(args):
         if not (math.isfinite(s) and 0 < s <= 1):
             raise ValueError("pair-wise level %d: pool_scale must be in (0, 1] (got %r)" % (ind, s))
         levels.append((l, s))
+    return levels
+
+
+def _is_int(v):
+    return isinstance(v, numbers.Integral) and not isinstance(v, bool)
+
+
+def _check_pa_window(what, k):
+    if not _is_int(k) or k % 2 == 0 or not 3 <= k <= PA_WINDOW_MAX:
+        raise ValueError("%s must be None or an odd int in 3..%d (got %r)" % (what, PA_WINDOW_MAX, k))
+    return int(k)
+
+
+def _check_pa_dilation(what, d):
+    if not _is_int(d) or not 1 <= d <= PA_DILATION_MAX:
+        raise ValueError("%s must be an int in 1..%d (got %r)" % (what, PA_DILATION_MAX, d))
+    return int(d)
+
+
+def check_pa_windows(args):
+    """`args.pa_window` / `args.pa_dilation` of NetModel, validated before any device work against the form of `lambda_pa`.  The
+    defaults (None and 1) keep every pair-wise level fully connected -> None.  Otherwise they follow lambda_pa: two scalars when it is
+    a scalar -> (window, dilation) of the single term on preds[-5], or None when the window is None; two lists of its length when it is a
+    list -> [(window or None, dilation)] per level, None keeping that level fully connected.  In the list form a default left as the
+    scalar (pa_window=None or pa_dilation=1) stands for every level.  A window is an odd int in 3..15, a dilation an int in 1..8, and a
+    fully connected level takes dilation 1; anything else raises ValueError naming the field and the level."""
+    win, dil = getattr(args, "pa_window", None), getattr(args, "pa_dilation", 1)
+    win_list, dil_list = isinstance(win, (list, tuple)), isinstance(dil, (list, tuple))
+    if not win_list and not dil_list and win is None and _is_int(dil) and dil == 1:
+        return None
+    lam = getattr(args, "lambda_pa", 0.5)
+    if not isinstance(lam, (list, tuple)):
+        if win_list or dil_list:
+            raise ValueError("pa_window and pa_dilation must be scalars when lambda_pa is a scalar (got %r and %r)" % (win, dil))
+        dil = _check_pa_dilation("pa_dilation", dil)
+        if win is None:
+            raise ValueError("pa_dilation %r needs a local window: pa_window is None (the fully connected term)" % (dil,))
+        return _check_pa_window("pa_window", win), dil
+    n = len(lam)
+    if win is None and not win_list:
+        win = [None] * n
+    elif not win_list:
+        raise ValueError("pa_window must be a list of %d entries when lambda_pa is a list (got %r)" % (n, win))
+    if _is_int(dil) and dil == 1 and not dil_list:
+        dil = [1] * n
+    elif not dil_list:
+        raise ValueError("pa_dilation must be a list of %d entries when lambda_pa is a list (got %r)" % (n, dil))
+    if len(win) != n or len(dil) != n:
+        raise ValueError("pa_window and pa_dilation lists must have %d entries like lambda_pa (got %d and %d)" % (n, len(win), len(dil)))
+    levels = []
+    for ind, (k, d) in enumerate(zip(win, dil)):
+        d = _check_pa_dilation("pair-wise level %d: pa_dilation" % ind, d)
+        if k is None:
+            if d != 1:
+                raise ValueError("pair-wise level %d: pa_dilation %d needs a local window (pa_window is None)" % (ind, d))
+        else:
+            k = _check_pa_window("pair-wise level %d: pa_window" % ind, k)
+        levels.append((k, d))
     return levels
 
 
@@ -123,10 +209,13 @@ def check_feature_levels(args, name, term, default):
     return levels
 
 
-def pair_wise_level_criteria(levels):
+def pair_wise_level_criteria(levels, windows=None):
     """One CriterionPairWiseforWholeFeatAfterPool per level of check_pa_levels(), level `ind` on preds[-(ind + 1)]
-    (kd_model.py:81)."""
-    return [CriterionPairWiseforWholeFeatAfterPool(scale=s, feat_ind=-(ind + 1)) for ind, (_, s) in enumerate(levels)]
+    (kd_model.py:81); a CriterionPairWiseLocal instead where `windows` (check_pa_windows()'s list) gives the level a window."""
+    windows = windows or [(None, 1)] * len(levels)
+    return [CriterionPairWiseforWholeFeatAfterPool(scale=s, feat_ind=-(ind + 1)) if k is None else
+            CriterionPairWiseLocal(scale=s, feat_ind=-(ind + 1), window=k, dilation=d)
+            for ind, ((_, s), (k, d)) in enumerate(zip(levels, windows))]
 
 
 class CriterionAT(nn.Module):

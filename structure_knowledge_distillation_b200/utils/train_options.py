@@ -15,7 +15,8 @@ DEFAULTS = dict(
     ohem=False, ohem_thres=0.7, ohem_keep=100000,   # ours: CriterionOhemDSN(thresh=ohem_thres, min_kept=ohem_keep) as the CE term
     class_weights=None,      # ours: per-class weights of the task cross entropy (e.g. dataset.class_frequency_weights), not with ohem
     student='resnet18', espnet_p=2, espnet_q=8,     # ours: 'resnet18' (ResNet18-PSP), 'espnet_c' (ESPNet-C with p / q ESP blocks), 'espnet' (ESPNet-C + decoder) or 'mobilenetv2' (dilated MobileNetV2 + PSP head)
-    at=False, lambda_at=500.0, mimic=False, lambda_mimic=1.0)   # ours: attention-transfer / MIMIC feature terms; a scalar weight: the PSP features, a list: one per level like lambda_pa
+    at=False, lambda_at=500.0, mimic=False, lambda_mimic=1.0,   # ours: attention-transfer / MIMIC feature terms; a scalar weight: the PSP features, a list: one per level like lambda_pa
+    pa_window=None, pa_dilation=1)   # ours: local pair-wise term, each pooled node against its pa_window x pa_window neighbours at pa_dilation (None: fully connected); scalars or lists like lambda_pa
 
 
 def make_args(**overrides):
