@@ -539,6 +539,20 @@ int skd_pairwise_local_fwd(int N, int h, int w, int CS, int CT, const float* poo
 int skd_pairwise_local_bwd(int N, int h, int w, int CS, const float* E, const float* pooled_S, const float* rnorm_S, int k, int d,
                            const float* grad_out, float* dpooled, cudaStream_t);
 
+/* ---- L. channel-wise distillation (csrc/cwd.cu): p = softmax over the HW positions of x / tau per (image, channel) of the student
+        map S and the teacher map T, both N x C x HW at (image, channel, pixel) strides (NCHW, NHWC, pitched NHWC, channel slices);
+        loss = tau^2 / (N*C) * sum pT (log pT - log pS), log p = x / tau - lse max-subtracted.  Any C >= 1 and HW >= 1 (N <= 32767).
+        Fixed-order double reductions, no atomics, no allocation: two calls give bit-identical results. ---- */
+/* doubles of `workspace` skd_cwd_fwd needs: 4 * N * C * chunks, the pixel chunks a function of (N, C, HW) */
+long long skd_cwd_workspace(int N, int C, int HW);
+/* loss[0]; lse [2][N][C] doubles (student, then teacher): the log-sum-exp of x / tau per (map, n, c), kept for the backward */
+int skd_cwd_fwd(int N, int C, int HW, const float* S, long long s_sn, long long s_sc, long long s_sp, const float* T, long long t_sn,
+                long long t_sc, long long t_sp, float tau, float* loss, double* lse, double* workspace, cudaStream_t);
+/* dS = tau / (N*C) * grad_out[0] * (pS - pT), pS and pT recomputed from the maps and lse, at dS's strides */
+int skd_cwd_bwd(int N, int C, int HW, const float* S, long long s_sn, long long s_sc, long long s_sp, const float* T, long long t_sn,
+                long long t_sc, long long t_sp, float tau, const double* lse, const float* grad_out, float* dS, long long d_sn,
+                long long d_sc, long long d_sp, cudaStream_t);
+
 #ifdef __cplusplus
 }
 #endif

@@ -107,6 +107,27 @@ class MseLoss(torch.autograd.Function):
         return ops.mse_bwd(r, t, g.contiguous()), None
 
 
+class ChannelWiseLoss(torch.autograd.Function):
+    """Channel-wise distillation (Shu et al.): tau^2 / (N*C) * sum over (n, c) of KL(pT || pS), p the softmax of x / tau over the H*W
+    positions of each channel, S and T of one shape.  log p is computed as x / tau - logsumexp (max-subtracted), not as
+    softmax(...).log(): the two agree wherever pS does not underflow, and where it does this form stays finite while the other gives
+    inf / NaN.  The forward keeps the per-channel log-sum-exps; the backward recomputes both softmaxes from them, so no probability
+    map is stored.  The teacher gets no gradient."""
+
+    @staticmethod
+    def forward(ctx, feat_S, feat_T, tau):
+        loss, lse = ops.cwd_fwd(feat_S, feat_T, tau)
+        ctx.save_for_backward(feat_S, feat_T, lse)
+        ctx.tau = tau
+        return loss
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        feat_S, feat_T, lse = ctx.saved_tensors
+        return ops.cwd_bwd(feat_S, feat_T, lse, ctx.tau, g.contiguous()), None, None
+
+
 class DsnCrossEntropy(torch.autograd.Function):
     """CriterionDSN math (utils/criterion.py:179-188): fused upsample + log-softmax + NLL for both heads.  `weight` (C fp32 class
     weights on the device, or None) makes each head's term CrossEntropyLoss(weight=weight)'s weighted mean."""

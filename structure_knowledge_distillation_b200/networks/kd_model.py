@@ -4,7 +4,8 @@ Kept surface: NetModel(args), .set_input(data), .forward(), .student_backward(),
 .optimize_parameters(), .adjust_learning_rate(base_lr, optimizer, i_iter), .lr_poly, .print_info, .save_ckpt,
 .evalute_model; attributes .student .teacher .G_solver .D_solver .preds_S .preds_T .G_loss .mc_G_loss .pi_G_loss
 .pa_G_loss .D_loss (train_and_eval.py:19-30 reads them).  Ours: .at_G_loss / .mimic_G_loss (attention transfer and MIMIC, the
-paper's feature-level baselines; None while off) and .mimic_adapters.
+paper's feature-level baselines; None while off), .cwd_G_loss (channel-wise distillation; None while off) and .mimic_adapters /
+.cwd_adapters.
 
 The step machinery it shares with SegModel is StepModel's (networks/step_model.py); NetModel adds the frozen teacher, the
 discriminator and the distillation terms.
@@ -25,9 +26,10 @@ import torch.nn as nn
 
 from .. import functions as Fn
 from .. import ops
-from ..utils.criterion import (CriterionAdditionalGP, CriterionAdv, CriterionAdvForG, CriterionAT, CriterionMimic,
-                               CriterionPairWiseforWholeFeatAfterPool, CriterionPairWiseLocal, CriterionPixelWise, check_feature_levels,
-                               check_pa_levels, check_pa_windows, feature_level_criteria, pair_wise_level_criteria)
+from ..utils.criterion import (CriterionAdditionalGP, CriterionAdv, CriterionAdvForG, CriterionAT, CriterionCWD, CriterionMimic,
+                               CriterionPairWiseforWholeFeatAfterPool, CriterionPairWiseLocal, CriterionPixelWise, check_cwd_args,
+                               check_feature_levels, check_pa_levels, check_pa_windows, feature_level_criteria,
+                               pair_wise_level_criteria)
 from ..utils.utils import load_D_model, load_S_model, load_T_model
 from .pspnet_combine import Conv2d
 from .sagan_models import Discriminator
@@ -36,9 +38,9 @@ from .step_model import StepModel, _LazyScalar, _arg, build_seg_network
 STUDENTS = ("resnet18", "espnet_c", "espnet", "mobilenetv2")
 
 def mimic_adapters(student, teacher, levels):
-    """MIMIC's 1x1 adapters (with bias, nn.Conv2d's init), one per level of check_feature_levels() with a non-zero weight, from the
-    student's width at that level to the teacher's, as the two networks' level_channels() give them: key `level<ind>` for
-    preds[-(ind + 1)]."""
+    """MIMIC's (and CWD's) 1x1 adapters (with bias, nn.Conv2d's init), one per level of check_feature_levels() with a non-zero
+    weight, from the student's width at that level to the teacher's, as the two networks' level_channels() give them: key
+    `level<ind>` for preds[-(ind + 1)]."""
     cs, ct = student.level_channels(), teacher.level_channels()
     return nn.ModuleDict({"level%d" % (-i - 1): Conv2d(cs[-i - 1], ct[-i - 1], 1, bias=True) for i, w in levels if w != 0.0})
 
@@ -59,6 +61,9 @@ class NetModel(StepModel):
         self.at_levels = check_feature_levels(args, "lambda_at", "attention-transfer", 500.0)
         self.mimic_levels = check_feature_levels(args, "lambda_mimic", "MIMIC", 1.0)
         self.at, self.mimic = _arg(args, "at", False) == True, _arg(args, "mimic", False) == True
+        # channel-wise distillation: the logit term's weight, the temperature and [(feat_ind, weight)] of lambda_cwd_feat ([]: none)
+        self.lambda_cwd, self.cwd_tau, self.cwd_levels = check_cwd_args(args)
+        self.cwd = _arg(args, "cwd", False) == True
         self._check_device()
         self._check_kind("student", "resnet18", STUDENTS)
         device = self.device
@@ -82,10 +87,13 @@ class NetModel(StepModel):
         self.D_model = D_model.float().to(device).train()
         self.parallel_D = self.D_model
 
-        self.mimic_adapters = None
+        self.mimic_adapters = self.cwd_adapters = None
         if self.mimic:                                            # trained with the student: same flat buffer, decay, exchange, graph
             self.mimic_adapters = mimic_adapters(self.student, self.teacher, self.mimic_levels).float().to(device).train()
-        self._init_training(self.student, self.D_model, extra=self.mimic_adapters)
+        if self.cwd and any(w != 0.0 for _, w in self.cwd_levels):   # CWD's own, after MIMIC's (in the flat buffer and the RNG)
+            self.cwd_adapters = mimic_adapters(self.student, self.teacher, self.cwd_levels).float().to(device).train()
+        adapters = [a for a in (self.mimic_adapters, self.cwd_adapters) if a is not None]
+        self._init_training(self.student, self.D_model, extra=nn.ModuleList(adapters) if adapters else None)
         self.criterion_pixel_wise = CriterionPixelWise()
         if self.pa_levels is None and self.pa_windows is None:
             self.criterion_pair_wise_for_interfeat = CriterionPairWiseforWholeFeatAfterPool(scale=args.pool_scale, feat_ind=-5)
@@ -102,6 +110,9 @@ class NetModel(StepModel):
         self.criterion_at = feature_level_criteria(self.at_levels, CriterionAT) if self.at else []
         self.criterion_mimic = feature_level_criteria(
             self.mimic_levels, lambda i: CriterionMimic(i, self.mimic_adapters["level%d" % (-i - 1)])) if self.mimic else []
+        self.criterion_cwd_logits = CriterionCWD(0, self.cwd_tau) if self.cwd and self.lambda_cwd != 0.0 else None
+        self.criterion_cwd = feature_level_criteria(
+            self.cwd_levels, lambda i: CriterionCWD(i, self.cwd_tau, self.cwd_adapters["level%d" % (-i - 1)])) if self.cwd else []
 
         self._teacher_stream = None
         self._d_stream = None
@@ -109,6 +120,7 @@ class NetModel(StepModel):
         self.pa_G_loss = 0.0 if self.pa_levels is None else [0.0] * len(self.pa_levels)
         self.at_G_loss = self._zero_terms(self.at_levels, "lambda_at") if self.at else None
         self.mimic_G_loss = self._zero_terms(self.mimic_levels, "lambda_mimic") if self.mimic else None
+        self.cwd_G_loss = (([0.0] * (1 + len(self.cwd_levels)) if self.cwd_levels else 0.0) if self.cwd else None)
         self.D_loss = 0.0
 
     def forward(self):
@@ -136,8 +148,8 @@ class NetModel(StepModel):
     def _resample_teacher(self):
         """Students on another grid than the teacher (ESPNet-C: 45x60 at 360x480, PSPNet's ceil-mode pool: 46x61; the full ESPNet's
         logits: 360x480): the teacher tensors the distillation terms read -- preds_T[0] and preds_T[-5], or with pair-wise levels
-        preds_T[0] and the preds_T[-(ind + 1)] of every level with a non-zero weight, plus those of the weighted attention-transfer
-        and MIMIC levels -- are each resized onto the grid of their own
+        preds_T[0] and the preds_T[-(ind + 1)] of every level with a non-zero weight, plus those of the weighted attention-transfer,
+        MIMIC and CWD feature levels -- are each resized onto the grid of their own
         student counterpart (bilinear, align_corners=True; forward only, the teacher is frozen).  Equal grids (the ResNet18
         student): nothing runs.  The teacher's own logits stay in `logits_T` for the discriminator of a full-resolution student."""
         self.logits_T = self.preds_T[0]
@@ -148,7 +160,7 @@ class NetModel(StepModel):
             read = [0] + ([len(preds) - 1 - ind for ind, (lam, _) in enumerate(self.pa_levels) if lam != 0.0]
                           if self.args.pa == True else [])
         read = list(read)
-        for terms_on, levels in ((self.at, self.at_levels), (self.mimic, self.mimic_levels)):
+        for terms_on, levels in ((self.at, self.at_levels), (self.mimic, self.mimic_levels), (self.cwd, self.cwd_levels)):
             read += [len(preds) + i for i, w in levels if terms_on and w != 0.0 and len(preds) + i not in read]
         for i in read:
             size = tuple(self.preds_S[i].shape[2:])
@@ -185,6 +197,8 @@ class NetModel(StepModel):
             G_loss, self.at_G_loss = self._feature_terms(G_loss, self.at_levels, self.criterion_at, "lambda_at")
         if self.mimic:
             G_loss, self.mimic_G_loss = self._feature_terms(G_loss, self.mimic_levels, self.criterion_mimic, "lambda_mimic")
+        if self.cwd:
+            G_loss = self._cwd_loss(G_loss)
         if args.ho == True:
             d_out_S = self.parallel_D(self._d_inputs()[0])
             G_loss = G_loss + args.lambda_d * self.criterion_adv_for_G(d_out_S, d_out_S)
@@ -232,9 +246,29 @@ class NetModel(StepModel):
             G_loss = G_loss + w * temp
         return G_loss, (terms if isinstance(_arg(self.args, name, None), (list, tuple)) else terms[0])
 
+    def _cwd_loss(self, G_loss):
+        """G_loss + lambda_cwd * CWD(logits) + sum over lambda_cwd_feat's levels of weight * CWD(adapter(level)), in that order.
+        cwd_G_loss holds the unweighted terms as lazy device scalars: the logit term alone without feature levels, else
+        [logits, level 0, ...] (one feature entry for a scalar lambda_cwd_feat).  A zero weight launches nothing and logs 0.0."""
+        logits = 0.0
+        if self.criterion_cwd_logits is not None:
+            temp = self.criterion_cwd_logits(self.preds_S, self.preds_T)
+            logits = _LazyScalar(temp)
+            G_loss = G_loss + self.lambda_cwd * temp
+        if not self.cwd_levels:
+            self.cwd_G_loss = logits
+            return G_loss
+        G_loss, feat = self._feature_terms(G_loss, self.cwd_levels, self.criterion_cwd, "lambda_cwd_feat")
+        self.cwd_G_loss = [logits] + (feat if isinstance(feat, list) else [feat])
+        return G_loss
+
     def _extra_states(self):
-        adapters = getattr(self, "mimic_adapters", None)
-        return {} if adapters is None else {"mimic_state_dict": adapters}
+        states = {}
+        for field, adapters in (("mimic_state_dict", getattr(self, "mimic_adapters", None)),
+                                ("cwd_state_dict", getattr(self, "cwd_adapters", None))):
+            if adapters is not None:
+                states[field] = adapters
+        return states
 
     def discriminator_backward(self):
         self._discriminator_phase()
@@ -306,7 +340,7 @@ class NetModel(StepModel):
         def terms(v):                                               # a list: one unweighted term per level
             return '[' + ', '.join('{:.5f}'.format(float(t)) for t in v) + ']' if isinstance(v, list) else '{:.5f}'.format(float(v))
         pa = terms(self.pa_G_loss)
-        for name in ('at', 'mimic'):                                # appended only while the term is on
+        for name in ('at', 'mimic', 'cwd'):                         # appended only while the term is on
             v = getattr(self, name + '_G_loss', None)
             if v is not None:
                 pa += ' {}:{}'.format(name, terms(v))

@@ -135,7 +135,7 @@ class StepModel():
     def _init_training(self, net, D_model=None, extra=None):
         """Training state for `net` (on the device): sync_bn, FlatSGD G_solver (and D_solver for NetModel's discriminator `D_model`),
         the gradient exchange across ranks, the task criterion, the CUDA-graph option and the snapshot directory.  `extra`: a module
-        trained with `net` (NetModel's MIMIC adapters), its parameters after net's in G_solver's flat buffer."""
+        trained with `net` (NetModel's MIMIC and CWD adapters), its parameters after net's in G_solver's flat buffer."""
         args = self.args
         if _arg(args, "sync_bn", False):                          # cross-rank batch statistics (the reference's InPlaceABNSync semantics)
             from ..libs import InPlaceABNSync
@@ -332,7 +332,8 @@ class StepModel():
         return parts
 
     def _extra_states(self):
-        """{field: module} saved and restored beside the trained network (NetModel: `mimic_state_dict`, the MIMIC adapters)."""
+        """{field: module} saved and restored beside the trained network (NetModel: `mimic_state_dict` / `cwd_state_dict`, the MIMIC
+        and CWD adapters)."""
         return {}
 
     def save_training_state(self, path, step, epoch=0, best_mean_IU=None, IU_array=None, loader=None):
@@ -342,6 +343,7 @@ class StepModel():
             in S_ckpt_path / ckpt_path, the file loads through load_S_model / load_seg_model (S_resume / resume) like the reference's;
           * `D_state_dict` (spectral-norm u / v, BN buffers included), `G_solver` / `D_solver` (momentum, steps, lr, flat length);
           * with MIMIC, `mimic_state_dict`: the adapters (their momentum is in G_solver);
+          * with CWD feature levels, `cwd_state_dict`: their adapters (likewise);
           * `ranks`: per rank, the torch CPU and CUDA generators, Python `random`, numpy's global generator and `loader.state_dict()`;
           * `format`, `version`, `world_size`, `kind`, `classes_num`: what load_training_state checks.
         Collective: every rank calls it.  Rank 0 writes a temporary file beside `path` and renames it over `path`, so an interrupted

@@ -3,6 +3,8 @@
 Activations are torch tensors of logical shape (N, C, H, W) in channels-last memory (NHWC rows, optional row pitch
 when the tensor is a channel slice of a wider buffer).  Everything runs on the caller's current CUDA stream.
 """
+import math
+
 import torch
 
 from ._cabi import lib
@@ -521,6 +523,37 @@ def mse_bwd(R, T, grad_out):
     dR = empty_nhwc(n, c, h, w, R.device)
     lib().skd_mse_bwd(n * h * w, c, _p(R), ldr, _p(T), nhwc_meta(T)[4], _p(grad_out), _p(dR), c, _st())
     return dR
+
+
+def _cwd_check(S, T, tau):
+    if S.dim() != 4 or tuple(T.shape) != tuple(S.shape):
+        raise ValueError("channel-wise distillation: student %s and teacher %s maps differ in batch, channels or grid"
+                         % (tuple(S.shape), tuple(T.shape)))
+    if not (math.isfinite(tau) and tau > 0):
+        raise ValueError("channel-wise distillation: the temperature must be finite and > 0 (got %r)" % (tau,))
+
+
+def cwd_fwd(S, T, tau):
+    """Channel-wise distillation (csrc/cwd.cu) of student / teacher maps of one (N, C, H, W) shape, NCHW or NHWC (pitch allowed) ->
+    (loss, lse (2, N, C) float64: the log-sum-exp of x / tau over H*W per (map, image, channel), what the backward reads)."""
+    _f32(S, T)
+    _cwd_check(S, T, tau)
+    n, c, h, w = S.shape
+    loss = torch.empty((), device=S.device, dtype=torch.float32)
+    lse = torch.empty((2, n, c), device=S.device, dtype=torch.float64)
+    ws = _ws(S.device, lib().skd_cwd_workspace(n, c, h * w))
+    lib().skd_cwd_fwd(n, c, h * w, _p(S), *pixel_strides(S), _p(T), *pixel_strides(T), float(tau), _p(loss), _p(lse), _p(ws), _st())
+    return loss, lse
+
+
+def cwd_bwd(S, T, lse, tau, grad_out):
+    """d loss / d S of cwd_fwd, in S's layout."""
+    _cwd_check(S, T, tau)
+    n, c, h, w = S.shape
+    dS = torch.empty_strided(S.shape, S.stride(), device=S.device, dtype=torch.float32)
+    lib().skd_cwd_bwd(n, c, h * w, _p(S), *pixel_strides(S), _p(T), *pixel_strides(T), float(tau), _p(lse), _p(grad_out), _p(dS),
+                      *pixel_strides(dS), _st())
+    return dS
 
 
 def _class_weight(weight, l0):

@@ -14,6 +14,8 @@
   CriterionAdditionalGP                       utils/criterion.py:92-120
   CriterionAT / CriterionMimic                the feature-level baselines the paper compares with (no reference source: attention
                                               transfer after Zagoruyko & Komodakis, MIMIC after Li et al.)
+  CriterionCWD                                channel-wise distillation (Shu et al., ICCV 2021), the structured term's usual
+                                              competitor (no reference source)
 
 The OHEM criteria follow the reference's threshold rule (scipy's zoom to a 1/factor grid with its exact arithmetic, the order
 statistic, pixels with p[label] <= threshold kept) but compute it on the device, without the reference's host round trip.
@@ -241,6 +243,49 @@ class CriterionMimic(nn.Module):
 
     def forward(self, preds_S, preds_T):
         return Fn.MseLoss.apply(self.adapter(preds_S[self.feat_ind]), preds_T[self.feat_ind].detach())
+
+
+class CriterionCWD(nn.Module):
+    """Channel-wise distillation (Shu et al.): tau^2 / (N*C) * sum over (n, c) of KL(softmax_HW(T / tau) || softmax_HW(S / tau)), S =
+    preds_S[feat_ind] (through `adapter`, a 1x1 convolution from the student's to the teacher's width, when given) and T =
+    preds_T[feat_ind] detached, on one grid (Fn.ChannelWiseLoss)."""
+
+    def __init__(self, feat_ind, tau, adapter=None):
+        super().__init__()
+        self.feat_ind = feat_ind
+        self.tau = float(tau)
+        self.adapter = adapter
+
+    def forward(self, preds_S, preds_T):
+        s = preds_S[self.feat_ind]
+        if self.adapter is not None:
+            s = self.adapter(s)
+        return Fn.ChannelWiseLoss.apply(s, preds_T[self.feat_ind].detach(), self.tau)
+
+
+def check_cwd_args(args):
+    """NetModel's channel-wise distillation options, validated before any device work -> (lambda_cwd, cwd_tau, feature levels):
+    lambda_cwd a number, finite and >= 0 (the logit term's weight, 0 turns it off); cwd_tau a number, finite and > 0; lambda_cwd_feat
+    None (no feature term, []) or check_feature_levels()' form.  Anything else raises ValueError naming the field."""
+    lam = getattr(args, "lambda_cwd", 3.0)
+    if isinstance(lam, (list, tuple)):
+        raise ValueError("lambda_cwd must be a number, the weight of the logit term (got the list %r; feature levels go in "
+                         "lambda_cwd_feat)" % (lam,))
+    try:
+        lam = float(lam)
+    except (TypeError, ValueError):
+        raise ValueError("lambda_cwd must be a number (got %r)" % (lam,)) from None
+    _check_level_weight("lambda_cwd", lam)
+    tau = getattr(args, "cwd_tau", 4.0)
+    try:
+        tau = float(tau)
+    except (TypeError, ValueError):
+        raise ValueError("cwd_tau must be a number (got %r)" % (tau,)) from None
+    if not (math.isfinite(tau) and tau > 0):
+        raise ValueError("cwd_tau must be finite and > 0 (got %r)" % (tau,))
+    if getattr(args, "lambda_cwd_feat", None) is None:
+        return lam, tau, []
+    return lam, tau, check_feature_levels(args, "lambda_cwd_feat", "CWD", None)
 
 
 def feature_level_criteria(levels, make):

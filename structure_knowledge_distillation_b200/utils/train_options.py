@@ -16,7 +16,8 @@ DEFAULTS = dict(
     class_weights=None,      # ours: per-class weights of the task cross entropy (e.g. dataset.class_frequency_weights), not with ohem
     student='resnet18', espnet_p=2, espnet_q=8,     # ours: 'resnet18' (ResNet18-PSP), 'espnet_c' (ESPNet-C with p / q ESP blocks), 'espnet' (ESPNet-C + decoder) or 'mobilenetv2' (dilated MobileNetV2 + PSP head)
     at=False, lambda_at=500.0, mimic=False, lambda_mimic=1.0,   # ours: attention-transfer / MIMIC feature terms; a scalar weight: the PSP features, a list: one per level like lambda_pa
-    pa_window=None, pa_dilation=1)   # ours: local pair-wise term, each pooled node against its pa_window x pa_window neighbours at pa_dilation (None: fully connected); scalars or lists like lambda_pa
+    pa_window=None, pa_dilation=1,   # ours: local pair-wise term, each pooled node against its pa_window x pa_window neighbours at pa_dilation (None: fully connected); scalars or lists like lambda_pa
+    cwd=False, lambda_cwd=3.0, lambda_cwd_feat=None, cwd_tau=4.0)   # ours: channel-wise distillation on the logits (lambda_cwd) and on feature levels (lambda_cwd_feat: None, or lambda_at's form), one temperature
 
 
 def make_args(**overrides):
