@@ -97,6 +97,45 @@ __device__ __forceinline__ float up_at(const float* __restrict__ p, long long sp
   return (1.f - ly) * ((1.f - lx) * v00 + lx * v01) + ly * ((1.f - lx) * v10 + lx * v11);
 }
 
+// bilinear (align_corners) source index pair and weights of output coordinate dst: v = l0 * src[i0] + l1 * src[i1], with ATen's
+// area_pixel_compute_source_index(align_corners=True): src = scale * dst, scale = (in - 1) / (out - 1)
+struct Bilin { int i0, i1; float l0, l1; };
+__device__ __forceinline__ Bilin bilin(int dst, float scale, int in) {
+  const float src = scale * (float)dst;
+  Bilin b;
+  b.i0 = (int)src; if (b.i0 > in - 1) b.i0 = in - 1;
+  b.i1 = b.i0 + (b.i0 < in - 1 ? 1 : 0);
+  b.l1 = src - (float)b.i0; b.l0 = 1.f - b.l1;
+  return b;
+}
+
+// softmax probability of class lab at the upsampled pixel (by, bx) of logits L (strides sn, sc, sp over image, class, pixel; w source
+// columns), with exactly the DSN row kernel's arithmetic (losses.cu): the two source rows blended first, then the two columns, __expf,
+// times the reciprocal of the sum.  OHEM ranks these values on its threshold grid (ohem.cu) and the row kernel keeps a pixel when its
+// value is <= the threshold: where a grid point lies on a pixel, both must compute the same bits, or the pixel that defines the
+// threshold can come out above it and be dropped.
+template <int CT>
+__device__ __forceinline__ float up_label_prob(const float* __restrict__ L, long long sn, long long sc, long long sp, int n, int C,
+                                               int w, Bilin by, Bilin bx, int lab) {
+  const float* b0 = L + n * sn + (long long)by.i0 * w * sp;
+  const float* b1 = L + n * sn + (long long)by.i1 * w * sp;
+  const long long x0 = (long long)bx.i0 * sp, x1 = (long long)bx.i1 * sp;
+  float v[CT];
+  float m = -INFINITY;
+#pragma unroll
+  for (int c = 0; c < CT; ++c) if (c < C) {
+    const long long o = (long long)c * sc;
+    const float r0 = by.l0 * __ldg(b0 + x0 + o) + by.l1 * __ldg(b1 + x0 + o);
+    const float r1 = by.l0 * __ldg(b0 + x1 + o) + by.l1 * __ldg(b1 + x1 + o);
+    v[c] = bx.l0 * r0 + bx.l1 * r1;
+    m = fmaxf(m, v[c]);
+  }
+  float z = 0.f, e = 0.f;
+#pragma unroll
+  for (int c = 0; c < CT; ++c) if (c < C) { v[c] = __expf(v[c] - m); z += v[c]; if (c == lab) e = v[c]; }
+  return e * (1.f / z);
+}
+
 // Cityscapes label id -> train id (reference dataset/datasets.py:146-151, ids 0..33; everything else passes through).  The one
 // copy of the table: augment.cu maps labels with it, skd_cityscapes_id_tables derives the reverse (train id -> label id) map
 // that evaluation writes test-split predictions with.

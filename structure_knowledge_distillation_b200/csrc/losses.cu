@@ -137,17 +137,6 @@ pixelwise_bwd_kernel(const float* __restrict__ S, const float* __restrict__ T, f
 // ------------------------------------------------------------------------------------------------
 // DSN cross-entropy with fused align_corners bilinear upsampling
 // ------------------------------------------------------------------------------------------------
-struct Bilin { int i0, i1; float l0, l1; };                 // v = l0*src[i0] + l1*src[i1]
-__device__ __forceinline__ Bilin bilin(int dst, float scale, int in) {
-  // ATen area_pixel_compute_source_index(align_corners=True): src = scale*dst, scale=(in-1)/(out-1)
-  const float src = scale * (float)dst;
-  Bilin b;
-  b.i0 = (int)src; if (b.i0 > in - 1) b.i0 = in - 1;
-  b.i1 = b.i0 + (b.i0 < in - 1 ? 1 : 0);
-  b.l1 = src - (float)b.i0; b.l0 = 1.f - b.l1;
-  return b;
-}
-
 // logits of one upsampled pixel + its log-sum-exp
 __device__ __forceinline__ float up_logits(const float* __restrict__ L, Strides st, int n, int C, int w, Bilin by, Bilin bx,
                                            float* v) {

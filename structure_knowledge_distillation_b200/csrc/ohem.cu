@@ -4,7 +4,9 @@
 //     per grid point restates that exactly: source coordinate o * r in double with r = (in - 1) / (out - 1), mode 'constant'
 //     (a coordinate past in - 1 reads 0 for probability AND label), order 0 = floor(c + 0.5), order 1 = the four neighbours
 //     combined in double in scipy's summation order.  The four full-resolution probabilities come straight from the
-//     low-resolution logits (align_corners upsample, fp32 softmax), so nothing at full resolution is materialised.
+//     low-resolution logits (align_corners upsample, fp32 softmax), so nothing at full resolution is materialised; they are computed
+//     as the row kernel that applies the mask computes them (common.cuh up_label_prob), so a grid point that lies on a pixel holds
+//     that pixel's probability bit for bit.
 //   * radix select: the exact k-th smallest zoomed probability (criterion.py:41-47) over the float bits (probabilities are >= 0,
 //     so their bit patterns order like the values; invalid points hold +inf and sort last), four 8-bit passes of integer
 //     histograms -- deterministic, multi-CTA, and without a host round trip, so the step stays capturable in a CUDA graph.
@@ -18,33 +20,6 @@ namespace {
 
 constexpr int kMaxClasses = 32;
 constexpr int kBins = 256;
-
-// p[lab] at full-resolution pixel (Y, X): align_corners bilinear upsample of the logits (ATen's source-index rule, as the DSN
-// kernels of losses.cu), then the fp32 softmax exp(v - max) / sum
-__device__ float up_prob(const float* __restrict__ L, long long sn, long long sc, long long sp, int n, int C, int h, int w,
-                         float sy, float sx, int Y, int X, int lab) {
-  const float fy = sy * (float)Y, fx = sx * (float)X;
-  int y0 = (int)fy; if (y0 > h - 1) y0 = h - 1;
-  int x0 = (int)fx; if (x0 > w - 1) x0 = w - 1;
-  const int y1 = y0 + (y0 < h - 1 ? 1 : 0), x1 = x0 + (x0 < w - 1 ? 1 : 0);
-  const float ly1 = fy - (float)y0, ly0 = 1.f - ly1, lx1 = fx - (float)x0, lx0 = 1.f - lx1;
-  const float* b = L + n * sn;
-  const float* p00 = b + ((long long)y0 * w + x0) * sp; const float* p01 = b + ((long long)y0 * w + x1) * sp;
-  const float* p10 = b + ((long long)y1 * w + x0) * sp; const float* p11 = b + ((long long)y1 * w + x1) * sp;
-  float v[kMaxClasses];
-  float m = -INFINITY, pick = 0.f;
-#pragma unroll
-  for (int c = 0; c < kMaxClasses; ++c) if (c < C) {
-    const long long o = c * sc;
-    v[c] = ly0 * (lx0 * __ldg(p00 + o) + lx1 * __ldg(p01 + o)) + ly1 * (lx0 * __ldg(p10 + o) + lx1 * __ldg(p11 + o));
-    m = fmaxf(m, v[c]);
-    if (c == lab) pick = v[c];
-  }
-  float z = 0.f;
-#pragma unroll
-  for (int c = 0; c < kMaxClasses; ++c) if (c < C) z += expf(v[c] - m);
-  return expf(pick - m) / z;
-}
 
 __global__ void __launch_bounds__(256)
 ohem_grid_kernel(const float* __restrict__ L, long long sn, long long sc, long long sp, const long long* __restrict__ labels,
@@ -72,10 +47,12 @@ ohem_grid_kernel(const float* __restrict__ L, long long sn, long long sc, long l
       v = 0.f;
       if (!outside) {
         const int lb = (int)lab;
-        const double p00 = up_prob(L, sn, sc, sp, n, C, h, w, sy, sx, ay.i0, ax.i0, lb);
-        const double p01 = up_prob(L, sn, sc, sp, n, C, h, w, sy, sx, ay.i0, ax.i1, lb);
-        const double p10 = up_prob(L, sn, sc, sp, n, C, h, w, sy, sx, ay.i1, ax.i0, lb);
-        const double p11 = up_prob(L, sn, sc, sp, n, C, h, w, sy, sx, ay.i1, ax.i1, lb);
+        // p[lab] at the four full-resolution pixels, computed as the row kernel that applies the mask computes them
+        const Bilin by0 = bilin(ay.i0, sy, h), by1 = bilin(ay.i1, sy, h), bx0 = bilin(ax.i0, sx, w), bx1 = bilin(ax.i1, sx, w);
+        const double p00 = up_label_prob<kMaxClasses>(L, sn, sc, sp, n, C, w, by0, bx0, lb);
+        const double p01 = up_label_prob<kMaxClasses>(L, sn, sc, sp, n, C, w, by0, bx1, lb);
+        const double p10 = up_label_prob<kMaxClasses>(L, sn, sc, sp, n, C, w, by1, bx0, lb);
+        const double p11 = up_label_prob<kMaxClasses>(L, sn, sc, sp, n, C, w, by1, bx1, lb);
         v = (float)zoom_lerp(p00, p01, p10, p11, ay, ax);                     // the zoomed array has the input's dtype
       }
     }

@@ -43,6 +43,41 @@ def ohem_grid(prob, target, factor, ignore_label=255):
     return np.where(valid, pred, np.float32(np.inf)).astype(np.float32), zt.astype(np.int64)
 
 
+def zoom_axis64(n_in, n_out, device=None):
+    """scipy.ndimage.zoom's source coordinates along one axis (csrc/common.cuh zoom_ratio / zoom_axis), float64 torch ->
+    (i0, i1, t, w0, nearest, outside): i0 / i1 the order-1 neighbours with weights w0 = 1 - t / t, `nearest` the order-0 source
+    (floor(c + 0.5)), `outside` the points past n_in - 1 that mode 'constant' reads as 0."""
+    r = (n_in - 1) / (n_out - 1) if n_out > 1 else 1.0
+    c = torch.arange(n_out, dtype=torch.float64, device=device) * r
+    outside = c > n_in - 1
+    f = torch.floor(c)
+    t = c - f
+    i0 = f.long().clamp_max(n_in - 1)                          # (an outside point reads nothing: the clamp only keeps it indexable)
+    i1 = (i0 + 1).clamp_max(n_in - 1)
+    nearest = torch.floor(c + 0.5).long().clamp_max(n_in - 1)
+    return i0, i1, t, 1.0 - t, nearest, outside
+
+
+def ohem_grid64(prob, target, gh, gw, ignore_label=255):
+    """ohem_grid in float64 torch on any device: prob (N, C, H, W) float64, target (N, H, W) int64 -> (pred (N, gh, gw) float64 with
+    +inf where the zoomed label is ignored, zoomed labels (N, gh, gw) int64).  The four neighbours are weighted value * w_y * w_x
+    and summed in scipy's order (common.cuh zoom_lerp); for float32 `prob` upcast to float64, pred.float() is scipy's output."""
+    H, W = target.shape[1:]
+    y0, y1, ty, wy, ny, oy = (a[:, None] for a in zoom_axis64(H, gh, prob.device))
+    x0, x1, tx, wx, nx, ox = zoom_axis64(W, gw, prob.device)
+    outside = oy | ox
+    lab = torch.where(outside, 0, target[:, ny, nx])
+    valid = lab != ignore_label
+    idx = torch.where(valid, lab, 0).clamp(0, prob.shape[1] - 1)[:, None]
+    p = [prob[:, :, a, b].gather(1, idx)[:, 0] for a, b in ((y0, x0), (y0, x1), (y1, x0), (y1, x1))]
+    v = p[0] * wy * wx
+    v = v + p[1] * wy * tx
+    v = v + p[2] * ty * wx
+    v = v + p[3] * ty * tx
+    v = torch.where(outside, 0.0, v)
+    return torch.where(valid, v, float("inf")), lab
+
+
 def ohem_threshold(pred, min_kept, thresh):
     """criterion.py:27-48 on the grid values: 1.0 when min_kept >= valid, else thresh raised to the (min_kept-1)-th smallest."""
     valid = pred[np.isfinite(pred)]
