@@ -553,6 +553,26 @@ int skd_cwd_bwd(int N, int C, int HW, const float* S, long long s_sn, long long 
                 long long t_sc, long long t_sp, float tau, const double* lse, const float* grad_out, float* dS, long long d_sn,
                 long long d_sc, long long d_sp, cudaStream_t);
 
+/* ---- M. intra-class feature variation distillation (csrc/ifv.cu): per image n and class k in [0, K), 1 <= K <= 255, the prototype
+        P[n,k] = sum of the features of the pixels labelled k / (count + 1e-6), separately for the student map S (CS channels) and the
+        teacher map T (CT channels), both N x HW NHWC rows at (image, pixel) strides with contiguous channels (pitches and channel
+        slices allowed); cos_i = cosine_similarity(f_i, P[n, lab_i]) (eps 1e-8); loss = sum over the pixels labelled in [0, K) of
+        (cos_S - cos_T)^2 / (N * HW).  Pixels with another label add exactly 0 to the loss and the gradient.  Fixed-order double
+        reductions, no atomics, no allocation: two calls give bit-identical results. ---- */
+/* out[N][h][w] int32 = labels[N][H][W] (contiguous int64) at F.interpolate(mode="nearest")'s source pixel
+   min(floor(dst * (float(in) / out)), in - 1), the product rounded once in fp32; labels outside the int32 range become -1 */
+int skd_labels_nearest(int N, int H, int W, const long long* labels, int h, int w, int* out, cudaStream_t);
+/* doubles of `workspace` skd_ifv_fwd and skd_ifv_bwd need */
+long long skd_ifv_workspace(int N, int HW, int K, int CS, int CT);
+/* lab[N][HW] int32 (skd_labels_nearest's map) -> loss[0]; PS [N][K][CS] fp32 (the student's prototypes); stats [3][N][K] doubles:
+   the counts, |P_S|^2 and |P_T|^2; pix [3][N][HW] fp32: cos_S, cos_S - cos_T and |f_S| (0 for an ignored pixel) */
+int skd_ifv_fwd(int N, int HW, int K, const int* lab, const float* S, int CS, long long s_sn, long long s_sp, const float* T, int CT,
+                long long t_sn, long long t_sp, float* loss, float* PS, double* stats, float* pix, double* workspace, cudaStream_t);
+/* dS = grad_out[0] * d loss / d S (through the student's cosines and its prototypes) from what skd_ifv_fwd kept, at dS's strides */
+int skd_ifv_bwd(int N, int HW, int K, const int* lab, const float* S, int CS, long long s_sn, long long s_sp, const float* PS,
+                const double* stats, const float* pix, const float* grad_out, float* dS, long long d_sn, long long d_sp,
+                double* workspace, cudaStream_t);
+
 #ifdef __cplusplus
 }
 #endif

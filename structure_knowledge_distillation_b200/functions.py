@@ -128,6 +128,28 @@ class ChannelWiseLoss(torch.autograd.Function):
         return ops.cwd_bwd(feat_S, feat_T, lse, ctx.tau, g.contiguous()), None, None
 
 
+class IntraClassVariationLoss(torch.autograd.Function):
+    """Intra-class feature variation distillation (Wang et al., IFVD): per image and class k in [0, K), the prototype of each map is the
+    mean feature of the pixels labelled k (the labels taken down to the maps' grid by nearest, / (count + 1e-6)); the loss is the mean
+    over all N*h*w pixels of (cos(f_S, P_S) - cos(f_T, P_T))^2, cos torch's cosine_similarity (eps 1e-8).  A pixel labelled outside
+    [0, K) (the ignore label) adds exactly 0 to the loss and the gradient; IFVD's code makes it its own centre, cos = 1 in both maps, which
+    agrees up to the last bits.  S gets its gradient through its cosines and through its prototypes; the teacher gets none.  S and T may
+    differ in width."""
+
+    @staticmethod
+    def forward(ctx, feat_S, feat_T, labels, classes_num):
+        loss, saved = ops.ifv_fwd(feat_S, feat_T, labels, classes_num)
+        ctx.save_for_backward(feat_S, *saved)
+        ctx.classes_num = classes_num
+        return loss
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        feat_S, *saved = ctx.saved_tensors
+        return ops.ifv_bwd(feat_S, saved, ctx.classes_num, g.contiguous()), None, None, None
+
+
 class DsnCrossEntropy(torch.autograd.Function):
     """CriterionDSN math (utils/criterion.py:179-188): fused upsample + log-softmax + NLL for both heads.  `weight` (C fp32 class
     weights on the device, or None) makes each head's term CrossEntropyLoss(weight=weight)'s weighted mean."""

@@ -4,8 +4,8 @@ Kept surface: NetModel(args), .set_input(data), .forward(), .student_backward(),
 .optimize_parameters(), .adjust_learning_rate(base_lr, optimizer, i_iter), .lr_poly, .print_info, .save_ckpt,
 .evalute_model; attributes .student .teacher .G_solver .D_solver .preds_S .preds_T .G_loss .mc_G_loss .pi_G_loss
 .pa_G_loss .D_loss (train_and_eval.py:19-30 reads them).  Ours: .at_G_loss / .mimic_G_loss (attention transfer and MIMIC, the
-paper's feature-level baselines; None while off), .cwd_G_loss (channel-wise distillation; None while off) and .mimic_adapters /
-.cwd_adapters.
+paper's feature-level baselines; None while off), .cwd_G_loss (channel-wise distillation; None while off), .ifv_G_loss (intra-class
+feature variation distillation; None while off) and .mimic_adapters / .cwd_adapters.
 
 The step machinery it shares with SegModel is StepModel's (networks/step_model.py); NetModel adds the frozen teacher, the
 discriminator and the distillation terms.
@@ -26,10 +26,10 @@ import torch.nn as nn
 
 from .. import functions as Fn
 from .. import ops
-from ..utils.criterion import (CriterionAdditionalGP, CriterionAdv, CriterionAdvForG, CriterionAT, CriterionCWD, CriterionMimic,
-                               CriterionPairWiseforWholeFeatAfterPool, CriterionPairWiseLocal, CriterionPixelWise, check_cwd_args,
-                               check_feature_levels, check_pa_levels, check_pa_windows, feature_level_criteria,
-                               pair_wise_level_criteria)
+from ..utils.criterion import (CriterionAdditionalGP, CriterionAdv, CriterionAdvForG, CriterionAT, CriterionCWD, CriterionIFV,
+                               CriterionMimic, CriterionPairWiseforWholeFeatAfterPool, CriterionPairWiseLocal, CriterionPixelWise,
+                               check_cwd_args, check_feature_levels, check_ifv_args, check_pa_levels, check_pa_windows,
+                               feature_level_criteria, pair_wise_level_criteria)
 from ..utils.utils import load_D_model, load_S_model, load_T_model
 from .pspnet_combine import Conv2d
 from .sagan_models import Discriminator
@@ -64,6 +64,9 @@ class NetModel(StepModel):
         # channel-wise distillation: the logit term's weight, the temperature and [(feat_ind, weight)] of lambda_cwd_feat ([]: none)
         self.lambda_cwd, self.cwd_tau, self.cwd_levels = check_cwd_args(args)
         self.cwd = _arg(args, "cwd", False) == True
+        # intra-class feature variation distillation: [(feat_ind, weight)] of lambda_ifv while ifv is on, else []
+        self.ifv_levels = check_ifv_args(args)
+        self.ifv = bool(self.ifv_levels)
         self._check_device()
         self._check_kind("student", "resnet18", STUDENTS)
         device = self.device
@@ -113,6 +116,7 @@ class NetModel(StepModel):
         self.criterion_cwd_logits = CriterionCWD(0, self.cwd_tau) if self.cwd and self.lambda_cwd != 0.0 else None
         self.criterion_cwd = feature_level_criteria(
             self.cwd_levels, lambda i: CriterionCWD(i, self.cwd_tau, self.cwd_adapters["level%d" % (-i - 1)])) if self.cwd else []
+        self.criterion_ifv = feature_level_criteria(self.ifv_levels, lambda i: CriterionIFV(i, args.classes_num))
 
         self._teacher_stream = None
         self._d_stream = None
@@ -121,6 +125,7 @@ class NetModel(StepModel):
         self.at_G_loss = self._zero_terms(self.at_levels, "lambda_at") if self.at else None
         self.mimic_G_loss = self._zero_terms(self.mimic_levels, "lambda_mimic") if self.mimic else None
         self.cwd_G_loss = (([0.0] * (1 + len(self.cwd_levels)) if self.cwd_levels else 0.0) if self.cwd else None)
+        self.ifv_G_loss = self._zero_terms(self.ifv_levels, "lambda_ifv") if self.ifv else None
         self.D_loss = 0.0
 
     def forward(self):
@@ -149,7 +154,7 @@ class NetModel(StepModel):
         """Students on another grid than the teacher (ESPNet-C: 45x60 at 360x480, PSPNet's ceil-mode pool: 46x61; the full ESPNet's
         logits: 360x480): the teacher tensors the distillation terms read -- preds_T[0] and preds_T[-5], or with pair-wise levels
         preds_T[0] and the preds_T[-(ind + 1)] of every level with a non-zero weight, plus those of the weighted attention-transfer,
-        MIMIC and CWD feature levels -- are each resized onto the grid of their own
+        MIMIC, CWD and IFV feature levels -- are each resized onto the grid of their own
         student counterpart (bilinear, align_corners=True; forward only, the teacher is frozen).  Equal grids (the ResNet18
         student): nothing runs.  The teacher's own logits stay in `logits_T` for the discriminator of a full-resolution student."""
         self.logits_T = self.preds_T[0]
@@ -160,7 +165,8 @@ class NetModel(StepModel):
             read = [0] + ([len(preds) - 1 - ind for ind, (lam, _) in enumerate(self.pa_levels) if lam != 0.0]
                           if self.args.pa == True else [])
         read = list(read)
-        for terms_on, levels in ((self.at, self.at_levels), (self.mimic, self.mimic_levels), (self.cwd, self.cwd_levels)):
+        for terms_on, levels in ((self.at, self.at_levels), (self.mimic, self.mimic_levels), (self.cwd, self.cwd_levels),
+                                 (self.ifv, self.ifv_levels)):
             read += [len(preds) + i for i, w in levels if terms_on and w != 0.0 and len(preds) + i not in read]
         for i in read:
             size = tuple(self.preds_S[i].shape[2:])
@@ -199,6 +205,8 @@ class NetModel(StepModel):
             G_loss, self.mimic_G_loss = self._feature_terms(G_loss, self.mimic_levels, self.criterion_mimic, "lambda_mimic")
         if self.cwd:
             G_loss = self._cwd_loss(G_loss)
+        if self.ifv:                                            # the labels are taken down to each level's grid inside the term
+            G_loss, self.ifv_G_loss = self._feature_terms(G_loss, self.ifv_levels, self.criterion_ifv, "lambda_ifv", self.labels)
         if args.ho == True:
             d_out_S = self.parallel_D(self._d_inputs()[0])
             G_loss = G_loss + args.lambda_d * self.criterion_adv_for_G(d_out_S, d_out_S)
@@ -230,18 +238,19 @@ class NetModel(StepModel):
         return G_loss
 
     def _zero_terms(self, levels, name):
-        """What at_G_loss / mimic_G_loss log before the first step: 0.0, or one 0.0 per level when args.<name> is a list."""
+        """What at_G_loss / mimic_G_loss / ifv_G_loss log before the first step: 0.0, or one 0.0 per level when args.<name> is a list."""
         return [0.0] * len(levels) if isinstance(_arg(self.args, name, None), (list, tuple)) else 0.0
 
-    def _feature_terms(self, G_loss, levels, crits, name):
+    def _feature_terms(self, G_loss, levels, crits, name, *extra):
         """G_loss + sum over levels of weight * term -> (that sum, the unweighted terms as lazy device scalars: a list when args.<name>
-        is one, else the single term).  A level with weight 0 launches nothing and logs 0.0."""
+        is one, else the single term).  A level with weight 0 launches nothing and logs 0.0.  `extra`: further arguments of each
+        criterion after (preds_S, preds_T) (IFV's labels)."""
         terms = []
         for (_, w), crit in zip(levels, crits):
             if crit is None:
                 terms.append(0.0)
                 continue
-            temp = crit(self.preds_S, self.preds_T)
+            temp = crit(self.preds_S, self.preds_T, *extra)
             terms.append(_LazyScalar(temp))
             G_loss = G_loss + w * temp
         return G_loss, (terms if isinstance(_arg(self.args, name, None), (list, tuple)) else terms[0])
@@ -340,7 +349,7 @@ class NetModel(StepModel):
         def terms(v):                                               # a list: one unweighted term per level
             return '[' + ', '.join('{:.5f}'.format(float(t)) for t in v) + ']' if isinstance(v, list) else '{:.5f}'.format(float(v))
         pa = terms(self.pa_G_loss)
-        for name in ('at', 'mimic', 'cwd'):                         # appended only while the term is on
+        for name in ('at', 'mimic', 'cwd', 'ifv'):                  # appended only while the term is on
             v = getattr(self, name + '_G_loss', None)
             if v is not None:
                 pa += ' {}:{}'.format(name, terms(v))

@@ -556,6 +556,79 @@ def cwd_bwd(S, T, lse, tau, grad_out):
     return dS
 
 
+def _labels_check(labels, n):
+    if labels.dtype != torch.int64 or labels.dim() != 3 or not labels.is_contiguous():
+        raise ValueError("labels must be a contiguous (N, H, W) int64 tensor (got %s %s%s)"
+                         % (labels.dtype, tuple(labels.shape), "" if labels.is_contiguous() else ", not contiguous"))
+    if n is not None and labels.shape[0] != n:
+        raise ValueError("labels hold %d images for a batch of %d" % (labels.shape[0], n))
+
+
+def labels_nearest(labels, h, w):
+    """(N, H, W) int64 labels on the device -> (N, h, w) int32, each the label F.interpolate(labels[:, None].float(), (h, w),
+    mode="nearest") picks (torch's legacy rule src = min(floor(dst * (float(in) / out)), in - 1) in fp32); labels outside the int32
+    range become -1."""
+    _labels_check(labels, None)
+    if not labels.is_cuda:
+        raise RuntimeError("libskd_b200 has no CPU path: tensor is on %s" % labels.device)
+    if h < 1 or w < 1:
+        raise ValueError("labels_nearest: empty grid %dx%d" % (h, w))
+    n, H, W = labels.shape
+    out = torch.empty((n, h, w), device=labels.device, dtype=torch.int32)
+    lib().skd_labels_nearest(n, H, W, _p(labels), h, w, _p(out), _st())
+    return out
+
+
+def _ifv_check(S, T, labels, classes_num):
+    if S.dim() != 4 or T.dim() != 4 or S.shape[0] != T.shape[0] or tuple(S.shape[2:]) != tuple(T.shape[2:]):
+        raise ValueError("intra-class variation: student %s and teacher %s maps differ in batch or grid"
+                         % (tuple(S.shape), tuple(T.shape)))
+    _labels_check(labels, S.shape[0])
+    if not 1 <= classes_num <= 255:
+        raise ValueError("intra-class variation: the class count must be in [1, 255] (got %r)" % (classes_num,))
+
+
+def _row_strides(t):
+    """(sn, sp) of an NHWC-stored (pitch allowed) map."""
+    n, c, h, w, pitch = nhwc_meta(t)
+    return h * w * pitch, pitch
+
+
+def ifv_fwd(S, T, labels, classes_num):
+    """Intra-class feature variation distillation (csrc/ifv.cu) of NHWC-stored (pitch allowed) student / teacher maps on one grid, with
+    the step's (N, H, W) int64 labels -> (loss, saved): `saved` = (lab (N, h, w) int32 from labels_nearest, P_S (N, K, C_S) fp32, stats
+    (3, N, K) float64: counts, |P_S|^2, |P_T|^2, pix (3, N, h*w) fp32: cos_S, cos_S - cos_T, |f_S|), what ifv_bwd reads."""
+    _f32(S, T)
+    _ifv_check(S, T, labels, classes_num)
+    n, cs, h, w = S.shape
+    ct, k = T.shape[1], int(classes_num)
+    lab = labels_nearest(labels, h, w)
+    loss = torch.empty((), device=S.device, dtype=torch.float32)
+    PS = torch.empty((n, k, cs), device=S.device, dtype=torch.float32)
+    stats = torch.empty((3, n, k), device=S.device, dtype=torch.float64)
+    pix = torch.empty((3, n, h * w), device=S.device, dtype=torch.float32)
+    ws = _ws(S.device, lib().skd_ifv_workspace(n, h * w, k, cs, ct))
+    lib().skd_ifv_fwd(n, h * w, k, _p(lab), _p(S), cs, *_row_strides(S), _p(T), ct, *_row_strides(T), _p(loss), _p(PS), _p(stats),
+                      _p(pix), _p(ws), _st())
+    return loss, (lab, PS, stats, pix)
+
+
+def ifv_bwd(S, saved, classes_num, grad_out):
+    """d loss / d S of ifv_fwd (through the student's cosines and its prototypes) from its `saved` tensors, dense NHWC."""
+    lab, PS, stats, pix = saved
+    _f32(S)
+    if S.dim() != 4 or tuple(lab.shape) != (S.shape[0],) + tuple(S.shape[2:]) or tuple(PS.shape) != (S.shape[0], classes_num, S.shape[1]):
+        raise ValueError("intra-class variation: the saved tensors do not match the student map %s" % (tuple(S.shape),))
+    if not 1 <= classes_num <= 255:
+        raise ValueError("intra-class variation: the class count must be in [1, 255] (got %r)" % (classes_num,))
+    n, cs, h, w = S.shape
+    dS = empty_nhwc(n, cs, h, w, S.device)
+    ws = _ws(S.device, lib().skd_ifv_workspace(n, h * w, classes_num, cs, cs))
+    lib().skd_ifv_bwd(n, h * w, classes_num, _p(lab), _p(S), cs, *_row_strides(S), _p(PS), _p(stats), _p(pix), _p(grad_out), _p(dS),
+                      *_row_strides(dS), _p(ws), _st())
+    return dS
+
+
 def _class_weight(weight, l0):
     """The class-weight table as the weighted kernels read it: contiguous fp32, one entry per class, on the logits' device."""
     if weight.dtype != torch.float32 or not weight.is_contiguous() or weight.dim() != 1 or weight.device != l0.device:

@@ -16,6 +16,8 @@
                                               transfer after Zagoruyko & Komodakis, MIMIC after Li et al.)
   CriterionCWD                                channel-wise distillation (Shu et al., ICCV 2021), the structured term's usual
                                               competitor (no reference source)
+  CriterionIFV                                intra-class feature variation distillation (Wang et al., ECCV 2020), structured KD's
+                                              successor on the same setting (no reference source)
 
 The OHEM criteria follow the reference's threshold rule (scipy's zoom to a 1/factor grid with its exact arithmetic, the order
 statistic, pixels with p[label] <= threshold kept) but compute it on the device, without the reference's host round trip.
@@ -286,6 +288,36 @@ def check_cwd_args(args):
     if getattr(args, "lambda_cwd_feat", None) is None:
         return lam, tau, []
     return lam, tau, check_feature_levels(args, "lambda_cwd_feat", "CWD", None)
+
+
+class CriterionIFV(nn.Module):
+    """Intra-class feature variation distillation (Wang et al., IFVD) of preds_S[feat_ind] against preds_T[feat_ind] detached, on one
+    grid, with the step's (N, H, W) int64 labels taken down to that grid by nearest (Fn.IntraClassVariationLoss): per image and class in
+    [0, classes_num) the prototype of each map, then the mean over all pixels of (cos(f_S, P_S) - cos(f_T, P_T))^2.  `ignore_index`
+    names the unlabelled pixels' label; like every label outside [0, classes_num) they add nothing, so it must lie outside that range."""
+
+    def __init__(self, feat_ind, classes_num, ignore_index=255):
+        super().__init__()
+        if not 1 <= int(classes_num) <= 255:
+            raise ValueError("IFV needs 1 <= classes_num <= 255 (got %r)" % (classes_num,))
+        if 0 <= ignore_index < classes_num:
+            raise ValueError("IFV: ignore_index %r is one of the %d classes" % (ignore_index, classes_num))
+        self.feat_ind = feat_ind
+        self.classes_num = int(classes_num)
+        self.ignore_index = ignore_index
+
+    def forward(self, preds_S, preds_T, labels):
+        return Fn.IntraClassVariationLoss.apply(preds_S[self.feat_ind], preds_T[self.feat_ind].detach(), labels, self.classes_num)
+
+
+def check_ifv_args(args):
+    """NetModel's IFV options, validated before any device work -> [(feat_ind, weight)] of lambda_ifv (check_feature_levels()' form),
+    or [] while the term is off.  `ifv` must be True or False (a string such as "False" would otherwise read as on)."""
+    on = getattr(args, "ifv", False)
+    if not (isinstance(on, (bool, int)) and on in (0, 1)):
+        raise ValueError("ifv must be True or False (got %r)" % (on,))
+    levels = check_feature_levels(args, "lambda_ifv", "IFV", 200.0)
+    return levels if on else []
 
 
 def feature_level_criteria(levels, make):

@@ -17,7 +17,8 @@ DEFAULTS = dict(
     student='resnet18', espnet_p=2, espnet_q=8,     # ours: 'resnet18' (ResNet18-PSP), 'espnet_c' (ESPNet-C with p / q ESP blocks), 'espnet' (ESPNet-C + decoder) or 'mobilenetv2' (dilated MobileNetV2 + PSP head)
     at=False, lambda_at=500.0, mimic=False, lambda_mimic=1.0,   # ours: attention-transfer / MIMIC feature terms; a scalar weight: the PSP features, a list: one per level like lambda_pa
     pa_window=None, pa_dilation=1,   # ours: local pair-wise term, each pooled node against its pa_window x pa_window neighbours at pa_dilation (None: fully connected); scalars or lists like lambda_pa
-    cwd=False, lambda_cwd=3.0, lambda_cwd_feat=None, cwd_tau=4.0)   # ours: channel-wise distillation on the logits (lambda_cwd) and on feature levels (lambda_cwd_feat: None, or lambda_at's form), one temperature
+    cwd=False, lambda_cwd=3.0, lambda_cwd_feat=None, cwd_tau=4.0,   # ours: channel-wise distillation on the logits (lambda_cwd) and on feature levels (lambda_cwd_feat: None, or lambda_at's form), one temperature
+    ifv=False, lambda_ifv=200.0)   # ours: intra-class feature variation distillation, lambda_at's form (a scalar: the PSP features); 200 is a starting value, not tuned here
 
 
 def make_args(**overrides):
