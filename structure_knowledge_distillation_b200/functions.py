@@ -268,7 +268,8 @@ def _direct_grad(param, shape_ohwi=None):
         return None
     if shape_ohwi is not None:
         cout, kh, kw, cin = shape_ohwi
-        if tuple(g.shape) != (cout, cin, kh, kw) or g.stride() != (kh * kw * cin, 1, kw * cin, cin):
+        dense = (kh * kw * cin, 1, kw * cin, cin)                # the stride of a size-1 dimension does not matter (1x1 filters)
+        if tuple(g.shape) != (cout, cin, kh, kw) or any(n > 1 and s != d for n, s, d in zip(g.shape, g.stride(), dense)):
             return None
     elif g.dim() != 1 or not g.is_contiguous():
         return None
