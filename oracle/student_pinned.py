@@ -31,13 +31,14 @@ def pin(t):
 class _Pinned(torch.autograd.Function):
     """y = op(x, w) exactly in float64; the backward differentiates op at the pinned operands: dx from (tf32(w), tf32(dy)), dw from
     (tf32(x), tf32(dy)).  op is linear in each argument, so both gradients come from one autograd pass over the rounded values.
-    pinned=False differentiates at the operands themselves (plain float64 autograd)."""
+    pinned=False differentiates at the operands themselves (plain float64 autograd).  pinned_forward=True evaluates the forward at
+    (tf32(x), tf32(w)) too, exactly in float64, as a TF32 (not 3xTF32) forward kernel reads its operands."""
 
     @staticmethod
-    def forward(ctx, x, w, op, pinned):
+    def forward(ctx, x, w, op, pinned, pinned_forward=False):
         ctx.save_for_backward(x, w)
         ctx.op, ctx.pinned = op, pinned
-        return op(x, w)
+        return op(pin(x), pin(w)) if pinned_forward else op(x, w)
 
     @staticmethod
     def backward(ctx, dy):
@@ -47,15 +48,16 @@ class _Pinned(torch.autograd.Function):
         with torch.enable_grad():
             y = ctx.op(xr, wr)
         dx, dw = torch.autograd.grad(y, (xr, wr), rnd(dy))
-        return (dx if ctx.needs_input_grad[0] else None), (dw if ctx.needs_input_grad[1] else None), None, None
+        return (dx if ctx.needs_input_grad[0] else None), (dw if ctx.needs_input_grad[1] else None), None, None, None
 
 
-def conv2d(x, w, bias=None, stride=1, padding=0, dilation=1, pinned=True):
+def conv2d(x, w, bias=None, stride=1, padding=0, dilation=1, pinned=True, pinned_forward=False):
     """F.conv2d(x, w, bias, stride, padding, dilation) in float64 with (pinned=True) the TF32-pinned backward (the bias gradient, a
-    plain sum of dy, is not rounded: the kernels form it from float32 dy)."""
+    plain sum of dy, is not rounded: the kernels form it from float32 dy) and (pinned_forward=True) the TF32-pinned forward (the bias
+    is added unrounded, as the kernels' epilogue adds it)."""
     def op(a, b):
         return F.conv2d(a, b, None, stride, padding, dilation)
-    y = _Pinned.apply(x, w, op, pinned)
+    y = _Pinned.apply(x, w, op, pinned, pinned_forward)
     return y if bias is None else y + bias[:, None, None]
 
 
@@ -70,12 +72,14 @@ def conv_transpose2d(x, w, pinned=True):
 
 
 class PinnedConv2d(nn.Conv2d):
-    """nn.Conv2d (groups = 1) whose forward is conv2d(..., pinned=self.pinned); same parameters and state-dict keys."""
+    """nn.Conv2d (groups = 1) whose forward is conv2d(..., pinned=self.pinned, pinned_forward=self.pinned_forward); same parameters
+    and state-dict keys."""
 
     pinned = True
+    pinned_forward = False
 
     def forward(self, x):
-        return conv2d(x, self.weight, self.bias, self.stride, self.padding, self.dilation, self.pinned)
+        return conv2d(x, self.weight, self.bias, self.stride, self.padding, self.dilation, self.pinned, self.pinned_forward)
 
 
 class PinnedConvTranspose2d(nn.ConvTranspose2d):
